@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the DynaBOA per-frame hot path: adapted frames/sec on the synthetic 3DPW-shape stream.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c2|c3|c5]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c2|c3|c5] [--dump-outputs DIR]
 
 One "step" = one adapted frame at BASELINE.json configs[1] (C2: 1 inner step, batch 1; S-adapt scope of
 SURVEY.md §8d: adaptation + one output forward/SMPL).  Prints ONE JSON line (see DESIGN.md "Measurement").
@@ -33,7 +33,7 @@ WORKLOADS = {
     # BASELINE.json configs[4]: C3 + the dynamic re-adaptation loop at the reference's threshold (dynaboa_benchmark.py:48-49); the
     # trip count is data dependent; under torchrun the (a.b, |a|^2, |b|^2) sums are all-reduced so that every rank takes the same one
     # The reference threshold 3.1e-4 never fires on the seeded random weights of the synthetic stream (1 - cos of feature 12 after one
-    # outer step is 5e-6 .. 9e-5 there, profiles/r02_summary.md); 2e-5 sits inside that distribution, so the trip counts are mixed
+    # outer step is 5e-6 .. 9e-5 there); 2e-5 sits inside that distribution, so the trip counts are mixed
     # (0..8 per frame), which is what configs[4] asks to exercise.  --cos-threshold overrides.
     'c5': dict(inner_step=3, retrieval=1, lower_level_mixtrain=1, upper_level_mixtrain=1, dynamic_boa=1, sample_num=8,
                cos_sim_threshold=2e-5, optim_steps=7),
@@ -57,7 +57,7 @@ def default_options(**over):
 
 
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (B200_PROFILING.md) through NVML, every 20 ms from a
+    """SM clock and throttle reasons sampled DURING the timed region through NVML, every 20 ms from a
     thread (the timed region is ~0.15 s: `nvidia-smi -lms` starts too slowly to see it)."""
     REASONS = (('hw_slowdown', 0x8), ('sw_thermal_slowdown', 0x20), ('hw_thermal_slowdown', 0x40), ('sw_power_cap', 0x4))
 
@@ -116,7 +116,7 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
-    return 6650.0, 'fallback (B200_PROFILING.md)'
+    return 3350.0, 'H100 SXM data sheet (HBM3)'
 
 
 # ------------------------------------------------------------------------------------------------ CPU oracle arm
@@ -178,7 +178,7 @@ def time_oracle(workload, steps, warmup):
 
 def time_reference_code(workload, steps, warmup):
     """The reference's OWN CPU implementation (oracle/ref_harness.py: model/hmr.py, base_adaptor.py, dynaboa_benchmark.Adaptor from
-    /root/reference or its copy baseline/_ref, unmodified; smplx / learn2learn restated, synthetic stream), S-adapt scope:
+    DBOA_REFERENCE_ROOT, unmodified; smplx / learn2learn restated, synthetic stream), S-adapt scope:
     ``Adaptor.adaptation`` evaluates the model after every inner step and after the outer step (two ``inference`` calls per frame
     in C2), the GPU arm runs ONE output forward per frame -- the time of all but the last ``inference`` call of a frame is
     measured by a wrapper and subtracted.  Returns (frames/s, seconds, description) or None when the reference tree is absent."""
@@ -218,19 +218,7 @@ def time_reference_code(workload, steps, warmup):
             if t >= warmup:
                 times.append(dt)
     shutil.rmtree(work, ignore_errors=True)
-    root = 'baseline/_ref' if 'baseline' in ref_harness.REF else ref_harness.REF
-    return 1.0 / float(np.median(times)), float(np.sum(times)), f'unmodified reference code from {root} (oracle/ref_harness.py)'
-
-
-def forward_traffic_mb():
-    """DRAM bytes of one dboa_hmr_forward (b=1) from the committed ncu capture; None when the capture is absent."""
-    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'profiles', 'r02_forward_traffic.json')
-    try:
-        with open(path) as f:
-            d = json.load(f)
-        return (d['dram_bytes_read'] + d['dram_bytes_write']) / 1e6
-    except (OSError, KeyError, ValueError):
-        return None
+    return 1.0 / float(np.median(times)), float(np.sum(times)), f'unmodified reference code from {ref_harness.REF} (oracle/ref_harness.py)'
 
 
 def cpu_model():
@@ -266,6 +254,16 @@ def run_reference(args, rank, world):
 
 
 # ------------------------------------------------------------------------------------------------ GPU arm
+def dump_outputs(out_dir, pred):
+    """The prediction of the last timed frame (what ``Adaptor.predict`` hands a caller: rotmat, betas, cam, joints, vertices),
+    one float32 .npy per array (< 0.2 MB in all).  The stream and the weights are seeded, so two builds run with the same
+    arguments can be compared array by array."""
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in pred.items():
+        if torch.is_tensor(v):
+            np.save(os.path.join(out_dir, f'{k}.npy'), v.detach().float().cpu().numpy())
+
+
 def run_ours(args, rank, world, local):
     from dynaboa_b200 import _lib, config, dist as ddist, hmr as hmr_mod, synthetic
     from dynaboa_b200.adaptor import Adaptor
@@ -354,7 +352,7 @@ def run_ours(args, rank, world, local):
             e0.record()
             marks = []
             for t in range(PRELUDE + args.warmup, n_frames):
-                step(t, from_host)
+                pred = step(t, from_host)
                 if args.frame_times:                     # diagnostic: one event per frame on the adaptation stream
                     marks.append(torch.cuda.Event(enable_timing=True))
                     marks[-1].record()
@@ -371,7 +369,7 @@ def run_ours(args, rank, world, local):
                              f' | drain {ms - ts[-1]:.2f}\n')
         launches = lib.dboa_launch_count() - l0
         clocks = sampler.stop() if sampler else None
-        return ddist.max_over_ranks(ms, dev), launches, clocks
+        return ddist.max_over_ranks(ms, dev), launches, clocks, pred
 
     # reset model state between the two measurements so both see the same trajectory
     snapshot = (ad.model.module.arena.clone(), ad.teacher.arena.clone())
@@ -381,10 +379,12 @@ def run_ours(args, rank, world, local):
         ad.optimizer.m.zero_(); ad.optimizer.v.zero_(); ad.optimizer.step_count = 0
 
     sys.stderr.write('[bench] setup done\n')
-    ms_dev, launches, clocks = timed(False)
+    ms_dev, launches, clocks, _ = timed(False)
     sys.stderr.write(f'[bench] device-resident: {ms_dev / args.steps:.2f} ms/frame\n')
     restore()
-    ms_e2e, _, clocks_e2e = timed(True)
+    ms_e2e, _, clocks_e2e, last = timed(True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     value = world * args.steps / (ms_dev / 1000.0)
     e2e = world * args.steps / (ms_e2e / 1000.0)
 
@@ -403,7 +403,7 @@ def run_ours(args, rank, world, local):
         reps, tot = 20, 0.0
         l0 = lib.dboa_launch_count()
         for _ in range(reps):
-            flush.zero_()                                            # evict L2 (126 MB) between timed iterations
+            flush.zero_()                                            # evict L2 (50 MB) between timed iterations
             a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record()
             hmr_mod.raw_forward(model.arena, model._buffers, x, None, tape)
@@ -413,10 +413,9 @@ def run_ours(args, rank, world, local):
         fwd_ms = tot / reps
         fwd_launches = (lib.dboa_launch_count() - l0) // reps
         achieved = FWD_MB(1) / 1e3 / (fwd_ms / 1e3)
-        roof = {'bound': 'hbm', 'kernel': f'dboa_hmr_forward b=1 ({fwd_launches} launches: fused plan -- stride-1 convs apply the GroupNorm of their operand on load)',
+        roof = {'bound': 'hbm', 'kernel': f'dboa_hmr_forward b=1 ({fwd_launches} launches: one convolution and one GroupNorm launch per layer)',
                 'achieved': achieved, 'peak': peak, 'peak_source': peak_src, 'unit': 'GB/s', 'frac': achieved / peak,
-                'traffic': forward_traffic_mb(), 'traffic_unit': 'MB per forward (dram__bytes_read.sum + dram__bytes_write.sum, ncu capture '
-                'profiles/r02_forward_traffic.json)', 'algorithmic_MB_per_launch': FWD_MB(1), 'ms_per_launch': fwd_ms,
+                'algorithmic_MB_per_launch': FWD_MB(1), 'ms_per_launch': fwd_ms,
                 'step_model': {'algorithmic_GB_per_frame': 3.63, 'achieved_GBps': 3.63 / (ms_dev / 1000.0 / args.steps),
                                'frac': 3.63 / (ms_dev / 1000.0 / args.steps) / peak}}
         if world == 1 and not args.no_cpu_baseline:
@@ -443,7 +442,7 @@ def run_ours(args, rank, world, local):
                            'one_minus_cos12_first_test': ([round(1.0 - v[0][12]['cos'], 7) for _, v in sorted(ad.feat_sims.items())][-args.steps:]
                                                           if WORKLOADS[args.workload]['dynamic_boa'] else None),
                            'l2': 'per-step working set (theta, fast weights, Adam m/v, teacher, gradient arena: 6 x 108 MB + '
-                                 'activations) exceeds the 126 MB L2; the isolated forward timing flushes L2 with a 256 MB memset'},
+                                 'activations) exceeds the 50 MB L2; the isolated forward timing flushes L2 with a 256 MB memset'},
                 'e2e': {'value': e2e, 'unit': 'frames/s', 'h2d_bytes_per_step': h2d, 'd2h_bytes_per_step': d2h,
                         'ms_per_step': ms_e2e / args.steps},
                 'gpu_launches': int(launches), 'clocks': clocks, 'roofline': roof, 'cpu_baseline': cpu_base}
@@ -465,8 +464,12 @@ def main():
     ap.add_argument('--no-clock-sampler', action='store_true', help='diagnostic: no NVML polling during the timed region')
     ap.add_argument('--serial-output', action='store_true',
                     help='run the output forward on the adaptation stream (no overlap with the next frame)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed frame to DIR/<name>.npy (float32)')
     ap.add_argument('--tc', type=int, default=-1, help='tensor-core conv mode override (0 fp32 CUDA cores, 1 forward, 2 forward+dgrad+wgrad, 3 forward+dgrad)')
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == 'reference':
+        ap.error('--dump-outputs writes the outputs of the GPU path; it does not apply to --impl reference')
     if args.warmup < 3 and args.impl == 'ours':
         args.warmup = 3
     from dynaboa_b200 import dist as ddist

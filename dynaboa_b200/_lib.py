@@ -47,15 +47,10 @@ SIGNATURES = {
     'dboa_set_fused_forward': (I, [I]),
     'dboa_get_fused_forward': (I, []),
     'dboa_set_fused_backward': (I, [I]),
-    'dboa_set_forward_cta_budget': (I, [I]),
-    'dboa_set_operand_tmem': (I, [I]),
-    'dboa_get_operand_tmem': (I, []),
-    'dboa_set_chain_flags': (I, [I]),
-    'dboa_get_chain_flags': (I, []),
-    'dboa_selftest_map_cache': (I, [I, I, I]),
     'dboa_dgrad_fused': (I, [C.POINTER(DgradFusedStruct), I, I, I, I, I, P]),
     'dboa_conv_fused_part_floats': (L, [I, I, I]),
     'dboa_conv_fused_fwd': (I, [C.POINTER(FusedConvStruct), I, I, P]),
+    'dboa_conv2d_wgrad_tma': (I, [P, P, P, I, I, I, I, I, I, I, I, I, P]),
     'dboa_hmr_num_params': (I, []),
     'dboa_hmr_arena_floats': (L, []),
     'dboa_hmr_param_info': (I, [I, C.c_char_p, I, C.POINTER(L), C.POINTER(I), C.POINTER(L), C.POINTER(L)]),
@@ -71,7 +66,6 @@ SIGNATURES = {
     'dboa_conv2d_tc_fwd': (I, [P, P, P, I, I, I, I, I, I, I, I, I, P]),
     'dboa_conv2d_tc_dgrad': (I, [P, P, P, I, I, I, I, I, I, I, I, I, I, P]),
     'dboa_conv2d_tc_wgrad': (I, [P, P, P, I, I, I, I, I, I, I, I, I, P]),
-    'dboa_conv2d_wgrad_tma': (I, [P, P, P, I, I, I, I, I, I, I, I, I, P]),
     'dboa_gn_partial_floats': (L, [I, I, I]),
     'dboa_gn_bwd_partial_floats': (L, [I, I, I]),
     'dboa_groupnorm_fwd': (I, [P, P, P, P, P, P, P, I, I, I, I, P]),
@@ -121,7 +115,7 @@ def load():
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
-            raise RuntimeError(f'{LIB_PATH} is missing: run `python -m dynaboa_b200.build` (nvcc, sm_100a). '
+            raise RuntimeError(f'{LIB_PATH} is missing: run `python -m dynaboa_b200.build` (nvcc, sm_90a). '
                                'dynaboa_b200 has no CPU or PyTorch fallback.')
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():

@@ -54,7 +54,7 @@ class BaseAdaptor:
         else:
             self.summary_writer = _NullWriter()
         if not torch.cuda.is_available():
-            raise RuntimeError('dynaboa_b200 needs a CUDA device (sm_100a); there is no CPU path')
+            raise RuntimeError('dynaboa_b200 needs a CUDA device (sm_90a); there is no CPU path')
         self.device = torch.device('cuda', torch.cuda.current_device())
         _lib.load()
         self.seed_everything(options.seed)

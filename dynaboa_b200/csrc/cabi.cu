@@ -19,8 +19,6 @@ void hmr_arm_bucket_events(cudaEvent_t e0, cudaEvent_t e1, cudaEvent_t e2);
 long long hmr_bucket_offset(int k);
 void hmr_set_fused_forward(bool on);
 void hmr_set_fused_backward(bool on);
-void hmr_set_chain_flags(bool on);
-bool hmr_chain_flags();
 bool hmr_fused_forward();
 int hmr_num_params();
 long long hmr_arena_floats();
@@ -68,7 +66,7 @@ static bool cabi_pdl() {
 
 extern "C" {
 
-const char* dboa_version(void) { return "dynaboa_b200 0.1 (sm_100a)"; }
+const char* dboa_version(void) { return "dynaboa_b200 0.1 (sm_90a)"; }
 int dboa_last_cuda_error(void) { return g_last_cuda_error; }
 long long dboa_launch_count(void) { return g_launch_count; }
 int dboa_set_tensor_core_conv(int enable) { conv_tc_set_mode(enable); return DBOA_OK; }
@@ -76,12 +74,6 @@ int dboa_set_tensor_core_conv(int enable) { conv_tc_set_mode(enable); return DBO
 int dboa_set_fused_forward(int enable) { hmr_set_fused_forward(enable != 0); return DBOA_OK; }
 int dboa_get_fused_forward(void) { return hmr_fused_forward() ? 1 : 0; }
 int dboa_set_fused_backward(int enable) { hmr_set_fused_backward(enable != 0); return DBOA_OK; }
-int dboa_set_forward_cta_budget(int n) { conv_wide_set_cta_budget(n < 0 ? 0 : n); return DBOA_OK; }
-int dboa_set_operand_tmem(int enable) { conv_wide_set_operand_tmem(enable != 0); return DBOA_OK; }
-int dboa_selftest_map_cache(int bound, int n, int window) { return map_cache_selftest(bound, n, window); }
-int dboa_set_chain_flags(int enable) { hmr_set_chain_flags(enable != 0); return DBOA_OK; }
-int dboa_get_chain_flags(void) { return hmr_chain_flags() ? 1 : 0; }
-int dboa_get_operand_tmem(void) { return conv_wide_operand_tmem() ? 1 : 0; }
 
 int dboa_hmr_num_params(void) { return hmr_num_params(); }
 long long dboa_hmr_arena_floats(void) { return hmr_arena_floats(); }
@@ -146,7 +138,7 @@ int dboa_conv2d_tc_wgrad(const float* dy, const float* x, float* dw, int B, int 
 int dboa_conv2d_wgrad_tma(const float* dy, const float* x, float* dw, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad,
                           int Kpitch, dboa_stream_t stream) {
     if (!dy || !x || !dw) return DBOA_ERR_ARG;
-    return conv_wgrad_wide(dy, x, dw, make_dims(B, Hi, Wi, Cin, Cout, k, stride, pad, Kpitch), ST(stream), false);
+    return conv_wgrad_tc(dy, x, dw, make_dims(B, Hi, Wi, Cin, Cout, k, stride, pad, Kpitch), ST(stream));
 }
 int dboa_dgrad_fused(const dboa_dgrad_args* f, int B, int H, int Cin, int Cout, int k, dboa_stream_t stream) {
     if (!f || !f->dz || !f->y_c || !f->w || !f->stats_c || !f->sums_c || !f->gamma_c || !f->out) return DBOA_ERR_ARG;
@@ -159,7 +151,7 @@ int dboa_dgrad_fused(const dboa_dgrad_args* f, int B, int H, int Cin, int Cout, 
         d.prep[j].sums = f->prep_sums[j]; d.prep[j].dgb = f->prep_dgb[j];
         if (f->mask && j < f->nprep && (!d.prep[j].y || !d.prep[j].stats || !d.prep[j].gamma || !d.prep[j].sums || !d.prep[j].dgb)) return DBOA_ERR_ARG;
     }
-    return dgrad_wide(d, make_dims(B, H, H, Cin, Cout, k, 1, k / 2, k * k * Cin), ST(stream), cabi_pdl());
+    return dgrad_fused(d, make_dims(B, H, H, Cin, Cout, k, 1, k / 2, k * k * Cin), ST(stream), cabi_pdl());
 }
 long long dboa_conv_fused_part_floats(int B, int Ho, int Cout) { (void)Ho; (void)Cout; return (long long)B * 16; }
 int dboa_conv_fused_fwd(const dboa_fused_conv* probs, int nprob, int B, dboa_stream_t stream) {
@@ -178,10 +170,9 @@ int dboa_conv_fused_fwd(const dboa_fused_conv* probs, int nprob, int B, dboa_str
         f.y = c.y; f.part_out = c.part_out; f.mode = c.mode;
         f.Hi = c.Hi; f.Cin = c.Cin; f.Cout = c.Cout; f.k = c.k; f.stride = c.stride; f.pad = c.pad;
         f.Ho = (c.Hi + 2 * c.pad - c.k) / c.stride + 1;
-        if (!conv_wide_ok(f)) return DBOA_ERR_UNSUPPORTED;
+        if (!conv_fused_ok(f)) return DBOA_ERR_UNSUPPORTED;
     }
-    const int nz = conv_wide_plan(d, nprob, B);
-    return conv_wide_launch(d, nprob, B, nz, nullptr, 0, ST(stream), cabi_pdl());
+    return conv_fused_fwd(d, nprob, B, ST(stream), cabi_pdl());
 }
 long long dboa_gn_partial_floats(int B, int HW, int C) { return (long long)gn_partial_floats(B, HW, C); }
 long long dboa_gn_bwd_partial_floats(int B, int HW, int C) { return (long long)gn_bwd_partial_floats(B, HW, C); }

@@ -1,4 +1,4 @@
-// Shared device helpers and launch plumbing for libdynaboa_b200 (sm_100a only).
+// Shared device helpers and launch plumbing for libdynaboa_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -45,12 +45,22 @@ __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpre
 
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// SM count of the current device (queried once per process: one process drives one GPU)
+inline int num_sms() {
+    static const int n = [] {
+        int d = 0, v = 0;
+        cudaGetDevice(&d);
+        return cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, d) == cudaSuccess && v > 0 ? v : 132;
+    }();
+    return n;
+}
+
 // ---- programmatic dependent launch (PDL)
 // A kernel launched through launch_ex(..., pdl = true) may be scheduled while its predecessor in the stream is still
 // running; it must execute pdl_wait() before it touches anything the predecessor reads or writes (all global memory,
 // in practice: first statement), and calls pdl_trigger() right after so that ITS successor can be scheduled in turn.
 // At batch 1 every layer is a few-microsecond kernel and the launch + block-scheduling latency between dependent
-// kernels (~3 us measured in-situ, profiles/r02_trace.md) is a fifth of the step; PDL hides it.
+// kernels is a large part of the step; PDL hides it.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 

@@ -4,7 +4,7 @@
 // and their autograd backward (SURVEY.md §2.1 K1).  Activations are NHWC; weights are
 // [Cout][kh][kw][Cin] with a row pitch `Kpitch >= roundup16(kh*kw*Cin)` (zero padded).
 //
-// This is the exact-fp32 path: it is the numerical reference the tcgen05 TF32x3 path
+// This is the exact-fp32 path: it is the numerical reference the wgmma TF32x3 path
 // (conv_tc.cu) is checked against on the GPU, and it serves the shapes that path does not
 // take (Cin = 3 stem, odd tiles).  Split-K is deterministic: the K slices of a tile form a cluster
 // whose partial tiles are summed in a fixed order through distributed shared memory (cluster_reduce_store).
@@ -37,7 +37,7 @@ __device__ __forceinline__ void mma_slab(const float (*As)[BM + PADM], const flo
     }
 }
 
-// Split-K across a thread-block cluster (cluster dims (1,1,nz), nz <= 16): every K-slice parks its 64x64 partial
+// Split-K across a thread-block cluster (cluster dims (1,1,nz), nz <= 8): every K-slice parks its 64x64 partial
 // tile in its own shared memory, the cluster synchronises in hardware, and each CTA then sums a band of 64/nz rows over
 // all peers through distributed shared memory in the fixed order z = 0..nz-1 (deterministic) and writes that band.
 // No global partials, no atomics, no second launch.  `ncols` bounds the columns (weight gradient of the 7x7 stem).
@@ -155,7 +155,7 @@ __global__ void __launch_bounds__(NT) conv_fwd_kernel(const float* __restrict__ 
         bv = ldg4(wrow + k);                  // rows are zero padded up to Kpitch >= roundup16(K)
     };
     // register pipeline, PF slabs deep: at batch 1 the weight-streaming layers are bound by memory latency per CTA,
-    // so several slabs of loads stay in flight while one slab is multiplied (profiles/r01_summary.md)
+    // so several slabs of loads stay in flight while one slab is multiplied 
     float acc[4][4] = {};
     float av[PF][4];
     float4 bv[PF];
@@ -340,12 +340,11 @@ __global__ void __launch_bounds__(NT) conv_wgrad_kernel(const float* __restrict_
 // ---------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------
-static const int kTargetCtas = 296;      // 2 x 148 SMs
-
-// K-slices per tile: a power of two <= 16 (the non-portable cluster limit) that fills ~2 waves and leaves >= 4 iterations
+// K-slices per tile: a power of two <= 8 (the portable cluster size) that fills ~2 waves and leaves >= 4 iterations
 static int pick_split(int tiles, int kiters) {
+    const int target = 2 * num_sms();
     int ns = 1;
-    while (ns < 16 && tiles * ns * 2 <= kTargetCtas + tiles && kiters / (ns * 2) >= 4) ns *= 2;
+    while (ns < 8 && tiles * ns * 2 <= target + tiles && kiters / (ns * 2) >= 4) ns *= 2;
     return ns;
 }
 

@@ -5,8 +5,7 @@
 //
 // At batch 1 every layer is a few-microsecond problem: what sets the time is the number of DEPENDENT
 // steps (memory round trips, barriers) and the number of instructions each thread issues with few
-// warps to hide their latency -- not bytes (profiles/r01b_summary.md sections 3-4: the first version of these
-// kernels spent 8 / 16 us on tensors that stream in well under 1 us).  Hence:
+// warps to hide their latency -- not bytes.  Hence:
 //   * one (sample, group) is handled by ONE thread-block cluster of <= 16 CTAs x 1024 threads; every
 //     thread owns <= 4 float4 (same channels, rows a fixed stride apart: no integer division, the
 //     channels-per-group count is a power of two);

@@ -114,7 +114,6 @@ static const Net& net() {
 // activation tape
 // ---------------------------------------------------------------------------------------------
 struct ConvTape { long long y, part, stats, a; };   // a == -1: output lives in the block's conv3 slot
-constexpr int kChainFlags = 128;            // one 32-bit counter per fused forward launch (conv_wide.cu: chain_wait)
 struct Tape {
     long long x0, p0, p0_idx;
     long long acc;                  // fixed-point GroupNorm statistics of the fused plan: long long [conv][B][4][2]
@@ -147,7 +146,7 @@ static Tape build_tape(int B) {
             const ConvLayer& c = n.convs[ci];
             t.conv[ci].a = take((long long)B * c.hout * c.hout * c.cout);
         }
-    t.acc = take((long long)n.convs.size() * B * 16 + kChainFlags);      // + the chain-dependency counters of the fused launches (zeroed with it)
+    t.acc = take((long long)n.convs.size() * B * 16);
     t.xc = take(3LL * B * HEAD_LD);
     t.h1pre = take(3LL * B * HID); t.h1post = take(3LL * B * HID);
     t.h2pre = take(3LL * B * HID); t.h2post = take(3LL * B * HID);
@@ -201,7 +200,7 @@ struct Scratch {
 
 // Weight gradients run on two library-owned side streams (alternating): every wgrad only needs (dy of its layer, the saved input
 // activation) and writes its own slice of the gradient arena, so the chain  gn_bwd -> dgrad -> gn_bwd -> ...  on the
-// caller's stream never waits for them.  At batch 1 each kernel fills a fraction of the 148 SMs, and the two chains
+// caller's stream never waits for them.  At batch 1 each kernel fills a fraction of the SMs, and the two chains
 // overlap.  Buffers read by a pending wgrad are protected by per-buffer events; the side stream is joined before return.
 struct BwdAsync {
     static const int NSIDE = 2;
@@ -269,21 +268,14 @@ static const int g_wgrad_streams = [] { const char* e = getenv("DBOA_WGRAD_STREA
 
 static ConvDims dims_of(const ConvLayer& c, int B);
 
-// Fused data-gradient chain (dgrad_wide.cu): GroupNorm backward on operand load, ReLU mask / residual addend / the sums of the
-// next GroupNorm backward in the epilogue -- 96 launches fewer per frame.  Default ON since the kernel went on its instruction
-// diet (32-bit shared addressing, folded coefficient tables, plain per-warp partials instead of shared CAS loops): C2, 1 x B200,
-// 178.4 frames/s against 169.9 for the round-1 chain (gn_bwd_fused -> conv dgrad -> relu_mask), profiles/r02_summary.md.
-// DBOA_FUSED_BWD=0 (or dboa_set_fused_backward(0)) selects the round-1 chain (kept as the A/B reference; same tape, same results
-// to rounding).
-static bool g_fused_bwd = [] { const char* e = getenv("DBOA_FUSED_BWD"); return !(e && e[0] == '0'); }();
+// Fused plan (conv_tc.cu with an operand transform): every convolution applies the GroupNorm (+ residual, ReLU) of its operand on
+// load and leaves the statistics of its output as fixed-point sums; the fused data gradient applies GroupNorm backward on load
+// and produces the sums of the next GroupNorm backward in its epilogue.  Both plans fill the same tape.  The default is one
+// convolution and one GroupNorm launch per layer: on an H100 SXM (700 W) the fused plan measured 65.7 adapted frames/s for C2
+// against 129.0, since the per-element transform in the loader costs more than the launches it saves.  DBOA_FUSED_FWD=1 / DBOA_FUSED_BWD=1 (or dboa_set_fused_forward(1) / dboa_set_fused_backward(1)) select it.
+static bool g_fused_bwd = [] { const char* e = getenv("DBOA_FUSED_BWD"); return e && e[0] == '1'; }();
 void hmr_set_fused_backward(bool on) { g_fused_bwd = on; }
-// DBOA_FUSED_FWD=0 in the environment (or dboa_set_fused_forward(0)) selects the round-1 forward: one convolution launch and
-// one GroupNorm launch per layer (kept as the A/B reference of the fused path; both fill the same tape)
-// DBOA_CHAIN_FLAGS=1 (or dboa_set_chain_flags(1)): the fused forward launches wait for each other through counters instead of grid completion
-static bool g_chain_flags = [] { const char* e = getenv("DBOA_CHAIN_FLAGS"); return e && e[0] == '1'; }();
-void hmr_set_chain_flags(bool on) { g_chain_flags = on; }
-bool hmr_chain_flags() { return g_chain_flags; }
-static bool g_fused_fwd = [] { const char* e = getenv("DBOA_FUSED_FWD"); return !(e && e[0] == '0'); }();
+static bool g_fused_fwd = [] { const char* e = getenv("DBOA_FUSED_FWD"); return e && e[0] == '1'; }();
 void hmr_set_fused_forward(bool on) { g_fused_fwd = on; }
 bool hmr_fused_forward() { return g_fused_fwd; }
 
@@ -308,7 +300,7 @@ static const GnItems& gn_items() {
     }();
     return gi;
 }
-// backward convolutions: tcgen05 implicit GEMM when enabled and the shape is taken, else the fp32 CUDA-core kernels
+// backward convolutions: wgmma implicit GEMM when enabled and the shape is taken, else the fp32 CUDA-core kernels
 static int conv_backward_data(const ConvLayer& c, int B, const float* dy, const float* w, float* dx, int accumulate, float* ws, cudaStream_t st);
 static int conv_backward_weight(const ConvLayer& c, int B, const float* dy, const float* x, float* dw, float* ws, cudaStream_t st);
 
@@ -319,7 +311,7 @@ static ConvDims dims_of(const ConvLayer& c, int B) {
     return d;
 }
 
-// conv forward: tcgen05 implicit GEMM when enabled and the shape is taken (Cin % 32 == 0), else the fp32 CUDA-core kernel
+// conv forward: wgmma implicit GEMM when enabled and the shape is taken (Cin % 64 == 0, Cout % 64 == 0), else the fp32 CUDA-core kernel
 static int conv_forward(const ConvLayer& c, int B, const float* x, const float* w, float* y, float* ws, cudaStream_t st) {
     if (conv_tc_enabled()) {
         int s = conv_tc_fwd(x, w, y, dims_of(c, B), st);
@@ -335,13 +327,7 @@ static int conv_backward_data(const ConvLayer& c, int B, const float* dy, const 
     }
     return conv_dgrad(dy, w, dx, dims_of(c, B), accumulate, ws, (size_t)kConvWs, st);
 }
-// DBOA_WGRAD_TMA=0 keeps every weight gradient on the CUDA-core kernel (A/B reference)
-static const bool g_wgrad_tma = [] { const char* e = getenv("DBOA_WGRAD_TMA"); return !(e && e[0] == '0'); }();
 static int conv_backward_weight(const ConvLayer& c, int B, const float* dy, const float* x, float* dw, float* ws, cudaStream_t st) {
-    if (g_wgrad_tma && conv_tc_enabled()) {                 // tcgen05, MN-major operands through TMA (stride 1, Cout >= 128)
-        int s = conv_wgrad_wide(dy, x, dw, dims_of(c, B), st, false);
-        if (s != DBOA_ERR_UNSUPPORTED) return s;
-    }
     if (conv_tc_wgrad_enabled()) {
         int s = conv_tc_wgrad(dy, x, dw, dims_of(c, B), st);
         if (s != DBOA_ERR_UNSUPPORTED) return s;
@@ -433,16 +419,15 @@ int hmr_forward(const float* P, const float* init_pose, const float* init_shape,
                             c.cout, relu, st);
     };
     if (g_fused_fwd && conv_tc_enabled())
-        cudaMemsetAsync(T + t.acc, 0, (n.convs.size() * (size_t)B * 16 + kChainFlags) * sizeof(float), st);      // statistics accumulators and chain counters of this forward
+        cudaMemsetAsync(T + t.acc, 0, n.convs.size() * (size_t)B * 16 * sizeof(float), st);      // statistics accumulators of this forward
     DBOA_TRY(nchw_to_nhwc(image, T + t.x0, B, 3, 224, 224, st));
     DBOA_TRY(conv_forward(n.convs[0], B, T + t.x0, P + n.convs[0].w_off, T + t.conv[0].y, sc.ws, st));
     DBOA_TRY(gn_plain(0, T + t.conv[0].a, 1, nullptr));
     DBOA_TRY(maxpool3x3s2_fwd(T + t.conv[0].a, T + t.p0, reinterpret_cast<unsigned char*>(T + t.p0_idx), B, 112, 112, 64, st));
     const float* x = T + t.p0;
     if (g_fused_fwd && conv_tc_enabled()) {
-        // ---- fused plan (conv_wide.cu): every convolution applies the GroupNorm (+ residual, ReLU) of its operand on load and
-        // leaves the statistics of its output as fixed-point sums; 3 launches per bottleneck (conv1 and the shortcut
-        // convolution of a block share one launch).
+        // ---- fused plan (conv_tc.cu operand transform): every convolution applies the GroupNorm (+ residual, ReLU) of its operand on
+        // load and leaves the statistics of its output as fixed-point sums; one launch per convolution.
         auto acc_of = [&](int ci) { return T + t.acc + (long long)ci * B * 16; };
         auto base_desc = [&](int ci) {
             const ConvLayer& c = n.convs[ci];
@@ -458,23 +443,7 @@ int hmr_forward(const float* P, const float* init_pose, const float* init_shape,
             f.gamma = P + c.g_off; f.beta = P + c.b_off;
             f.a_out = T + t.conv[src].a; f.stats_out = T + t.conv[src].stats;
         };
-        // consecutive fused launches depend on each other through per-launch counters in the tape instead of grid completion
-        unsigned* flags = reinterpret_cast<unsigned*>(T + t.acc + (long long)n.convs.size() * B * 16);
-        int n_run = 0;
-        unsigned prev_ctas = 0;
-        auto run = [&](FusedConv* d, int np, int next_ci) {
-            const int nz = conv_wide_plan(d, np, B);
-            const ConvLayer* nx = next_ci >= 0 ? &n.convs[next_ci] : nullptr;
-            ChainDep dep = {nullptr, 0u, nullptr, nullptr};
-            const bool chained = g_chain_flags && pdl_enabled() && n_run < kChainFlags;
-            if (chained) {
-                if (n_run > 0) { dep.wait_flag = flags + n_run - 1; dep.wait_count = prev_ctas; }
-                dep.signal_flag = flags + n_run; dep.signal_count = &prev_ctas;
-            }
-            ++n_run;
-            return conv_wide_launch(d, np, B, nz, nx ? P + nx->w_off : nullptr, nx ? (size_t)nx->cout * nx->kpitch * sizeof(float) : 0, st, true,
-                                    chained ? &dep : nullptr);
-        };
+        auto run = [&](FusedConv* d, int np) { return conv_fused_fwd(d, np, B, st, true); };
         for (size_t bi = 0; bi < n.blocks.size(); ++bi) {
             const Block& b = n.blocks[bi];
             // ---- conv1 (+ the shortcut convolution in the same launch: both read the previous block's output, formed on load)
@@ -496,11 +465,11 @@ int hmr_forward(const float* P, const float* init_pose, const float* init_shape,
                 }
                 if (i == 1) { f.a_out = nullptr; f.stats_out = nullptr; f.stats2_out = nullptr; }     // conv1 is the writer
             }
-            DBOA_TRY(run(d, np, b.c2));
+            DBOA_TRY(run(d, np));
             d[0] = base_desc(b.c2); gn_of(d[0], b.c1);
-            DBOA_TRY(run(d, 1, b.c3));
+            DBOA_TRY(run(d, 1));
             d[0] = base_desc(b.c3); gn_of(d[0], b.c2);
-            DBOA_TRY(run(d, 1, bi + 1 < n.blocks.size() ? n.blocks[bi + 1].c1 : -1));
+            DBOA_TRY(run(d, 1));
         }
         const Block& lb = n.blocks.back();
         const ConvLayer& l3 = n.convs[lb.c3];
@@ -656,7 +625,7 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
     };
     const bool fused = g_fused_bwd && conv_tc_bwd_enabled();
     if (fused) {
-        // ---- fused chain (dgrad_wide.cu): per stride-1 layer ONE launch does GroupNorm backward (on load), the data gradient, the
+        // ---- fused chain (conv_tc.cu, GroupNorm backward on load): per stride-1 layer ONE launch does GroupNorm backward (on load), the data gradient, the
         // shortcut add, the ReLU mask of the producing layer and the sums of ITS GroupNorm backward; the stride-2 layers (conv2
         // and shortcut of layer2.0 / 3.0 / 4.0) keep the unfused kernels, stitched in with gn_bwd_prep.
         auto sums_of = [&](int ci) { return sc.bsums + (long long)ci * B * 16; };
@@ -675,7 +644,7 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
             f.dy_out = dy_out; f.addend = addend; f.out = out; f.mask = mask; f.nprep = mask ? np : 0;
             if (mask && np >= 1) f.prep[0] = prep_of(p0);
             if (mask && np >= 2) f.prep[1] = prep_of(p1);
-            return dgrad_wide(f, dims_of(c, B), st, true);
+            return dgrad_fused(f, dims_of(c, B), st, true);
         };
         cudaMemsetAsync(sc.bsums, 0, (size_t)sc.bacc_floats * sizeof(float), st);
         if (B > 1) cudaMemsetAsync(sc.gnp, 0, (size_t)sc.gnp_floats * sizeof(float), st);       // rows of the layers that stay fused are never written

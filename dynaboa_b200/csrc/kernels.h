@@ -15,7 +15,7 @@ int conv_fwd(const float* x, const float* w, float* y, const ConvDims& d, float*
 int conv_dgrad(const float* dy, const float* w, float* dx, const ConvDims& d, int accumulate, float* ws, size_t ws_floats, cudaStream_t st);
 int conv_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, float* ws, size_t ws_floats, cudaStream_t st);
 
-// ---- conv_tc.cu (tcgen05 TF32x3 GEMM for 1x1 / stride-1 convolutions); returns DBOA_ERR_UNSUPPORTED when the shape is not taken
+// ---- conv_tc.cu (wgmma TF32x3 implicit GEMM); returns DBOA_ERR_UNSUPPORTED when the shape is not taken
 // `pdl`: launch with programmatic stream serialization.  The forward / data-gradient kernels prefetch WEIGHT tiles before
 // their dependency wait, which is only safe when the preceding kernel in the stream does not write the weights (true inside
 // the network plan; the stand-alone C-ABI wrappers pass false).
@@ -29,48 +29,24 @@ bool conv_tc_enabled();
 void conv_tc_set_enabled(bool on);
 void conv_tc_set_mode(int mode);                      // 0 off, 1 forward, 2 forward + dgrad + wgrad, 3 forward + dgrad
 
-// ---- description of one fused convolution (conv_wide.cu)
+int conv_wgrad_tc(const float* dy, const float* x, float* dw, const ConvDims& d, cudaStream_t st);   // any mode; dw +=
+
+// ---- fused convolutions (conv_tc.cu, same kernel with an operand transform on load and sums in the epilogue)
 struct FusedConv {
     const float *x, *res, *w;                 // operand source (see `mode`), second source (modes 2, 3), weights [Cout][k*k*Cin]
     float *a_out, *stats_out, *stats2_out;    // optional tape stores: transformed operand, (mean, rstd) [B][4][2] of the operand's GroupNorm(s)
-    const float *part_in, *part2_in;          // statistics accumulators of x / res left by their producers
+    const float *part_in, *part2_in;          // fixed-point (sum, sum of squares) long long [B][4][2] of x / res left by their producers
     const float *gamma, *beta, *gamma2, *beta2;
-    float *y, *part_out;                      // raw output [B][Ho][Ho][Cout] and its statistics accumulators
+    float *y, *part_out;                      // raw output [B][Ho][Ho][Cout] and its statistics accumulators (ZEROED by the caller)
     int mode;                                 // 0: x as is; 1: relu(gn(x)); 2: relu(gn(x) + res); 3: relu(gn(x) + gn2(res))
-    int S_in, S2_in;                          // unused
     int Hi, Cin, Cout, k, stride, pad, Ho;    // square images
 };
-// ---- conv_wide.cu (fused convolution: both operands through TMA, 16 transform warps, fixed-point statistics)
-// part_in / part_out point to the fixed-point accumulators (long long [B][4][2], ZEROED by the caller
-// before the producing launch); S_in / S2_in are unused.  Stride-1 convolutions only.
-bool conv_wide_ok(const FusedConv& d);
-int conv_wide_plan(const FusedConv* d, int nprob, int B);
-void conv_wide_set_cta_budget(int n);                                  // 0: all SMs
-int map_cache_selftest(int bound, int n, int window);                   // host-only check of the tensor-map cache's eviction rule
-void conv_wide_set_operand_tmem(bool on);                              // transformed activation operand of conv_wide / dgrad_wide in tensor memory
-bool conv_wide_operand_tmem();
-// chain dependency between consecutive fused launches of one forward (conv_wide.cu: chain_wait): the launch waits until
-// *wait_flag >= wait_count instead of for the completion of its predecessor grid (wait_flag NULL: ordinary dependency), every CTA
-// of it increments *signal_flag when its outputs are stored, and *signal_count receives the number of CTAs (the next wait_count)
-struct ChainDep {
-    const unsigned* wait_flag; unsigned wait_count;
-    unsigned* signal_flag; unsigned* signal_count;
-};
-int conv_wide_launch(const FusedConv* d, int nprob, int B, int nz, const float* next_w, size_t next_bytes, cudaStream_t st, bool pdl,
-                     const ChainDep* dep = nullptr);
+bool conv_fused_ok(const FusedConv& f);
+int conv_fused_fwd(const FusedConv* f, int nprob, int B, cudaStream_t st, bool pdl);
 int gn_acc_res_avgpool(const float* y, const float* res, const float* acc, const float* gamma, const float* beta, float* a_out, float* stats_out,
                        float* out, int B, int HW, int C, int ld, int ncopy, size_t copy_stride, cudaStream_t st);
-
-// ---- conv_wgrad_wide.cu (tcgen05 weight gradient, MN-major operands through TMA); dw is accumulated (+=)
-// 7x7 / stride-2 stem weight gradient: row-per-CTA partials + fixed-order reduction (stem_wgrad.cu); needs 64 * 147 floats of
-// workspace per partial (DBOA_ERR_UNSUPPORTED for any other shape or without workspace)
-bool stem_wgrad_ok(const ConvDims& d);
-int stem_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, float* ws, size_t ws_floats, cudaStream_t st);
-bool conv_wgrad_wide_ok(const ConvDims& d);
-int conv_wgrad_wide(const float* dy, const float* x, float* dw, const ConvDims& d, cudaStream_t st, bool pdl);
-
-// ---- dgrad_wide.cu (fused data gradient: GroupNorm backward of the operand on load, ReLU mask + the next GroupNorm backward's
-// sums in the epilogue; see the file header).  All sums are 64-bit fixed point (long long, scale 2^28), zeroed by the caller.
+// fused data gradient: GroupNorm backward of the operand on load, ReLU mask + the next GroupNorm backward's sums in the epilogue.
+// All sums are 64-bit fixed point (long long, scale 2^28), zeroed by the caller.
 struct DgradPrep {
     const float* y;            // raw output of the layer whose GroupNorm backward is prepared [B][H][W][C]
     const float* stats;        // its (mean, rstd) [B][4][2]
@@ -88,11 +64,16 @@ struct DgradFused {
     DgradPrep prep[2];
     int nprep, accumulate;
 };
-bool dgrad_wide_ok(const ConvDims& d);
-int dgrad_wide(const DgradFused& f, const ConvDims& d, cudaStream_t st, bool pdl);
+bool dgrad_fused_ok(const ConvDims& d);
+int dgrad_fused(const DgradFused& f, const ConvDims& d, cudaStream_t st, bool pdl);
 int gn_bwd_prep(const float* dA, const float* mask, float* out, const DgradPrep& p, int B, int HW, int C, cudaStream_t st);
 struct GnFinishItem;
 int gn_dgb_finish(const GnFinishItem* items_dev, int n_items, const float* dgb, float* G, cudaStream_t st);
+
+// ---- stem_wgrad.cu: 7x7 / stride-2 stem weight gradient: row-per-CTA partials + fixed-order reduction (stem_wgrad.cu); needs 64 * 147 floats of
+// workspace per partial (DBOA_ERR_UNSUPPORTED for any other shape or without workspace)
+bool stem_wgrad_ok(const ConvDims& d);
+int stem_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, float* ws, size_t ws_floats, cudaStream_t st);
 
 // ---- groupnorm.cu (single-launch cluster kernels)
 size_t gn_partial_floats(int B, int HW, int C);     // forward scratch (none; kept for the C ABI)

@@ -14,7 +14,7 @@ namespace dboa {
 
 static inline int sweep_grid(size_t n4) {
     size_t blocks = (n4 + 255) / 256;
-    size_t cap = 148 * 16;
+    size_t cap = (size_t)num_sms() * 16;
     return (int)(blocks < cap ? (blocks ? blocks : 1) : cap);
 }
 

@@ -110,7 +110,7 @@ bool stem_wgrad_ok(const ConvDims& d) {
 int stem_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, float* ws, size_t ws_floats, cudaStream_t st) {
     if (!stem_wgrad_ok(d)) return DBOA_ERR_UNSUPPORTED;
     const int rows = d.B * stem::HO;
-    const int max_parts = (int)std::min<size_t>(296, ws_floats / (stem::CO * stem::KK));
+    const int max_parts = (int)std::min<size_t>(2 * num_sms(), ws_floats / (stem::CO * stem::KK));
     if (ws == nullptr || max_parts < 1) return DBOA_ERR_UNSUPPORTED;
     const int rows_per = ceil_div(rows, max_parts), nparts = ceil_div(rows, rows_per);
     DBOA_TRY(launch_ex(stem::stem_wgrad_kernel, dim3(nparts), dim3(stem::NT), (size_t)stem::SMEM_FLOATS * sizeof(float), st, dim3(1, 1, 1), true,

@@ -3,7 +3,7 @@ full replica of theta / Adam state / teacher and adapts on its own frame (or its
 exchange step is ONE all-reduce (mean) of the flat fp32 outer gradient (107.9 MB) per outer update, plus a
 3-float all-reduce so that every rank takes the same ``dynamic_boa`` branch.
 
-The reference has no distributed code; this is the B200-native addition.  Semantics: per-rank inner SGD step,
+The reference has no distributed code; this is the CUDA-native addition.  Semantics: per-rank inner SGD step,
 rank-averaged outer gradient -- NOT identical to the reference at ``--batch_size R`` (which takes one inner step
 on the batch-mean loss); ``mode='replicas'`` (no collective, R independent videos) is the exact-semantics mode.
 """
@@ -22,8 +22,8 @@ def init_from_env(backend=None):
         if backend is None:
             backend = 'nccl' if torch.cuda.is_available() else 'gloo'
         os.environ.setdefault('MASTER_ADDR', '127.0.0.1')
-        # the bucketed all-reduce runs UNDER the backward: 16 channels were the best trade between link bandwidth and the SMs NCCL
-        # takes from the backward kernels on 2 x B200 (290 frames/s; 2: 241, 4: 288/260, 8: 276/291; profiles/r02_summary.md)
+        # the bucketed all-reduce runs UNDER the backward: NCCL's channel count trades link bandwidth against the SMs it takes
+        # from the backward kernels
         os.environ.setdefault('NCCL_MAX_NCHANNELS', '16')
         dist.init_process_group(backend=backend, rank=rank, world_size=world)
     return rank, world, local

@@ -4,7 +4,7 @@ Drop-in for reference model/hmr.py: ``hmr(smpl_mean_params)`` (:314-323) returns
 ``state_dict`` names/shapes, ``parameters()`` order and ``forward`` signature/returns (:127-181) match the
 reference, so ``load_state_dict(ckpt['model'], strict=True)`` and the unchanged driver work.
 
-B200-first design: all 169 parameters are strided views of ONE flat fp32 arena (conv weights stored
+GPU-first design: all 169 parameters are strided views of ONE flat fp32 arena (conv weights stored
 [Cout][kh][kw][Cin] for K-major GEMM tiles, fc1 rows padded to 2208 for 16-byte row pitch), so the
 inner SGD step, Adam, the EMA teacher and the gradient all-reduce are single sweeps.  The forward and the
 hand-written backward are single C-ABI calls (``dboa_hmr_forward`` / ``dboa_hmr_backward``); torch autograd

@@ -1,7 +1,7 @@
-/* libdynaboa_b200 -- C ABI of the B200-native DynaBOA hot path.
+/* libdynaboa_b200 -- C ABI of the CUDA-native (H100, sm_90a) DynaBOA hot path.
  *
  * The reference (syguan96/DynaBOA) has no FFI/plugin boundary of its own: its hot path is Python
- * calling stock PyTorch ops (SURVEY.md §8b).  This header is the boundary the B200 implementation
+ * calling stock PyTorch ops (SURVEY.md §8b).  This header is the boundary the CUDA implementation
  * introduces underneath the reference's Python API; each entry point names the reference code it
  * replaces.  Conventions:
  *   - every pointer is a DEVICE pointer to fp32 data unless stated otherwise; buffers are owned by
@@ -30,36 +30,18 @@ typedef void* dboa_stream_t;
 const char* dboa_version(void);
 int dboa_last_cuda_error(void);            /* cudaError_t of the last failed launch */
 long long dboa_launch_count(void);         /* kernels launched by this library so far */
-/* which convolution products of the HMR plan run on the tcgen05 TF32x3 kernel -- 0: none (fp32 CUDA cores); 1: forward;
- * 2: forward + dgrad + wgrad; 3 (default): forward + dgrad, weight gradients on CUDA cores */
+/* which convolution products of the HMR plan run on the wgmma TF32x3 kernel -- 0: none (fp32 CUDA cores); 1: forward;
+ * 2: forward + dgrad + wgrad; 3 (default, faster on H100 at batch 1): forward + dgrad, weight gradients on CUDA cores */
 int dboa_set_tensor_core_conv(int mode);
 
-/* 1 (default): dboa_hmr_forward runs the fused plan -- every GroupNorm applied by the consuming convolution on load, its
- * statistics produced by the epilogue of the producing one (3 launches per bottleneck); 0: one convolution and one
- * GroupNorm launch per layer (round-1 plan, kept as the A/B reference).  Both fill the same tape. */
+/* 1: dboa_hmr_forward runs the fused plan -- every GroupNorm applied by the consuming convolution on load, its statistics
+ * produced by the epilogue of the producing one (one convolution launch per layer); 0 (default, faster on H100): one
+ * convolution and one GroupNorm launch per layer.  Both fill the same tape.  Environment: DBOA_FUSED_FWD. */
 int dboa_set_fused_forward(int enable);
 int dboa_get_fused_forward(void);
-/* the same switch for dboa_hmr_backward: 1 = fused data-gradient chain (csrc/dgrad_wide.cu: parity-green, fewer launches, but
- * measured slower end to end), 0 (default) = GroupNorm-backward and data-gradient launches per layer */
+/* the same switch for dboa_hmr_backward: 1 = fused data-gradient chain (GroupNorm backward on load), 0 (default) =
+ * GroupNorm-backward and data-gradient launches per layer.  Environment: DBOA_FUSED_BWD. */
 int dboa_set_fused_backward(int enable);
-/* CTAs (= SMs) the fused convolutions of the following dboa_hmr_forward calls may use; 0 = all.  Forwards issued side by side
- * on different streams share the device when each is given about half of it (a fused launch owns its SMs). */
-int dboa_set_forward_cta_budget(int n);
-/* 1: the fused convolution / data-gradient kernels keep the transformed activation operand (TF32 hi and lo parts) in tensor
- * memory and the tensor core reads only the weight operand from shared memory; 0: both operands in shared memory (the A/B
- * reference of the same kernels).  Same results to fp32 rounding of the same products (the split is identical).
- * Environment: DBOA_OPERAND_TMEM. */
-int dboa_set_operand_tmem(int enable);
-int dboa_get_operand_tmem(void);
-/* 1: consecutive fused convolution launches of dboa_hmr_forward depend on each other through per-launch counters in the tape
- * (every producer CTA signals after its last store, the consumer's readers spin with acquire loads) instead of waiting for the
- * producer grid to complete and flush.  Same results; needs programmatic dependent launch (DBOA_PDL).  Environment: DBOA_CHAIN_FLAGS. */
-int dboa_set_chain_flags(int enable);
-int dboa_get_chain_flags(void);
-/* Host-only self test (no CUDA call, runs without a GPU) of the TMA tensor-map cache: `n` insertions into a cache bounded at
- * `bound` entries while the caller, like a launch, holds the pointers of its last `window` (<= 16) lookups; evictions must leave
- * those pointers intact (they are freed one eviction later).  0 = ok, 1 + i = a held map was corrupted after insertion i. */
-int dboa_selftest_map_cache(int bound, int n, int window);
 
 /* ---- HMR regressor: parameter arena and tape layout ----------------------------------------
  * replaces: model/hmr.py:67-124 (HMR.__init__/_make_layer state_dict contract).
@@ -101,11 +83,11 @@ int dboa_conv2d_dgrad(const float* dy, const float* w, float* dx, int B, int Hi,
                       int Kpitch, int accumulate, float* ws, long long ws_floats, dboa_stream_t stream);
 int dboa_conv2d_wgrad(const float* dy, const float* x, float* dw, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad,
                       int Kpitch, float* ws, long long ws_floats, dboa_stream_t stream);
-/* 1x1 / stride-1 convolution as a tcgen05 TF32x3 GEMM: y[M][Cout] = x[M][Cin] * w[Cout][Cin]^T (fp32-accurate);
- * needs dboa_set_tensor_core_conv(1); returns DBOA_ERR_UNSUPPORTED for shapes it does not take (Cin % 32, Cout % 64) */
+/* 1x1 / stride-1 convolution as a wgmma TF32x3 GEMM: y[M][Cout] = x[M][Cin] * w[Cout][Cin]^T (fp32-accurate);
+ * needs dboa_set_tensor_core_conv(1); returns DBOA_ERR_UNSUPPORTED for shapes it does not take (Cin % 64, Cout % 64) */
 int dboa_conv1x1_tc_fwd(const float* x, const float* w, float* y, int M, int Cin, int Cout, float* ws, long long ws_floats,
                         dboa_stream_t stream);
-/* general convolution forward as a tcgen05 TF32x3 implicit GEMM (same arguments as dboa_conv2d_fwd; Cin % 64 == 0,
+/* general convolution forward as a wgmma TF32x3 implicit GEMM (same arguments as dboa_conv2d_fwd; Cin % 64 == 0,
  * Cout % 64 == 0, Kpitch == k*k*Cin).  The stand-alone tensor-core entry points are launched with ordinary stream
  * serialization (inside dboa_hmr_forward/backward the same kernels use programmatic dependent launch and prefetch
  * weight tiles before their dependency wait, which needs the plan's guarantee that the preceding kernel does not write
@@ -117,11 +99,11 @@ int dboa_conv2d_tc_dgrad(const float* dy, const float* w, float* dx, int B, int 
                          int Kpitch, int accumulate, dboa_stream_t stream);
 int dboa_conv2d_tc_wgrad(const float* dy, const float* x, float* dw, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad,
                          int Kpitch, dboa_stream_t stream);
-/* weight gradient on tcgen05 with MN-major operands fed by TMA (csrc/conv_wgrad_wide.cu): dw += dy^T * im2col(x); stride 1,
- * Cout % 128 == 0, Cin % 64 == 0, k in {1, 3}, pad k/2, square images of 56 / 28 / 14 / 7 (DBOA_ERR_UNSUPPORTED otherwise) */
+/* weight gradient on the wgmma tensor-core kernel whatever dboa_set_tensor_core_conv selects (csrc/conv_tc.cu): dw += dy^T *
+ * im2col(x); Cin % 64 == 0, Cout % 64 == 0, Kpitch == k*k*Cin (DBOA_ERR_UNSUPPORTED otherwise) */
 int dboa_conv2d_wgrad_tma(const float* dy, const float* x, float* dw, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad,
                           int Kpitch, dboa_stream_t stream);
-/* Fused tcgen05 convolution, the unit the forward plan is made of (csrc/conv_wide.cu).
+/* Fused convolution, the unit the forward plan is made of (csrc/conv_tc.cu: the operand transform runs in the loader).
  * replaces: nn.Conv2d + the nn.GroupNorm(4, C) / ReLU / residual add that PRECEDES it in Bottleneck.forward
  * (model/hmr.py:40-60), + the statistics pass of the GroupNorm that follows it.
  *   y = conv(T(x), w);  part_out[b][g] += (sum y, sum y^2) of group g of sample b, as 64-bit fixed point (scale 2^24):
@@ -129,8 +111,7 @@ int dboa_conv2d_wgrad_tma(const float* dy, const float* x, float* dw, int B, int
  *   mode 0: T(x) = x;  1: relu(gn(x));  2: relu(gn(x) + res);  3: relu(gn(x) + gn2(res))
  * gn statistics come from `part_in` (`part2_in`): the accumulators a previous call filled for x (res).
  * a_out / stats_out / stats2_out (optional): T(x) materialised, (mean, rstd) [B][4][2] of the GroupNorm(s).
- * Up to 2 problems of equal mode, operand and reduction length share one launch.
- * Cin % 64 == 0, Cout % 64 == 0, k in {1, 3}, stride 1, pad k/2, H <= 128 (DBOA_ERR_UNSUPPORTED otherwise). */
+ * Up to 2 problems per call (one launch each).  Cin % 64 == 0, Cout % 64 == 0, k in {1, 3}, stride 1 or 2 (DBOA_ERR_UNSUPPORTED otherwise). */
 typedef struct dboa_fused_conv {
     const float *x, *res, *w;
     float *a_out, *stats_out, *stats2_out;
@@ -142,7 +123,7 @@ typedef struct dboa_fused_conv {
 long long dboa_conv_fused_part_floats(int B, int Ho, int Cout);   /* size of part_out in floats (= B * 16) */
 int dboa_conv_fused_fwd(const dboa_fused_conv* probs, int nprob, int B, dboa_stream_t stream);
 
-/* Fused data gradient, the unit the backward plan is made of (csrc/dgrad_wide.cu).
+/* Fused data gradient, the unit the backward plan is made of (csrc/conv_tc.cu: GroupNorm backward in the loader).
  * replaces: the autograd backward of nn.GroupNorm (layer c) -> nn.Conv2d data gradient (layer c) -> residual add -> ReLU mask of
  * the producing layer p, + the reduction pass of GroupNorm_p's backward (model/hmr.py:40-60 under loss.backward()).
  *   dy  = rstd (dz gamma - m1 - x^ m2)                with (m1, m2) = sums_c / N, x^ = (y_c - mean) rstd     [dy_out: optional store]

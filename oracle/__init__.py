@@ -19,7 +19,7 @@ algorithm of the reference's per-frame hot path (SURVEY.md §8):
 Pinning status (see DESIGN.md "Oracle"):
 
 * geometry / prior / hmr restatements are checked bit-for-bit against the reference's own
-  modules imported from /root/reference by ``oracle/make_golden.py`` (run in the build
+  modules imported from the reference checkout by ``oracle/make_golden.py`` (run in the build
   container, where the reference is mounted), and the resulting vectors are committed under
   ``tests/golden/``.
 * the loss assembly and the adaptation orchestration are checked against the reference's own

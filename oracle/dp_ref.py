@@ -1,6 +1,6 @@
 """Oracle of the data-parallel mode (test infrastructure only; SURVEY.md §8e "CPU emulation of R ranks").
 
-The reference has no distributed code.  The B200 implementation shards independent frame streams over ranks: every rank
+The reference has no distributed code.  The CUDA implementation shards independent frame streams over ranks: every rank
 holds a replica of theta / Adam state / teacher, takes its OWN inner SGD step(s) on its own frame, and the outer gradient is
 the mean over ranks (one all-reduce); under ``dynamic_boa`` the (a.b, |a|^2, |b|^2) sums of every feature are summed over the
 ranks before the cosine is formed, which is the reference's batch-level decision (``cal_feature_diff`` flattens across the

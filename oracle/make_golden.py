@@ -1,4 +1,4 @@
-"""Golden-vector generator (run in the BUILD CONTAINER, where /root/reference is mounted).
+"""Golden-vector generator (run where a reference checkout is available; DBOA_REFERENCE_ROOT names it).
 
     python -m oracle.make_golden            # writes tests/golden/*.npz
 
@@ -14,7 +14,7 @@ What it does (test infrastructure only; nothing here ships or runs on the GPU bo
    restatements/stubs below, ``__init__``'s file loading is replaced by the synthetic assets --
    asserts ``oracle/adaptor_ref.py`` reproduces the trajectory, and stores it as fixtures.
 
-The reference is read from /root/reference at run time and never copied.
+The reference is read from that checkout at run time and never copied.
 """
 import importlib
 import importlib.util
@@ -29,7 +29,7 @@ import numpy as np
 import torch
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = '/root/reference'
+REF = os.environ.get('DBOA_REFERENCE_ROOT', '')
 OUT = os.path.join(REPO, 'tests', 'golden')
 sys.path.insert(0, REPO)
 
@@ -326,7 +326,7 @@ def golden_adapt(workdir, tag, n_frames, **over):
 def golden_dp(R=2, n_frames=3):
     """Data-parallel trajectory (oracle/dp_ref.py: R replicas in lock step, rank-mean outer gradient, rank-summed cosine
     terms): 1 inner step, deterministic teacher, dynamic loop armed with a low threshold so that it fires.  The reference has no
-    distributed mode; this fixture pins the B200 implementation's NCCL path to the CPU emulation of SURVEY.md section 8e."""
+    distributed mode; this fixture pins the CUDA implementation's NCCL path to the CPU emulation of SURVEY.md section 8e."""
     from oracle import dp_ref
     opts = adaptor_ref.default_options(inner_step=1, retrieval=0, lower_level_mixtrain=0, upper_level_mixtrain=0, dynamic_boa=1,
                                        cos_sim_threshold=1e-7, optim_steps=2, teacher_dropout=0)

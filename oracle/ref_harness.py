@@ -1,8 +1,7 @@
 """The reference's OWN adaptor code on CPU (test / benchmark infrastructure only; never imported by the product).
 
-``make_reference_adaptor`` builds ``dynaboa_benchmark.Adaptor`` from the reference tree -- ``/root/reference`` in the build
-container, the byte-for-byte copy ``baseline/_ref/`` (scripts/install_reference.py, git-ignored, travels with gpurun) on the GPU
-box -- with the constructor's I/O replaced: the two third-party packages that are not in this image (``smplx``,
+``make_reference_adaptor`` builds ``dynaboa_benchmark.Adaptor`` from the reference's own files (syguan96/DynaBOA: the checkout
+named by DBOA_REFERENCE_ROOT, or the copy ``build()`` stages in oracle/_ref/), with the constructor's I/O replaced: the two third-party packages that are not in this image (``smplx``,
 ``learn2learn``) are the restatements of this package, the datasets are the synthetic stream / exemplar bank, the device is the
 CPU.  Everything that runs per frame -- ``model/hmr.py``, ``base_adaptor.BaseAdaptor``'s losses and levels,
 ``dynaboa_benchmark.Adaptor.adaptation`` / ``inference``, ``utils/geometry.py``, ``utils/smplify/prior.py``,
@@ -25,11 +24,12 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def reference_root():
-    """/root/reference when present (build container), else the copy under baseline/_ref, else None
-    (DBOA_REFERENCE_ROOT overrides; ``none`` disables the reference tree: the callers fall back to the oracle port)."""
-    if os.environ.get('DBOA_REFERENCE_ROOT') == 'none':
+    """The reference checkout named by DBOA_REFERENCE_ROOT, else the copy ``build()`` staged in oracle/_ref/ (oracle/stage_reference.py),
+    else None; DBOA_REFERENCE_ROOT=none disables the reference tree (the callers fall back to the oracle port)."""
+    env = os.environ.get('DBOA_REFERENCE_ROOT')
+    if env == 'none':
         return None
-    for root in (os.environ.get('DBOA_REFERENCE_ROOT'), '/root/reference', os.path.join(REPO, 'baseline', '_ref')):
+    for root in (env, os.path.join(REPO, 'oracle', '_ref')):
         if root and os.path.exists(os.path.join(root, 'dynaboa_benchmark.py')) and os.path.exists(os.path.join(root, 'model', 'hmr.py')):
             return root
     return None

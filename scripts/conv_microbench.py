@@ -1,5 +1,5 @@
 """Per-layer timing of the three convolution products (forward, data gradient, weight gradient) of the HMR backbone at
-batch B, for the fp32 CUDA-core kernels and the tcgen05 TF32x3 kernel, through the C ABI.
+batch B, for the fp32 CUDA-core kernels and the wgmma TF32x3 kernel, through the C ABI.
 
 Each shape is launched `iters` times back to back on one stream (inputs stay in L2, as inside the running step);
 the figure is the mean time per launch in microseconds, launch gaps included.  The stand-alone tensor-core entry points are

@@ -4,7 +4,7 @@ ncu serialises kernels and flushes caches between replays, so its per-launch dur
 about the gaps between launches.  This script records the running step instead: for every kernel its start and
 duration on the device, from which it prints (a) per-kernel-name count / total / mean, (b) the busy time of the
 device versus the span of the frame (the rest is launch gaps / dependencies), (c) how much of the span has two or
-more kernels in flight (stream overlap).  Writes gpurun_out/trace_<tag>.json (summary) next to the table.
+more kernels in flight (stream overlap).  Writes traces/trace_<tag>.json (summary) next to the table.
 
     python scripts/trace_step.py --tag r02 [--region frame|forward|fwdbwd]
 """
@@ -107,7 +107,7 @@ print(f'region={args.region} kernels={len(evs)} copies={len(copies)} span={span:
 print(f'{"kernel":48s} {"n":>5s} {"total_us":>10s} {"mean_us":>9s} {"share":>7s}')
 for k, (n, t) in rows[:40]:
     print(f'{k[:48]:48s} {n:5d} {t:10.1f} {t / n:9.2f} {t / tot:7.1%}')
-os.makedirs(os.path.join(REPO, 'gpurun_out'), exist_ok=True)
-with open(os.path.join(REPO, 'gpurun_out', f'trace_{args.tag}_{args.region}.json'), 'w') as f:
+os.makedirs(os.path.join(REPO, 'traces'), exist_ok=True)
+with open(os.path.join(REPO, 'traces', f'trace_{args.tag}_{args.region}.json'), 'w') as f:
     json.dump({'region': args.region, 'kernels': len(evs), 'span_us': span, 'busy_us': busy, 'overlap_us': overlap,
                'by_kernel': [{'name': k, 'n': n, 'total_us': t, 'mean_us': t / n} for k, (n, t) in rows]}, f, indent=1)

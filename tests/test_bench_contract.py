@@ -1,5 +1,5 @@
 """bench.py's driver contract on a machine without a GPU: the reference arm (`--impl reference`: the reference's own code from
-/root/reference or baseline/_ref through oracle/ref_harness.py, else the CPU port of the path) prints ONE JSON line with the keys the driver reads, and our own arm fails loudly instead of falling back."""
+the checkout named by DBOA_REFERENCE_ROOT through oracle/ref_harness.py, else the CPU port of the path) prints ONE JSON line with the keys the driver reads, and our own arm fails loudly instead of falling back."""
 import json
 import os
 import subprocess

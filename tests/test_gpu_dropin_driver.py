@@ -1,5 +1,4 @@
-"""The UNCHANGED reference driver (`dynaboa_benchmark.py`, copied byte for byte into the git-ignored baseline/_ref/ by
-scripts/install_reference.py) executed on the GPU on top of the drop-in module tree, against the trajectory the
+"""The UNCHANGED reference driver (`dynaboa_benchmark.py`, staged byte for byte into the git-ignored oracle/_ref/ by build()) executed on the GPU on top of the drop-in module tree, against the trajectory the
 reference itself produced on CPU (tests/golden/adapt_c2.npz, recorded by oracle/make_golden.py from the same file).
 This is the north-star claim "dynaboa_benchmark.py drops in unchanged", run rather than AST-checked."""
 import os
@@ -11,14 +10,15 @@ import pytest
 import torch
 
 from conftest import rel_err
+from oracle import ref_harness
 
 pytestmark = pytest.mark.gpu
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DRIVER = os.path.join(REPO, 'baseline', '_ref', 'dynaboa_benchmark.py')
+DRIVER = os.path.join(ref_harness.REF or '', 'dynaboa_benchmark.py')
 SHADOWED = ('constants', 'config', 'model', 'utils', 'base_adaptor', 'boa_dataset', 'learn2learn')
 
 
-@pytest.mark.skipif(not os.path.exists(DRIVER), reason='baseline/_ref/dynaboa_benchmark.py absent: run scripts/install_reference.py in the build container')
+@pytest.mark.skipif(not os.path.exists(DRIVER), reason='reference files not staged (oracle/_ref/, built from a reference checkout)')
 def test_unchanged_reference_driver_follows_reference_trajectory(asset_dir, tmp_path, golden, monkeypatch):
     import joblib
     from dynaboa_b200 import hmr as hmr_mod

@@ -1,4 +1,4 @@
-"""Fused tcgen05 convolution (csrc/conv_wide.cu): both operands through TMA, GroupNorm of the operand applied on load,
+"""Fused convolution (csrc/conv_tc.cu with an operand transform): GroupNorm of the operand applied on load,
 GroupNorm statistics of the output as fixed-point sums from the epilogue.  Checked against torch (fp64 convolution,
 F.group_norm) on the device, one problem and two problems per launch, every transform mode, and end to end against the
 unfused plan."""
@@ -175,7 +175,7 @@ def test_block_output_on_load_two_problems(L, B, H, C, planes, stride, mode):
 
 
 def test_fused_forward_fills_the_same_tape_as_the_unfused_plan(L):
-    """Whole HMR forward: fused plan (3 launches per bottleneck) against the round-1 plan (conv + GroupNorm launches);
+    """Whole HMR forward: fused plan (one launch per convolution) against the unfused plan (conv + GroupNorm launches);
     outputs, all 15 features and the complete tape (y, statistics, activations: what the backward reads)."""
     from dynaboa_b200 import hmr as hmr_mod, synthetic
     from oracle import hmr_ref
@@ -186,6 +186,7 @@ def test_fused_forward_fills_the_same_tape_as_the_unfused_plan(L):
     for B in (1, 2, 9):
         x = torch.randn(B, 3, 224, 224, generator=torch.Generator().manual_seed(B)).cuda()
         outs = {}
+        prev = lib.dboa_get_fused_forward()
         for fused in (0, 1):
             lib.dboa_set_fused_forward(fused)
             try:
@@ -194,7 +195,7 @@ def test_fused_forward_fills_the_same_tape_as_the_unfused_plan(L):
                 torch.cuda.synchronize()
                 outs[fused] += (lib.dboa_launch_count() - n0,)
             finally:
-                lib.dboa_set_fused_forward(1)
+                lib.dboa_set_fused_forward(prev)
         (r0, s0, c0, p0, t0, n_un), (r1, s1, c1, p1, t1, n_fu) = outs[0], outs[1]
         print(f'B={B}: launches unfused {n_un} fused {n_fu}')
         assert n_fu <= n_un - 40
@@ -212,46 +213,6 @@ def test_fused_forward_fills_the_same_tape_as_the_unfused_plan(L):
         assert ((G1 - G0).norm() / G0.norm()).item() < 2e-3, B
 
 
-def test_operand_placement_and_chain_dependency_do_not_change_results(L):
-    """The two execution-model switches of the fused kernels change WHERE the transformed activation operand lives (tensor memory
-    instead of shared memory: dboa_set_operand_tmem) and HOW consecutive launches wait for each other (per-launch counters
-    instead of grid completion: dboa_set_chain_flags), not the arithmetic: identical TF32 splits, products and accumulation
-    order.  Forward outputs, all 15 features and the gradient of a whole backward are compared bit for bit."""
-    from dynaboa_b200 import hmr as hmr_mod, synthetic
-    from oracle import hmr_ref
-    m = hmr_mod.hmr(synthetic.make_mean_params()).cuda()
-    m.load_state_dict(hmr_ref.strip_prefix(synthetic.make_basemodel()['model']), strict=True)
-    m.eval()
-    lib = L.load()
-    tmem0, chain0 = lib.dboa_get_operand_tmem(), lib.dboa_get_chain_flags()
-    try:
-        for B in (1, 2, 9):
-            x = torch.randn(B, 3, 224, 224, generator=torch.Generator().manual_seed(40 + B)).cuda()
-            res = {}
-            for tmem, chain in ((0, 0), (1, 0), (1, 1), (0, 1)):
-                lib.dboa_set_operand_tmem(tmem)
-                lib.dboa_set_chain_flags(chain)
-                tape = torch.empty(hmr_mod.tape_floats(B), device='cuda')
-                for rep in range(3 if chain else 1):            # the counters live in the tape: a re-used tape must be re-armed
-                    r, s_, c, p, t = hmr_mod.raw_forward(m.arena, m._buffers, x, tape=tape)
-                G = torch.zeros_like(m.arena)
-                gen = torch.Generator(device='cuda').manual_seed(7)
-                dr, dsh, dc = (torch.randn(v.shape, device='cuda', generator=gen) for v in (r, s_, c))
-                hmr_mod.raw_backward(m.arena, t, B, False, dr, dsh, dc, G)
-                torch.cuda.synchronize()
-                res[(tmem, chain)] = (r.clone(), s_.clone(), c.clone(), [f.clone() for f in hmr_mod._feature_views(t, B)], G)
-            ref = res[(0, 0)]
-            for key, got in res.items():
-                assert torch.equal(got[0], ref[0]) and torch.equal(got[1], ref[1]) and torch.equal(got[2], ref[2]), (B, key)
-                for i in range(15):
-                    assert torch.equal(got[3][i], ref[3][i]), (B, key, i)
-                # the backward runs weight gradients on side streams next to the chain: same kernels, same operands
-                assert (got[4] - ref[4]).abs().max().item() <= 1e-6 * ref[4].abs().max().item(), (B, key)
-    finally:
-        lib.dboa_set_operand_tmem(tmem0)
-        lib.dboa_set_chain_flags(chain0)
-
-
 WGRAD = [  # B, H (input), Cin, Cout, k, stride
     (1, 56, 64, 256, 1, 1), (1, 28, 128, 128, 3, 1), (2, 28, 512, 128, 1, 1), (1, 14, 256, 256, 3, 1), (3, 14, 1024, 256, 1, 1), (1, 7, 512, 512, 3, 1),
     (2, 7, 512, 2048, 1, 1), (9, 7, 2048, 512, 1, 1), (1, 14, 256, 1024, 1, 1), (1, 56, 128, 128, 3, 2), (2, 28, 256, 256, 3, 2), (1, 14, 512, 512, 3, 2),
@@ -260,7 +221,7 @@ WGRAD = [  # B, H (input), Cin, Cout, k, stride
 
 @pytest.mark.parametrize('case', WGRAD)
 def test_weight_gradient_on_tensor_cores_mn_major(L, case):
-    """tcgen05 weight gradient with MN-major TMA operands (csrc/conv_wgrad_wide.cu) against the fp32 CUDA-core kernel and an fp64
+    """Tensor-core weight gradient (dboa_conv2d_wgrad_tma: the wgmma kernel of csrc/conv_tc.cu) against the fp32 CUDA-core kernel and an fp64
     reference; dw is accumulated."""
     B, H, Cin, Cout, k, st = case
     g = torch.Generator().manual_seed(sum(case) + 3)
@@ -308,8 +269,8 @@ def _expand(st, Cc):                                                         # (
 
 @pytest.mark.parametrize('case', DGRAD)
 def test_fused_data_gradient(L, case):
-    """csrc/dgrad_wide.cu against an fp64 torch restatement: GroupNorm_c backward on load, transposed convolution (MN-major weight
-    operand), shortcut addend, ReLU mask, and the fixed-point sums of the producing layer's GroupNorm backward(s)."""
+    """Fused data gradient (csrc/conv_tc.cu) against an fp64 torch restatement: GroupNorm_c backward on load, transposed convolution,
+    shortcut addend, ReLU mask, and the fixed-point sums of the producing layer's GroupNorm backward(s)."""
     B, H, Cin, Cout, k, nprep, with_add = case
     g = torch.Generator().manual_seed(sum(case[:5]) + 17)
     rn = lambda *s: torch.randn(*s, generator=g).cuda()
@@ -370,7 +331,7 @@ def test_fused_data_gradient(L, case):
 
 
 def test_fused_backward_chain_matches_the_unfused_chain(L):
-    """dboa_hmr_backward through the fused data-gradient chain (dgrad_wide.cu + gn_bwd_prep seams) against the default chain, same
+    """dboa_hmr_backward through the fused data-gradient chain (conv_tc.cu + gn_bwd_prep seams) against the default chain, same
     tape, B = 1, 2 and 9: the complete gradient arena."""
     from dynaboa_b200 import hmr as hmr_mod, synthetic
     from oracle import hmr_ref
@@ -391,7 +352,7 @@ def test_fused_backward_chain_matches_the_unfused_chain(L):
                 torch.cuda.synchronize()
                 G.append(g)
             finally:
-                lib.dboa_set_fused_backward(1)
+                lib.dboa_set_fused_backward(0)          # the library default
         assert ((G[1] - G[0]).norm() / G[0].norm()).item() < 1e-4, B
         lay = hmr_mod.layout()
         for name, a, b in zip(lay.names, lay.views(G[0]), lay.views(G[1])):

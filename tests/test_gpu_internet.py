@@ -1,4 +1,4 @@
-"""Second client of the hot path (N3): the UNCHANGED reference `dynaboa_internet.py` (baseline/_ref/, byte-for-byte copy) on the
+"""Second client of the hot path (N3): the UNCHANGED reference `dynaboa_internet.py` (staged byte for byte into the git-ignored oracle/_ref/ by build()) on the
 drop-in tree, fed by a small synthetic "Internet video" on disk (PNG frames + the reference's npz annotation layout) whose crops
 and keypoints go through the GPU input side (N2), against the CPU oracle run on the oracle-processed frames.  Also the
 library's own ``InternetAdaptor`` (autograd and fused paths)."""
@@ -12,10 +12,11 @@ import pytest
 import torch
 
 from conftest import rel_err
+from oracle import ref_harness
 
 pytestmark = pytest.mark.gpu
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DRIVER = os.path.join(REPO, 'baseline', '_ref', 'dynaboa_internet.py')
+DRIVER = os.path.join(ref_harness.REF or '', 'dynaboa_internet.py')
 SHADOWED = ('constants', 'config', 'model', 'utils', 'base_adaptor', 'boa_dataset', 'learn2learn')
 FLAGS = dict(inner_step=1, retrieval=0, lower_level_mixtrain=0, upper_level_mixtrain=0, dynamic_boa=0)
 N = 3
@@ -63,7 +64,7 @@ def oracle_trajectory(frames, centers, scales, parts, masks):
     return preds
 
 
-@pytest.mark.skipif(not os.path.exists(DRIVER), reason='baseline/_ref/dynaboa_internet.py absent: run scripts/install_reference.py in the build container')
+@pytest.mark.skipif(not os.path.exists(DRIVER), reason='reference files not staged (oracle/_ref/, built from a reference checkout)')
 def test_unchanged_internet_driver_on_gpu_input_side(asset_dir, tmp_path, monkeypatch):
     import joblib
     from dynaboa_b200 import config, hmr as hmr_mod

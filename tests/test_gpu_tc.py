@@ -1,4 +1,4 @@
-"""tcgen05 TF32x3 GEMM path (csrc/conv_tc.cu) validated on the device against the exact-fp32 CUDA-core conv
+"""wgmma TF32x3 GEMM path (csrc/conv_tc.cu) validated on the device against the exact-fp32 CUDA-core conv
 (csrc/conv.cu) and against the CPU oracle, then end to end through the HMR forward."""
 import pytest
 import torch
@@ -43,7 +43,7 @@ def test_descriptor_convention_and_accuracy(L):
             ref = (x.double() @ w.double().t())
             errs.append(((y.double() - ref).abs().max() / ref.abs().max()).item())
         results[mode] = max(errs)
-        print(f'tcgen05 mode {mode}: max rel err over shapes = {results[mode]:.3e}  per-shape {[f"{e:.1e}" for e in errs]}')
+        print(f'tensor-core mode {mode}: max rel err over shapes = {results[mode]:.3e}  per-shape {[f"{e:.1e}" for e in errs]}')
     assert results[1] < 5e-6, f'documented descriptor convention failed: {results}'
 
 
@@ -133,4 +133,4 @@ def test_hmr_forward_with_tensor_core_convs(L, golden):
                 gflat = params[key[5:]].grad.contiguous().flatten().double().cpu()
                 assert abs(gflat.norm().item() - gd[key][0]) <= 2e-3 * gd[key][0], key
     finally:
-        L.load().dboa_set_tensor_core_conv(3)
+        L.load().dboa_set_tensor_core_conv(3)             # the library default
