@@ -104,6 +104,8 @@ SIGNATURES = {
     'dboa_keypoint_transform': (I, [P, I, C.c_double, C.c_double, C.c_double, C.c_double, I, P, P]),
     'dboa_eval_scratch_floats': (L, [I, I]),
     'dboa_eval_metrics': (I, [P, P, P, P, I, I, P, I, P, P, I, P]),
+    'dboa_render_scratch_bytes': (L, [I, I, I, I, I]),
+    'dboa_render_overlay': (I, [P, P, P, P, I, I, C.POINTER(F), C.POINTER(F), C.POINTER(F), P, I, I, I, P, L, P, P, P]),
 }
 
 _ERRORS = {-1: 'DBOA_ERR_ARG', -2: 'DBOA_ERR_SHAPE', -3: 'DBOA_ERR_CUDA', -4: 'DBOA_ERR_UNSUPPORTED'}

@@ -133,7 +133,8 @@ class BaseAdaptor:
         if self.options.dataset == '3dpw':
             dataset, self.imgdir = PW3D(self.options), config.PW3D_ROOT
         else:
-            dataset, self.imgdir = Internet_dataset(self.options), osp.join(config.InternetData_ROOT, 'images')
+            dataset = Internet_dataset(self.options)
+            self.imgdir = getattr(dataset, 'imgdir', osp.join(config.InternetData_ROOT, 'images'))   # DYNABOA_INTERNET_ROOT applies
         self.dataloader = DataLoader(dataset, batch_size=self.options.batch_size, shuffle=False, num_workers=0)
 
     def set_criterion(self):
@@ -325,7 +326,24 @@ class BaseAdaptor:
         pass
 
     def save_results(self, vts, cam_trans, images, name, bbox, prefix=None):
-        raise NotImplementedError('mesh rendering (pyrender) is outside the hot path (SURVEY.md §2: render_demo.py OUT)')
+        """reference :429-443: draws each adapted mesh over its original frame (``imgdir/name[i]``) on the GPU and writes
+        ``exppath/image/{prefix}_{global_step + i}.png``, plus the mesh as ``demo.obj`` in the working directory.  Like the
+        reference, the mesh colour (205, 129, 98) / 255 is given in RGB order and drawn into the BGR frame cv2 reads, so
+        the PNGs match the reference's.  ``images`` is unused (the reference un-normalises it and discards the result)."""
+        import cv2
+        from .render import Renderer, convert_crop_cam_to_orig_img
+        cam = cam_trans.detach().cpu().numpy()
+        bbox = bbox.detach().cpu().numpy() if torch.is_tensor(bbox) else np.asarray(bbox)
+        for i in range(vts.shape[0]):
+            oriimg = cv2.imread(os.path.join(self.imgdir, name[i]))
+            if oriimg is None:
+                raise FileNotFoundError(os.path.join(self.imgdir, name[i]))
+            ori_h, ori_w = oriimg.shape[:2]
+            ori_pred_cams = convert_crop_cam_to_orig_img(cam, bbox, ori_w, ori_h)
+            frame = torch.from_numpy(oriimg).to(self.device)
+            renderer = Renderer(resolution=(ori_w, ori_h), orig_img=True, wireframe=False)
+            rendered = renderer.render(frame, vts[i], ori_pred_cams[i], color=np.array([205, 129, 98]) / 255, mesh_filename='demo.obj')
+            cv2.imwrite(osp.join(self.exppath, 'image', f'{prefix}_{self.global_step + i}.png'), rendered.cpu().numpy())
 
     def write_summaries(self, losses_dict):
         for name, val in losses_dict.items():

@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libdynaboa_b200.so')
 HOSTMATH_LIB = os.path.join(HERE, 'libdboa_hostmath.so')
-CUDA_SOURCES = ['conv.cu', 'conv_tc.cu', 'stem_wgrad.cu', 'groupnorm.cu', 'gn_fused.cu', 'norm_pool.cu', 'head.cu', 'smpl.cu', 'losses.cu', 'eval.cu', 'dataprocess.cu', 'optim.cu', 'hmr_plan.cu', 'cabi.cu']
+CUDA_SOURCES = ['conv.cu', 'conv_tc.cu', 'stem_wgrad.cu', 'groupnorm.cu', 'gn_fused.cu', 'norm_pool.cu', 'head.cu', 'smpl.cu', 'losses.cu', 'eval.cu', 'dataprocess.cu', 'optim.cu', 'hmr_plan.cu', 'render.cu', 'cabi.cu']
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
               '--expt-relaxed-constexpr', '-Xptxas', '-v']

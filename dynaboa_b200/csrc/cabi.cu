@@ -343,4 +343,13 @@ int dboa_eval_metrics(const float* pred_verts, const float* gt_verts_joints, con
     return eval_metrics(pred_verts, gt_verts_joints, gt_verts_pve, J_regressor, NJ, NV, joint_map, n_map, scratch, out, B, ST(stream));
 }
 
+long long dboa_render_scratch_bytes(int W, int H, int NV, int NF, int samples) { return render_scratch_bytes(W, H, NV, NF, samples); }
+int dboa_render_overlay(const float* verts, const int* faces, const int* vf_offsets, const int* vf_faces, int NV, int NF, const float cam4[4],
+                        const float rot3x3[9], const float color3[3], const unsigned char* img, int W, int H, int samples, void* scratch,
+                        long long scratch_bytes, unsigned char* out, int* face_ids, dboa_stream_t stream) {
+    if (!verts || !faces || !vf_offsets || !vf_faces || !cam4 || !color3 || !img || !scratch || !out) return DBOA_ERR_ARG;
+    return render_overlay(verts, faces, vf_offsets, vf_faces, NV, NF, cam4, rot3x3, color3, img, W, H, samples, scratch, scratch_bytes, out,
+                          face_ids, ST(stream));
+}
+
 }  // extern "C"

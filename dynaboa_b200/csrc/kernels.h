@@ -122,4 +122,10 @@ size_t eval_scratch_floats(int B, int NJ);
 int eval_metrics(const float* pred_verts, const float* gt_verts_joints, const float* gt_verts_pve, const float* Jreg, int NJ, int NV,
                  const int* joint_map, int n_map, float* scratch, float* out, int B, cudaStream_t st);
 
+// render.cu: mesh overlay (include/dynaboa_b200.h, "mesh overlay")
+long long render_scratch_bytes(int W, int H, int NV, int NF, int samples);
+int render_overlay(const float* verts, const int* faces, const int* vf_offsets, const int* vf_faces, int NV, int NF, const float cam4[4],
+                   const float rot3x3[9], const float color3[3], const unsigned char* img, int W, int H, int samples, void* scratch,
+                   long long scratch_bytes, unsigned char* out, int* face_ids, cudaStream_t st);
+
 }  // namespace dboa

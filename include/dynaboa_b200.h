@@ -264,6 +264,22 @@ long long dboa_eval_scratch_floats(int B, int NJ);
 int dboa_eval_metrics(const float* pred_verts, const float* gt_verts_joints, const float* gt_verts_pve, const float* J_regressor, int NJ,
                       int NV, const int* joint_map, int n_map, float* scratch, float* out, int B, dboa_stream_t stream);
 
+/* ---- mesh overlay (render_demo.py:58-153) -----------------------------------------------------
+ * replaces: Renderer.render (pyrender + trimesh, OpenGL off-screen) as called by base_adaptor.py:429-443 and
+ * utils/webcam_utils.py:71-79.  Draws one mesh over one frame; the contract (camera, culling, fill rule, depth, sample
+ * pattern, shading, composite) is DESIGN.md section 6 "Mesh overlay" and the header of csrc/render.cu.
+ * verts (NV,3) fp32, faces (NF,3) int32; vf_offsets (NV+1) / vf_faces (3 NF) int32: the vertex->face adjacency (CSR, faces
+ * of each vertex in ascending order), built once per faces array.  Host arrays: cam4 = (sx, sy, tx, ty) in the frame
+ * (convert_crop_cam_to_orig_img :136-153), rot3x3 = row-major angle/axis rotation applied after Rx(180) (NULL: none),
+ * color3 = base colour (0..1).  img / out (H,W,3) uint8 (channels pass through in the order given); face_ids (H,W,samples)
+ * int32 = winning face per sample, -1 where nothing is covered (NULL: not written).  samples 1 or 4.
+ * scratch: dboa_render_scratch_bytes() bytes.  W, H <= 8192, NV, NF >= 0 (DBOA_ERR_SHAPE otherwise).  Two calls on the same
+ * inputs give bit-identical out and face_ids. */
+long long dboa_render_scratch_bytes(int W, int H, int NV, int NF, int samples);
+int dboa_render_overlay(const float* verts, const int* faces, const int* vf_offsets, const int* vf_faces, int NV, int NF, const float cam4[4],
+                        const float rot3x3[9], const float color3[3], const unsigned char* img, int W, int H, int samples, void* scratch,
+                        long long scratch_bytes, unsigned char* out, int* face_ids, dboa_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
