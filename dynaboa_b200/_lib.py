@@ -55,6 +55,7 @@ SIGNATURES = {
     'dboa_hmr_arena_floats': (L, []),
     'dboa_hmr_param_info': (I, [I, C.c_char_p, I, C.POINTER(L), C.POINTER(I), C.POINTER(L), C.POINTER(L)]),
     'dboa_hmr_tape_floats': (L, [I]),
+    'dboa_hmr_tape_offset': (L, [I, I, I]),
     'dboa_hmr_scratch_floats': (L, [I]),
     'dboa_hmr_feature_info': (I, [I, I, C.POINTER(L), C.POINTER(I), C.POINTER(L), C.POINTER(L)]),
     'dboa_hmr_forward': (I, [P, P, P, P, P, I, P, P, P, P, P, P, P, P]),

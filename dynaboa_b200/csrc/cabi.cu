@@ -24,6 +24,7 @@ int hmr_num_params();
 long long hmr_arena_floats();
 int hmr_param_info(int i, char* name, int cap, long long* off, int* ndim, long long shape[4], long long stride[4]);
 long long hmr_tape_floats(int B);
+long long hmr_tape_offset(int B, int kind, int conv);
 long long hmr_scratch_floats(int B);
 int hmr_feature_info(int B, int i, long long* off, int* ndim, long long shape[4], long long stride[4]);
 
@@ -82,6 +83,7 @@ int dboa_hmr_param_info(int i, char* name, int name_cap, long long* offset, int*
     return hmr_param_info(i, name, name_cap, offset, ndim, shape, stride);
 }
 long long dboa_hmr_tape_floats(int B) { return hmr_tape_floats(B); }
+long long dboa_hmr_tape_offset(int B, int kind, int conv) { return hmr_tape_offset(B, kind, conv); }
 long long dboa_hmr_scratch_floats(int B) { return hmr_scratch_floats(B); }
 int dboa_hmr_feature_info(int B, int i, long long* offset, int* ndim, long long shape[4], long long stride[4]) {
     if (!offset || !ndim || !shape || !stride) return DBOA_ERR_ARG;

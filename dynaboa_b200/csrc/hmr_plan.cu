@@ -13,6 +13,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "../../include/dynaboa_b200.h"
 
 namespace dboa {
 
@@ -769,6 +770,29 @@ int hmr_param_info(int i, char* name, int cap, long long* off, int* ndim, long l
     return DBOA_OK;
 }
 long long hmr_tape_floats(int B) { return (B < 1 || B > 64) ? -1 : tape_for(B).total; }
+long long hmr_tape_offset(int B, int kind, int conv) {
+    if (B < 1 || B > 64) return DBOA_ERR_SHAPE;
+    const Tape& t = tape_for(B);
+    if (kind == DBOA_TAPE_Y || kind == DBOA_TAPE_STATS || kind == DBOA_TAPE_A) {
+        if (conv < 0 || conv >= (int)t.conv.size()) return DBOA_ERR_ARG;
+        const ConvTape& c = t.conv[conv];
+        if (kind == DBOA_TAPE_A && c.a < 0) return DBOA_ERR_ARG;         // downsample: the block's output is conv3's `a`
+        return kind == DBOA_TAPE_Y ? c.y : (kind == DBOA_TAPE_STATS ? c.stats : c.a);
+    }
+    switch (kind) {
+        case DBOA_TAPE_X0: return t.x0;
+        case DBOA_TAPE_P0: return t.p0;
+        case DBOA_TAPE_P0_IDX: return t.p0_idx;
+        case DBOA_TAPE_XC: return t.xc;
+        case DBOA_TAPE_H1PRE: return t.h1pre;
+        case DBOA_TAPE_H1POST: return t.h1post;
+        case DBOA_TAPE_H2PRE: return t.h2pre;
+        case DBOA_TAPE_H2POST: return t.h2post;
+        case DBOA_TAPE_PARAMS: return t.params;
+        case DBOA_TAPE_MASKS: return t.masks;
+        default: return DBOA_ERR_ARG;
+    }
+}
 long long hmr_scratch_floats(int B) { return (B < 1 || B > 64) ? -1 : Scratch(nullptr, B).total; }
 int hmr_feature_info(int B, int i, long long* off, int* ndim, long long shape[4], long long stride[4]) {
     if (B < 1 || B > 64 || i < 0 || i > 14) return DBOA_ERR_ARG;

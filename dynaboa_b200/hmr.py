@@ -82,6 +82,59 @@ def tape_floats(B):
     return _TAPE_FLOATS[B]
 
 
+# region kinds of dboa_hmr_tape_offset (include/dynaboa_b200.h, DBOA_TAPE_*)
+TAPE_Y, TAPE_STATS, TAPE_A = 0, 1, 2
+TAPE_WHOLE = {'x0': 3, 'p0': 4, 'p0_idx': 5, 'xc': 6, 'h1pre': 7, 'h1post': 8, 'h2pre': 9, 'h2post': 10, 'params': 11, 'masks': 12}
+
+
+def conv_geometry():
+    """Per convolution i (weight = parameter 3*i): (name, Cin, Cout, k, stride, Hout), from the parameter table and the
+    ResNet-50 rule that the first block of layers 2..4 downsamples in its conv2 and its shortcut."""
+    lay = layout()
+    out = []
+    for i in range(0, lay.n - 10, 3):
+        name = lay.names[i][:-len('.weight')]
+        cout, cin, k, _ = lay.shapes[i]
+        if name == 'conv1':
+            out.append((name, cin, cout, k, 2, 112))
+            continue
+        li, bi, part = int(name[5]), int(name.split('.')[1]), name.split('.')[2]
+        down = li > 1 and bi == 0
+        stride = 2 if down and part in ('conv2', 'downsample') else 1
+        out.append((name, cin, cout, k, stride, 56 >> (li - 2 if down and part == 'conv1' else li - 1)))
+    return out
+
+
+def tape_views(tape, B):
+    """Named NHWC views of a forward's tape (dboa_hmr_tape_offset): 'y', 'stats', 'a' are lists over the 53 convolutions
+    ('a' is None for the downsample convs), plus the whole-tape regions.  'p0_idx' is a uint8 view."""
+    lib = _lib.load()
+
+    def off(kind, conv=0):
+        o = lib.dboa_hmr_tape_offset(B, kind, conv)
+        if o < 0:
+            raise RuntimeError(f'dboa_hmr_tape_offset({B}, {kind}, {conv}) failed: {o}')
+        return o
+
+    def view(o, shape):
+        return tape.as_strided(shape, [math.prod(shape[d + 1:]) for d in range(len(shape))], o)
+    v = {'y': [], 'stats': [], 'a': []}
+    for i, (name, _, cout, _, _, h) in enumerate(conv_geometry()):
+        v['y'].append(view(off(TAPE_Y, i), (B, h, h, cout)))
+        v['stats'].append(view(off(TAPE_STATS, i), (B, 4, 2)))
+        v['a'].append(None if 'downsample' in name else view(off(TAPE_A, i), (B, h, h, cout)))
+    v['x0'] = view(off(TAPE_WHOLE['x0']), (B, 224, 224, 3))
+    v['p0'] = view(off(TAPE_WHOLE['p0']), (B, 56, 56, 64))
+    n = B * 56 * 56 * 64
+    v['p0_idx'] = tape.view(torch.uint8)[4 * off(TAPE_WHOLE['p0_idx']):][:n].view(B, 56, 56, 64)
+    v['xc'] = view(off(TAPE_WHOLE['xc']), (3, B, 2208))
+    for k in ('h1pre', 'h1post', 'h2pre', 'h2post'):
+        v[k] = view(off(TAPE_WHOLE[k]), (3, B, 1024))
+    v['params'] = view(off(TAPE_WHOLE['params']), (4, B, 160))
+    v['masks'] = view(off(TAPE_WHOLE['masks']), (3, 2, B, 1024))
+    return v
+
+
 def scratch_for(B, device):
     """Per-(device, B, stream) scratch shared by forward and backward; stream-ordered reuse is safe, and forwards
     issued concurrently on different streams (teacher next to the fast-weight forward) get separate buffers."""

@@ -52,6 +52,28 @@ long long dboa_hmr_arena_floats(void);
 int dboa_hmr_param_info(int i, char* name, int name_cap, long long* offset, int* ndim, long long shape[4], long long stride[4]);
 long long dboa_hmr_tape_floats(int B);      /* activations saved by the forward (also holds the features) */
 long long dboa_hmr_scratch_floats(int B);   /* scratch shared by forward (split-K) and backward */
+/* Float offset of one region of the tape of batch B (host only, no device access), for tests and debugging tools that read
+ * what the forward saved.  Per convolution `conv` (the conv whose weight is dboa_hmr_param_info(3 * conv)), NHWC:
+ *   Y      (B,Ho,Wo,Cout) convolution output;  STATS (B,4,2) GroupNorm (mean, rstd) per (sample, group);
+ *   A      (B,Ho,Wo,Cout) post-activation output -- DBOA_ERR_ARG for a downsample conv, whose block output is conv3's A.
+ * Whole tape (`conv` ignored): X0 (B,224,224,3) image; P0 (B,56,56,64) max-pool output; P0_IDX the window position r*3+s of
+ * each max-pool output as one byte, same (B,56,56,64) order; XC (3,B,2208) regressor input rows; H1PRE, H1POST, H2PRE, H2POST
+ * (3,B,1024) hidden rows before / after dropout; PARAMS (4,B,160) running SMPL parameters (first 157 used); MASKS (3,2,B,1024)
+ * dropout keep-masks.  Returns DBOA_ERR_SHAPE for B outside 1..64 and DBOA_ERR_ARG for an unknown kind or conv. */
+#define DBOA_TAPE_Y 0
+#define DBOA_TAPE_STATS 1
+#define DBOA_TAPE_A 2
+#define DBOA_TAPE_X0 3
+#define DBOA_TAPE_P0 4
+#define DBOA_TAPE_P0_IDX 5
+#define DBOA_TAPE_XC 6
+#define DBOA_TAPE_H1PRE 7
+#define DBOA_TAPE_H1POST 8
+#define DBOA_TAPE_H2PRE 9
+#define DBOA_TAPE_H2POST 10
+#define DBOA_TAPE_PARAMS 11
+#define DBOA_TAPE_MASKS 12
+long long dboa_hmr_tape_offset(int B, int kind, int conv);
 /* feature i of HMR.forward(need_feature=True) (model/hmr.py:138-168) as a strided view of the tape */
 int dboa_hmr_feature_info(int B, int i, long long* offset, int* ndim, long long shape[4], long long stride[4]);
 
