@@ -23,7 +23,8 @@ class SmplModelStruct(C.Structure):
 class LossArgsStruct(C.Structure):
     _fields_ = ([('B', I)] + [(n, P) for n in ('p2d', 'j3d', 'R', 'beta', 'kp', 'prior_b', 't_p2d', 't_j3d', 't_beta',
                                                  't_R', 'gt_s3d')]
-                + [('w', F * 8), ('terms', P), ('dp2d', P), ('dj3d', P), ('dR', P), ('dbeta', P), ('dR_accumulate', I), ('kp_first', I), ('kp_count', I)])
+                + [('w', F * 8), ('terms', P), ('dp2d', P), ('dj3d', P), ('dR', P), ('dbeta', P), ('dR_accumulate', I), ('kp_first', I), ('kp_count', I),
+                   ('groups', I)])
 
 
 class FusedConvStruct(C.Structure):
@@ -47,6 +48,7 @@ SIGNATURES = {
     'dboa_set_fused_forward': (I, [I]),
     'dboa_get_fused_forward': (I, []),
     'dboa_set_fused_backward': (I, [I]),
+    'dboa_get_fused_backward': (I, []),
     'dboa_dgrad_fused': (I, [C.POINTER(DgradFusedStruct), I, I, I, I, I, P]),
     'dboa_conv_fused_part_floats': (L, [I, I, I]),
     'dboa_conv_fused_fwd': (I, [C.POINTER(FusedConvStruct), I, I, P]),
@@ -60,6 +62,8 @@ SIGNATURES = {
     'dboa_hmr_feature_info': (I, [I, I, C.POINTER(L), C.POINTER(I), C.POINTER(L), C.POINTER(L)]),
     'dboa_hmr_forward': (I, [P, P, P, P, P, I, P, P, P, P, P, P, P, P]),
     'dboa_hmr_backward': (I, [P, P, I, I, P, P, P, P, P, P]),
+    'dboa_hmr_forward_groups': (I, [P, P, P, P, P, I, P, P, P, P, P, P, P, P, I]),
+    'dboa_hmr_backward_groups': (I, [P, P, I, I, P, P, P, P, P, P, I]),
     'dboa_conv2d_fwd': (I, [P, P, P, I, I, I, I, I, I, I, I, I, P, L, P]),
     'dboa_conv2d_dgrad': (I, [P, P, P, I, I, I, I, I, I, I, I, I, I, P, L, P]),
     'dboa_conv2d_wgrad': (I, [P, P, P, I, I, I, I, I, I, I, I, I, P, L, P]),
@@ -89,6 +93,7 @@ SIGNATURES = {
     'dboa_loss_multi': (I, [C.POINTER(LossArgsStruct), P]),
     'dboa_loss_motion': (I, [P, P, P, P, F, P, P, P, I, I, P]),
     'dboa_loss_motion_joints': (I, [P, P, P, P, F, P, P, P, I, I, I, I, P]),
+    'dboa_loss_motion_groups': (I, [P, P, P, P, F, P, P, P, I, I, I, I, I, P]),
     'dboa_sgd_update': (I, [P, P, P, F, L, P]),
     'dboa_adam_ema': (I, [P, P, P, P, P, L, F, F, F, F, I, F, P]),
     'dboa_ema_update': (I, [P, P, L, F, P]),

@@ -12,14 +12,15 @@
 namespace dboa {
 int hmr_forward(const float* P, const float* init_pose, const float* init_shape, const float* init_cam, const float* image, int B,
                 const float* drop_masks, float* T, float* scratch, float* rotmat, float* shape, float* cam, float* pose6d,
-                cudaStream_t st);
+                cudaStream_t st, int groups);
 int hmr_backward(const float* P, const float* T, int B, int masked, const float* d_rotmat, const float* d_shape, const float* d_cam,
-                 float* G, float* scratch, cudaStream_t st);
+                 float* G, float* scratch, cudaStream_t st, int groups);
 void hmr_arm_bucket_events(cudaEvent_t e0, cudaEvent_t e1, cudaEvent_t e2);
 long long hmr_bucket_offset(int k);
 void hmr_set_fused_forward(bool on);
 void hmr_set_fused_backward(bool on);
 bool hmr_fused_forward();
+bool hmr_fused_backward();
 int hmr_num_params();
 long long hmr_arena_floats();
 int hmr_param_info(int i, char* name, int cap, long long* off, int* ndim, long long shape[4], long long stride[4]);
@@ -75,6 +76,7 @@ int dboa_set_tensor_core_conv(int enable) { conv_tc_set_mode(enable); return DBO
 int dboa_set_fused_forward(int enable) { hmr_set_fused_forward(enable != 0); return DBOA_OK; }
 int dboa_get_fused_forward(void) { return hmr_fused_forward() ? 1 : 0; }
 int dboa_set_fused_backward(int enable) { hmr_set_fused_backward(enable != 0); return DBOA_OK; }
+int dboa_get_fused_backward(void) { return hmr_fused_backward() ? 1 : 0; }
 
 int dboa_hmr_num_params(void) { return hmr_num_params(); }
 long long dboa_hmr_arena_floats(void) { return hmr_arena_floats(); }
@@ -93,12 +95,24 @@ int dboa_hmr_forward(const float* arena, const float* init_pose, const float* in
                      int B, const float* drop_masks, float* tape, float* scratch, float* rotmat, float* shape, float* cam, float* pose6d,
                      dboa_stream_t stream) {
     if (!arena || !init_pose || !init_shape || !init_cam || !image || !tape || !scratch || !rotmat || !shape || !cam) return DBOA_ERR_ARG;
-    return hmr_forward(arena, init_pose, init_shape, init_cam, image, B, drop_masks, tape, scratch, rotmat, shape, cam, pose6d, ST(stream));
+    return hmr_forward(arena, init_pose, init_shape, init_cam, image, B, drop_masks, tape, scratch, rotmat, shape, cam, pose6d, ST(stream), 1);
 }
 int dboa_hmr_backward(const float* arena, const float* tape, int B, int masked, const float* d_rotmat, const float* d_shape,
                       const float* d_cam, float* grad_arena, float* scratch, dboa_stream_t stream) {
     if (!arena || !tape || !grad_arena || !scratch) return DBOA_ERR_ARG;
-    return hmr_backward(arena, tape, B, masked, d_rotmat, d_shape, d_cam, grad_arena, scratch, ST(stream));
+    return hmr_backward(arena, tape, B, masked, d_rotmat, d_shape, d_cam, grad_arena, scratch, ST(stream), 1);
+}
+int dboa_hmr_forward_groups(const float* arena, const float* init_pose, const float* init_shape, const float* init_cam, const float* image,
+                            int B, const float* drop_masks, float* tape, float* scratch, float* rotmat, float* shape, float* cam,
+                            float* pose6d, dboa_stream_t stream, int groups) {
+    if (!arena || !init_pose || !init_shape || !init_cam || !image || !tape || !scratch || !rotmat || !shape || !cam) return DBOA_ERR_ARG;
+    return hmr_forward(arena, init_pose, init_shape, init_cam, image, B, drop_masks, tape, scratch, rotmat, shape, cam, pose6d, ST(stream),
+                       groups);
+}
+int dboa_hmr_backward_groups(const float* arena, const float* tape, int B, int masked, const float* d_rotmat, const float* d_shape,
+                             const float* d_cam, float* grad_arena, float* scratch, dboa_stream_t stream, int groups) {
+    if (!arena || !tape || !grad_arena || !scratch) return DBOA_ERR_ARG;
+    return hmr_backward(arena, tape, B, masked, d_rotmat, d_shape, d_cam, grad_arena, scratch, ST(stream), groups);
 }
 
 int dboa_conv2d_fwd(const float* x, const float* w, float* y, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad, int Kpitch,
@@ -268,6 +282,12 @@ int dboa_loss_motion_joints(const float* p_cur, const float* p_hist, const float
                             float* dp_cur, float* dp_hist, int B, int accumulate_cur, int first, int count, dboa_stream_t stream) {
     if (!p_cur || !p_hist || !kp_cur || !kp_hist || !term || !dp_cur || !dp_hist || B < 1) return DBOA_ERR_ARG;
     return loss_motion_launch(p_cur, p_hist, kp_cur, kp_hist, weight, term, dp_cur, dp_hist, B, accumulate_cur, first, count, ST(stream));
+}
+int dboa_loss_motion_groups(const float* p_cur, const float* p_hist, const float* kp_cur, const float* kp_hist, float weight, float* term,
+                            float* dp_cur, float* dp_hist, int B, int accumulate_cur, int first, int count, int groups, dboa_stream_t stream) {
+    if (!p_cur || !p_hist || !kp_cur || !kp_hist || !term || !dp_cur || !dp_hist || B < 1) return DBOA_ERR_ARG;
+    return loss_motion_launch(p_cur, p_hist, kp_cur, kp_hist, weight, term, dp_cur, dp_hist, B, accumulate_cur, first, count, ST(stream),
+                              groups);
 }
 
 int dboa_sgd_update(const float* p, const float* g, float* out, float lr, long long n, dboa_stream_t stream) {

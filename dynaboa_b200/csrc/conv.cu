@@ -98,7 +98,8 @@ __device__ __forceinline__ void cluster_reduce_store(const float acc[4][4], floa
 // forward:  y[m][n] = sum_k xcol[m][k] * w[n][k],   m = (b,ho,wo), k = (r,s,ci)
 // grid (ceil(M/64), Cout/64, nsplit); each z-slice covers k in [z*klen, (z+1)*klen)
 // ---------------------------------------------------------------------------------------------
-template <int VEC>
+// GROUPED (all three kernels): a call over d.groups > 1 groups; the group arithmetic is compiled only into that instantiation
+template <int VEC, bool GROUPED>
 __global__ void __launch_bounds__(NT) conv_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                       float* __restrict__ out, ConvDims d, int klen) {
     __shared__ __align__(16) float As[BK][BM + PADM];
@@ -106,7 +107,13 @@ __global__ void __launch_bounds__(NT) conv_fwd_kernel(const float* __restrict__ 
     __shared__ __align__(16) float red[BM * BN];
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
     const int M = d.B * d.Ho * d.Wo, K = d.kh * d.kw * d.Cin;
-    const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
+    int bx = blockIdx.x;
+    if (GROUPED) {                                                       // the row tiles of group grp
+        const int gx = gridDim.x / d.groups, grp = blockIdx.x / gx;
+        x += (size_t)grp * d.B * d.Hi * d.Wi * d.Cin; w += grp * d.wstride; out += (size_t)grp * M * d.Cout;
+        bx -= grp * gx;
+    }
+    const int m0 = bx * BM, n0 = blockIdx.y * BN;
     const int kbeg = blockIdx.z * klen, kend = min(kbeg + klen, (K + BK - 1) / BK * BK);
 
     // loader roles: row = tid/4, kv = tid%4 (4 consecutive k)
@@ -186,6 +193,7 @@ __global__ void __launch_bounds__(NT) conv_fwd_kernel(const float* __restrict__ 
 //   m = (b,hi,wi);  ho = (hi + pad - r)/stride when divisible and in range
 // GEMM view: M = B*Hi*Wi, N = Cin, K = kh*kw*Cout ordered (r,s,co)
 // ---------------------------------------------------------------------------------------------
+template <bool GROUPED>
 __global__ void __launch_bounds__(NT) conv_dgrad_kernel(const float* __restrict__ dy, const float* __restrict__ w,
                                                         float* __restrict__ out, ConvDims d, int klen, int accumulate) {
     __shared__ __align__(16) float As[BK][BM + PADM];
@@ -193,7 +201,13 @@ __global__ void __launch_bounds__(NT) conv_dgrad_kernel(const float* __restrict_
     __shared__ __align__(16) float red[BM * BN];
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
     const int M = d.B * d.Hi * d.Wi, K = d.kh * d.kw * d.Cout;
-    const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
+    int bx = blockIdx.x;
+    if (GROUPED) {
+        const int gx = gridDim.x / d.groups, grp = blockIdx.x / gx;
+        dy += (size_t)grp * d.B * d.Ho * d.Wo * d.Cout; w += grp * d.wstride; out += (size_t)grp * M * d.Cin;
+        bx -= grp * gx;
+    }
+    const int m0 = bx * BM, n0 = blockIdx.y * BN;
     const int kbeg = blockIdx.z * klen, kend = min(kbeg + klen, K);
 
     const int lrow = tid >> 2, lkv = (tid & 3) * 4;       // A loader: 4 consecutive co
@@ -260,7 +274,7 @@ __global__ void __launch_bounds__(NT) conv_dgrad_kernel(const float* __restrict_
 // weight gradient:  dw[co][(r,s,ci)] (+)= sum_m dy[m][co] * xcol[m][(r,s,ci)]
 // GEMM view: M' = Cout, N' = kh*kw*Cin, K' = B*Ho*Wo (split over blockIdx.z)
 // ---------------------------------------------------------------------------------------------
-template <int VEC>
+template <int VEC, bool GROUPED>
 __global__ void __launch_bounds__(NT) conv_wgrad_kernel(const float* __restrict__ dy, const float* __restrict__ x,
                                                         float* __restrict__ out, ConvDims d, int plen) {
     __shared__ __align__(16) float As[BK][BM + PADM];
@@ -268,7 +282,13 @@ __global__ void __launch_bounds__(NT) conv_wgrad_kernel(const float* __restrict_
     __shared__ __align__(16) float red[BM * BN];
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
     const int Mpix = d.B * d.Ho * d.Wo, K = d.kh * d.kw * d.Cin;
-    const int m0 = blockIdx.x * BM /* co */, n0 = blockIdx.y * BN /* (r,s,ci) */;
+    int bx = blockIdx.x;
+    if (GROUPED) {                                                       // K' = this group's B*Ho*Wo pixels
+        const int gx = gridDim.x / d.groups, grp = blockIdx.x / gx;
+        dy += (size_t)grp * Mpix * d.Cout; x += (size_t)grp * d.B * d.Hi * d.Wi * d.Cin; out += grp * d.wstride;
+        bx -= grp * gx;
+    }
+    const int m0 = bx * BM /* co */, n0 = blockIdx.y * BN /* (r,s,ci) */;
     const int pbeg = blockIdx.z * plen, pend = min(pbeg + plen, Mpix);
 
     const int lk = tid >> 4, lv = (tid & 15) * 4;
@@ -355,29 +375,32 @@ static int launch_z_cluster(K kernel, dim3 grid, cudaStream_t st, Args... args) 
 
 int conv_fwd(const float* x, const float* w, float* y, const ConvDims& d, float* ws, size_t ws_floats, cudaStream_t st) {
     (void)ws; (void)ws_floats;
+    if (d.groups < 1) return DBOA_ERR_SHAPE;
     if (d.Cout % BN != 0 || d.Kpitch % 4 != 0) return DBOA_ERR_SHAPE;
     const int M = d.B * d.Ho * d.Wo, K = d.kh * d.kw * d.Cin;
     if (d.Kpitch < (K + BK - 1) / BK * BK) return DBOA_ERR_SHAPE;
     const int kiters = (K + BK - 1) / BK;
-    const int tiles = ceil_div(M, BM) * (d.Cout / BN);
+    const int tiles = d.groups * ceil_div(M, BM) * (d.Cout / BN);
     const int ns = pick_split(tiles, kiters);
     const int klen = ((kiters + ns - 1) / ns) * BK;
-    dim3 grid(ceil_div(M, BM), d.Cout / BN, ns);
-    if (d.Cin % 4 == 0) return launch_z_cluster(conv_fwd_kernel<4>, grid, st, x, w, y, d, klen);
-    return launch_z_cluster(conv_fwd_kernel<1>, grid, st, x, w, y, d, klen);
+    dim3 grid(d.groups * ceil_div(M, BM), d.Cout / BN, ns);
+    const bool g = d.groups > 1;
+    if (d.Cin % 4 == 0) return launch_z_cluster(g ? conv_fwd_kernel<4, true> : conv_fwd_kernel<4, false>, grid, st, x, w, y, d, klen);
+    return launch_z_cluster(g ? conv_fwd_kernel<1, true> : conv_fwd_kernel<1, false>, grid, st, x, w, y, d, klen);
 }
 
 int conv_dgrad(const float* dy, const float* w, float* dx, const ConvDims& d, int accumulate, float* ws, size_t ws_floats,
                cudaStream_t st) {
     (void)ws; (void)ws_floats;
+    if (d.groups < 1) return DBOA_ERR_SHAPE;
     if (d.Cin % BN != 0 || d.Cout % BK != 0) return DBOA_ERR_SHAPE;
     const int M = d.B * d.Hi * d.Wi, K = d.kh * d.kw * d.Cout;
     const int kiters = K / BK;
-    const int tiles = ceil_div(M, BM) * (d.Cin / BN);
+    const int tiles = d.groups * ceil_div(M, BM) * (d.Cin / BN);
     const int ns = pick_split(tiles, kiters);
     const int klen = ((kiters + ns - 1) / ns) * BK;
-    dim3 grid(ceil_div(M, BM), d.Cin / BN, ns);
-    return launch_z_cluster(conv_dgrad_kernel, grid, st, dy, w, dx, d, klen, accumulate);
+    dim3 grid(d.groups * ceil_div(M, BM), d.Cin / BN, ns);
+    return launch_z_cluster(d.groups > 1 ? conv_dgrad_kernel<true> : conv_dgrad_kernel<false>, grid, st, dy, w, dx, d, klen, accumulate);
 }
 
 int conv_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, float* ws, size_t ws_floats, cudaStream_t st) {
@@ -386,15 +409,16 @@ int conv_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, fl
         const int s = stem_wgrad(dy, x, dw, d, ws, ws_floats, st);
         if (s != DBOA_ERR_UNSUPPORTED) return s;
     }
-    if (d.Cout % BM != 0) return DBOA_ERR_SHAPE;
+    if (d.Cout % BM != 0 || d.groups < 1) return DBOA_ERR_SHAPE;
     const int Mpix = d.B * d.Ho * d.Wo, K = d.kh * d.kw * d.Cin;
     const int piters = ceil_div(Mpix, BK);
-    const int tiles = (d.Cout / BM) * ceil_div(K, BN);
+    const int tiles = d.groups * (d.Cout / BM) * ceil_div(K, BN);
     const int ns = pick_split(tiles, piters);
     const int plen = ((piters + ns - 1) / ns) * BK;
-    dim3 grid(d.Cout / BM, ceil_div(K, BN), ns);
-    if (d.Cin % 4 == 0) return launch_z_cluster(conv_wgrad_kernel<4>, grid, st, dy, x, dw, d, plen);
-    return launch_z_cluster(conv_wgrad_kernel<1>, grid, st, dy, x, dw, d, plen);
+    dim3 grid(d.groups * (d.Cout / BM), ceil_div(K, BN), ns);
+    const bool g = d.groups > 1;
+    if (d.Cin % 4 == 0) return launch_z_cluster(g ? conv_wgrad_kernel<4, true> : conv_wgrad_kernel<4, false>, grid, st, dy, x, dw, d, plen);
+    return launch_z_cluster(g ? conv_wgrad_kernel<1, true> : conv_wgrad_kernel<1, false>, grid, st, dy, x, dw, d, plen);
 }
 
 }  // namespace dboa

@@ -181,7 +181,8 @@ __device__ __forceinline__ void add_fixed(long long* p, double v, double scale) 
 }
 
 // P: the operand that pairs with the weights in FWD/DGRAD (x or dy); Q: weights (FWD/DGRAD) or x (WGRAD, with P = dy)
-template <int MODE, int XF>
+// GROUPED: a call over d.groups > 1 groups (the group arithmetic is compiled only into this instantiation)
+template <int MODE, int XF, bool GROUPED = false>
 __global__ void __launch_bounds__(NT, 1) conv_tf32x3_kernel(const float* __restrict__ P, const float* __restrict__ Q, float* __restrict__ O,
                                                             ConvDims d, int kb_per_split, int accumulate, const Ext e) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
@@ -191,18 +192,29 @@ __global__ void __launch_bounds__(NT, 1) conv_tf32x3_kernel(const float* __restr
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     DBOA_TL(0);
     const int Ktaps = d.kh * d.kw, Kfull = Ktaps * d.Cin;
+    // Grouped call: blockIdx.x = group * gx + tile, and group grp reads / writes only its own samples and weights (no tile
+    // straddles two groups, since the weight operand differs per group).  groups == 1: grp = 0, bx = blockIdx.x.
+    int gx = gridDim.x, bx = blockIdx.x;
+    if (GROUPED) {
+        const int grp = blockIdx.x / (gridDim.x / d.groups);
+        gx = gridDim.x / d.groups; bx = blockIdx.x - grp * gx;
+        const size_t xin = (size_t)grp * d.B * d.Hi * d.Wi * d.Cin, yout = (size_t)grp * d.B * d.Ho * d.Wo * d.Cout;
+        if (MODE == FWD) { P += xin; Q += grp * d.wstride; O += yout; }
+        else if (MODE == DGRAD) { P += yout; Q += grp * d.wstride; O += xin; }
+        else { P += yout; Q += xin; O += grp * d.wstride; }
+    }
     // GEMM extents of this mode
     // Stride-2 data gradient: an input pixel (hi, wi) only receives the filter taps r = hi + pad (mod 2), s = wi + pad (mod 2).
     // The rows are therefore enumerated per PARITY CLASS (hi & 1, wi & 1): blockIdx.x = class * tiles_per_class + tile, every
     // tile holds rows of one class and reduces over that class's taps only (3x3: 1, 2, 2, 4 of 9 taps; 1x1: one class, the
     // other three receive nothing).  Without this 3/4 of the rows of every 128-row tile were zero-filled.
     const bool par = MODE == DGRAD && d.stride == 2;
-    int py = 0, px = 0, Hh = d.Hi, Wh = d.Wi, r0 = 0, s0 = 0, nr = d.kh, nsx = d.kw, tstep = 1, mtile = blockIdx.x;
+    int py = 0, px = 0, Hh = d.Hi, Wh = d.Wi, r0 = 0, s0 = 0, nr = d.kh, nsx = d.kw, tstep = 1, mtile = bx;
     if (par) {
         // a 1-tap filter axis has ONE non-empty parity (the epilogue zero-fills the sibling pixels); classes = npy * npx
         const int npy = d.kh >= 2 ? 2 : 1, npx = d.kw >= 2 ? 2 : 1;
-        const int tpc = gridDim.x / (npy * npx), cls = blockIdx.x / tpc;
-        mtile = blockIdx.x - cls * tpc;
+        const int tpc = gx / (npy * npx), cls = bx / tpc;
+        mtile = bx - cls * tpc;
         py = npy == 2 ? cls / npx : (d.pad & 1); px = npx == 2 ? cls % npx : (d.pad & 1); Hh = d.Hi >> 1; Wh = d.Wi >> 1;
         r0 = (py + d.pad) & 1; s0 = (px + d.pad) & 1;
         nr = (d.kh - r0 + 1) >> 1; nsx = (d.kw - s0 + 1) >> 1; tstep = 2;
@@ -652,6 +664,7 @@ static int launch(const float* p, const float* q, float* o, const ConvDims& d, i
         mtiles = ncls * ceil_div(d.B * (d.Hi / 2) * (d.Wi / 2), BM);
         kred = ((d.kh + 1) / 2) * ((d.kw + 1) / 2) * d.Cout;
     }
+    mtiles *= d.groups;                                  // every group's tiles count towards the split-K sizing
     const int nkb = (kred + BK - 1) / BK;
     const int tiles = mtiles * (cols / BN);
     // K-slices per tile (cluster size): a power of two <= 8 (the portable cluster size) that keeps the grid within about one wave; a split must
@@ -662,12 +675,14 @@ static int launch(const float* p, const float* q, float* o, const ConvDims& d, i
     while (ns < 8 && tiles * ns * 2 <= slots + tiles && nkb / (ns * 2) >= min_kb) ns *= 2;
     const int per = (nkb + ns - 1) / ns;
     const size_t smem = sizeof(Smem) + 128;
-    return launch_ex(conv_tf32x3_kernel<MODE, XF>, dim3(mtiles, cols / BN, ns), dim3(NT), smem, st, dim3(1, 1, ns), pdl, p, q, o, d, per,
-                     accumulate, e);
+    auto kernel = conv_tf32x3_kernel<MODE, XF>;
+    if constexpr (XF < 0)                                 // the fused variants serve one group only
+        if (d.groups > 1) kernel = conv_tf32x3_kernel<MODE, XF, true>;
+    return launch_ex(kernel, dim3(mtiles, cols / BN, ns), dim3(NT), smem, st, dim3(1, 1, ns), pdl, p, q, o, d, per, accumulate, e);
 }
 
 static bool shape_ok(const ConvDims& d) {
-    return d.Cin % 64 == 0 && d.Cout % 64 == 0 && d.Kpitch == d.kh * d.kw * d.Cin;
+    return d.groups >= 1 && d.Cin % 64 == 0 && d.Cout % 64 == 0 && d.Kpitch == d.kh * d.kw * d.Cin;
 }
 
 }  // namespace tc

@@ -79,7 +79,7 @@ __device__ __forceinline__ float2 block_sum2(float a, float b, float* red) {
 __global__ void __launch_bounds__(GN_NT, 1) gn_fwd_fused_kernel(const float* __restrict__ y, const float* __restrict__ gamma,
                                                              const float* __restrict__ beta, const float* __restrict__ res,
                                                              float* __restrict__ out, float* __restrict__ stats, int HW, int C, int R,
-                                                             int lg, int relu) {
+                                                             int lg, int relu, int bper, long long pstride) {
     cg::cluster_group cluster = cg::this_cluster();
     __shared__ float red1[64], red2[64];
     __shared__ float part[4];                 // this CTA's (count, mean, M2)
@@ -92,6 +92,7 @@ __global__ void __launch_bounds__(GN_NT, 1) gn_fwd_fused_kernel(const float* __r
     const int cv = threadIdx.x & (cg4 - 1), rt = threadIdx.x >> lg, rstep = GN_NT >> lg;
     const size_t e0 = ((size_t)b * HW + r0 + rt) * C + g * cgc + cv * 4;
     const size_t estep = (size_t)rstep * C;
+    gamma += (b / bper) * pstride; beta += (b / bper) * pstride;          // the affine parameters of this sample's group
     const float4 ga = ldg4(gamma + g * cgc + cv * 4), be = ldg4(beta + g * cgc + cv * 4);
     float4 v[GN_V], rr[GN_V];
     bool ok[GN_V];
@@ -152,12 +153,13 @@ __global__ void __launch_bounds__(GN_NT, 1) gn_fwd_fused_kernel(const float* __r
 }
 
 int gn_fwd_fused(const float* y, const float* gamma, const float* beta, const float* res, float* out, float* stats, float* partial,
-                 int B, int HW, int C, int relu, cudaStream_t st) {
+                 int B, int HW, int C, int relu, cudaStream_t st, int bper, long long pstride) {
     (void)partial;
     GnPlan pl;
-    if (!gn_plan(HW, C, &pl)) return DBOA_ERR_SHAPE;
+    if (bper <= 0) bper = B;
+    if (!gn_plan(HW, C, &pl) || B % bper != 0) return DBOA_ERR_SHAPE;
     return launch_ex(gn_fwd_fused_kernel, dim3(pl.chunks, GN_G, B), dim3(GN_NT), 0, st, dim3(pl.chunks, 1, 1), true, y, gamma, beta, res, out,
-                     stats, HW, C, pl.rows, pl.lg, relu);
+                     stats, HW, C, pl.rows, pl.lg, relu, bper, pstride);
 }
 
 // backward: grid (chunks, 4, B), cluster (chunks, 1, 1)
@@ -168,7 +170,7 @@ __global__ void __launch_bounds__(GN_NT, 1) gn_bwd_fused_kernel(const float* __r
                                                              const float* __restrict__ gamma, float* __restrict__ dy,
                                                              float* __restrict__ dgamma, float* __restrict__ dbeta,
                                                              float* __restrict__ rows_g, float* __restrict__ rows_b, unsigned* pcounters,
-                                                             int HW, int C, int R, int lg, int defer) {
+                                                             int HW, int C, int R, int lg, int defer, int bper, long long pstride) {
     cg::cluster_group cluster = cg::this_cluster();
     __shared__ float red1[64];
     __shared__ float part[2];
@@ -186,6 +188,7 @@ __global__ void __launch_bounds__(GN_NT, 1) gn_bwd_fused_kernel(const float* __r
     const size_t e0 = ((size_t)b * HW + r0 + rt) * C + g * cgc + cv * 4;
     const size_t estep = (size_t)rstep * C;
     const float mean = stats[slot * 2], rstd = stats[slot * 2 + 1];
+    gamma += (b / bper) * pstride;
     const float4 ga = ldg4(gamma + g * cgc + cv * 4);
     float4 d[GN_V], xh[GN_V];
     bool ok[GN_V];
@@ -306,34 +309,42 @@ __global__ void __launch_bounds__(GN_NT, 1) gn_bwd_fused_kernel(const float* __r
 }
 
 int gn_bwd_fused(const float* dout, const float* mask_src, const float* y, const float* stats, const float* gamma, float* dy,
-                 float* dgamma, float* dbeta, float* partial, int B, int HW, int C, cudaStream_t st, int defer) {
+                 float* dgamma, float* dbeta, float* partial, int B, int HW, int C, cudaStream_t st, int defer, int bper,
+                 long long pstride) {
     GnPlan pl;
-    if (!gn_plan(HW, C, &pl) || (C / 16) > 128) return DBOA_ERR_SHAPE;
+    if (bper <= 0) bper = B;
+    if (!gn_plan(HW, C, &pl) || (C / 16) > 128 || B % bper != 0) return DBOA_ERR_SHAPE;
+    if (bper < B && !defer) return DBOA_ERR_UNSUPPORTED;       // per-group affine gradients are reduced by gn_param_finish
     unsigned* cnt = sync_words();
     if (!cnt) return DBOA_ERR_CUDA;
     return launch_ex(gn_bwd_fused_kernel, dim3(pl.chunks, GN_G, B), dim3(GN_NT), 0, st, dim3(pl.chunks, 1, 1), true, dout, mask_src, y, stats,
-                     gamma, dy, dgamma, dbeta, partial, partial + (size_t)B * C, cnt, HW, C, pl.rows, pl.lg, defer);
+                     gamma, dy, dgamma, dbeta, partial, partial + (size_t)B * C, cnt, HW, C, pl.rows, pl.lg, defer, bper, pstride);
 }
 
 // Deferred affine-parameter gradients of a whole network (B > 1): every GroupNorm backward left its per-sample rows
 // [B][C] (dgamma) | [B][C] (dbeta) at rows + 2 * B * item.cum_channels; ONE launch adds them to the gradient arena in sample
 // order.  This keeps the per-layer kernels free of the fence + ticket + last-CTA pass that B > 1 otherwise needs.
+// Grouped (gridDim.y groups of B / groups samples): group blockIdx.y sums its own rows into G + blockIdx.y * pstride.
 __global__ void __launch_bounds__(256) gn_param_finish_kernel(const GnFinishItem* __restrict__ items, const float* __restrict__ rows,
-                                                              float* __restrict__ G, int B) {
+                                                              float* __restrict__ G, int B, long long pstride) {
     pdl_wait();
     pdl_trigger();
     const GnFinishItem it = items[blockIdx.x];
+    const int bper = B / gridDim.y, r0 = blockIdx.y * bper;
+    G += blockIdx.y * pstride;
     const float* rg = rows + 2 * (size_t)B * it.cum_channels;
     const float* rb = rg + (size_t)B * it.C;
     for (int c = threadIdx.x; c < it.C; c += 256) {
         float a = 0.f, bsum = 0.f;
-        for (int r = 0; r < B; ++r) { a += rg[(size_t)r * it.C + c]; bsum += rb[(size_t)r * it.C + c]; }
+        for (int r = r0; r < r0 + bper; ++r) { a += rg[(size_t)r * it.C + c]; bsum += rb[(size_t)r * it.C + c]; }
         G[it.g_off + c] += a; G[it.b_off + c] += bsum;
     }
 }
 
-int gn_param_finish(const GnFinishItem* items_dev, int n_items, const float* rows, float* G, int B, cudaStream_t st) {
-    return launch_ex(gn_param_finish_kernel, dim3(n_items), dim3(256), 0, st, dim3(1, 1, 1), true, items_dev, rows, G, B);
+int gn_param_finish(const GnFinishItem* items_dev, int n_items, const float* rows, float* G, int B, cudaStream_t st, int groups,
+                    long long pstride) {
+    if (groups < 1 || B % groups != 0) return DBOA_ERR_SHAPE;
+    return launch_ex(gn_param_finish_kernel, dim3(n_items, groups), dim3(256), 0, st, dim3(1, 1, 1), true, items_dev, rows, G, B, pstride);
 }
 
 }  // namespace dboa

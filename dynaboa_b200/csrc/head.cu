@@ -19,10 +19,13 @@ __global__ void __launch_bounds__(256) linear_fwd_kernel(const float* __restrict
                                                          const float* __restrict__ bias, const float* __restrict__ addend, int ld_add,
                                                          const float* __restrict__ mask, float* __restrict__ pre,
                                                          float* __restrict__ post, int ld_out, float* __restrict__ post2, int ld_out2,
-                                                         int b0, int nb, int N, int K) {
+                                                         int b0, int nb, int N, int K, int bper, long long wstride) {
     __shared__ float sred[8][BT];
     pdl_wait();
     pdl_trigger();
+    b0 += blockIdx.y * bper;                                // grouped: rows of group blockIdx.y, its own weights
+    W += blockIdx.y * wstride;
+    if (bias) bias += blockIdx.y * wstride;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, part = warp & 3;
     const int n = blockIdx.x * 2 + (warp >> 2);
     float acc[BT];
@@ -85,10 +88,13 @@ __global__ void __launch_bounds__(256) linear_fwd_kernel(const float* __restrict
 }
 
 int linear_fwd(const float* x, int ldx, const float* W, int ldw, const float* bias, const float* addend, int ld_add, const float* mask,
-               float* pre, float* post, int ld_out, float* post2, int ld_out2, int B, int N, int K, cudaStream_t st) {
-    for (int b0 = 0; b0 < B; b0 += 8) {
-        int nb = B - b0 < 8 ? B - b0 : 8;
-        DBOA_TRY(launch_ex(linear_fwd_kernel<8>, dim3(ceil_div(N, 2)), dim3(256), 0, st, dim3(1, 1, 1), true, x, ldx, W, ldw, bias, addend, ld_add, mask, pre, post, ld_out, post2, ld_out2, b0, nb, N, K));
+               float* pre, float* post, int ld_out, float* post2, int ld_out2, int B, int N, int K, cudaStream_t st, int groups,
+               long long wstride) {
+    if (groups < 1 || B % groups != 0) return DBOA_ERR_SHAPE;
+    const int bper = B / groups;
+    for (int b0 = 0; b0 < bper; b0 += 8) {
+        int nb = bper - b0 < 8 ? bper - b0 : 8;
+        DBOA_TRY(launch_ex(linear_fwd_kernel<8>, dim3(ceil_div(N, 2), groups), dim3(256), 0, st, dim3(1, 1, 1), true, x, ldx, W, ldw, bias, addend, ld_add, mask, pre, post, ld_out, post2, ld_out2, b0, nb, N, K, bper, wstride));
     }
     return DBOA_OK;
 }
@@ -97,9 +103,12 @@ int linear_fwd(const float* x, int ldx, const float* W, int ldw, const float* bi
 // data gradient: dx[b][k] = sum_n dy[b][n] W[n][k]; grid (ceil(K/256), nsplit), fixed-order reduce
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) linear_dgrad_kernel(const float* __restrict__ dy, int ldy, const float* __restrict__ W, int ldw,
-                                                           float* __restrict__ part, int b0, int nb, int B, int N, int K, int nlen) {
+                                                           float* __restrict__ part, int b0, int nb, int B, int N, int K, int nlen,
+                                                           int bper, long long wstride) {
     pdl_wait();
     pdl_trigger();
+    b0 += blockIdx.z * bper;                                // grouped: rows of group blockIdx.z, its own weights
+    W += blockIdx.z * wstride;
     __shared__ float sdy[8][128];
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     const int nbeg = blockIdx.y * nlen, nend = min(nbeg + nlen, N);
@@ -138,7 +147,9 @@ __global__ void linear_dgrad_reduce_kernel(const float* __restrict__ part, float
 }
 
 int linear_dgrad(const float* dy, int ldy, const float* W, int ldw, float* dx, int ldx, int B, int N, int K, float* ws, size_t ws_floats,
-                 cudaStream_t st) {
+                 cudaStream_t st, int groups, long long wstride) {
+    if (groups < 1 || B % groups != 0) return DBOA_ERR_SHAPE;
+    const int bper = B / groups;
     // 32 rows of W per CTA: at batch 1-3 the kernel is a chain of dependent weight loads, so many short CTAs beat few long ones
     int nsplit = ceil_div(N, 32);
     while (nsplit > 1 && (size_t)nsplit * B * K > ws_floats) nsplit = (nsplit + 1) >> 1;
@@ -146,10 +157,11 @@ int linear_dgrad(const float* dy, int ldy, const float* W, int ldw, float* dx, i
     int nlen = ceil_div(N, nsplit);
     nlen = (nlen + 31) / 32 * 32;
     nsplit = ceil_div(N, nlen);
-    for (int b0 = 0; b0 < B; b0 += 8) {
-        int nb = B - b0 < 8 ? B - b0 : 8;
-        dim3 grid(ceil_div(K, 256), nsplit);
-        DBOA_TRY(launch_ex(linear_dgrad_kernel, dim3(grid), dim3(256), 0, st, dim3(1, 1, 1), true, dy, ldy, W, ldw, ws, b0, nb, B, N, K, nlen));
+    for (int b0 = 0; b0 < bper; b0 += 8) {
+        int nb = bper - b0 < 8 ? bper - b0 : 8;
+        dim3 grid(ceil_div(K, 256), nsplit, groups);
+        DBOA_TRY(launch_ex(linear_dgrad_kernel, dim3(grid), dim3(256), 0, st, dim3(1, 1, 1), true, dy, ldy, W, ldw, ws, b0, nb, B, N, K, nlen,
+                           bper, wstride));
     }
     return launch_ex(linear_dgrad_reduce_kernel, dim3(ceil_div(B * K, 256)), dim3(256), 0, st, dim3(1, 1, 1), true, ws, dx, ldx, B, K, nsplit);
 }
@@ -157,21 +169,35 @@ int linear_dgrad(const float* dy, int ldy, const float* W, int ldw, float* dx, i
 // ---------------------------------------------------------------------------------------------
 // weight gradient: dW[n][k] += sum_r dy[r][n] x[r][k]; db[n] += sum_r dy[r][n]; R <= 32 rows
 // ---------------------------------------------------------------------------------------------
+// Grouped (gridDim.z groups): group g reduces its R rows r -> slab r / bper, row g * bper + r % bper of the slab (bstride rows
+// apart), in order, into its own dW / db.  One group (GROUPED = false): the rows in memory order.
+template <bool GROUPED>
 __global__ void __launch_bounds__(256) linear_wgrad_kernel(const float* __restrict__ dy, int ldy, const float* __restrict__ x, int ldx,
-                                                           float* __restrict__ dW, int ldw, float* __restrict__ db, int R, int N, int K) {
+                                                           float* __restrict__ dW, int ldw, float* __restrict__ db, int R, int N, int K,
+                                                           int bper, int bstride, long long wstride) {
     pdl_wait();
     pdl_trigger();
     __shared__ float sdy[64];
     const int n = blockIdx.y;
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    const int g = blockIdx.z;
+    if (GROUPED) {
+        dW += g * wstride;
+        if (db != nullptr) db += g * wstride;
+    }
+    auto row = [&](int r) {
+        if (!GROUPED) return (size_t)r;
+        const int slab = r / bper;
+        return (size_t)slab * bstride + g * bper + (r - slab * bper);
+    };
     float acc = 0.f, bacc = 0.f;
     for (int r0 = 0; r0 < R; r0 += 64) {
         const int cnt = min(64, R - r0);
         __syncthreads();
-        if (threadIdx.x < cnt) sdy[threadIdx.x] = dy[(size_t)(r0 + threadIdx.x) * ldy + n];
+        if (threadIdx.x < cnt) sdy[threadIdx.x] = dy[row(r0 + threadIdx.x) * ldy + n];
         __syncthreads();
         for (int r = 0; r < cnt; ++r) {
-            if (k < K) acc = fmaf(sdy[r], __ldg(x + (size_t)(r0 + r) * ldx + k), acc);
+            if (k < K) acc = fmaf(sdy[r], __ldg(x + row(r0 + r) * ldx + k), acc);
             bacc += sdy[r];
         }
     }
@@ -179,9 +205,16 @@ __global__ void __launch_bounds__(256) linear_wgrad_kernel(const float* __restri
     if (db != nullptr && blockIdx.x == 0 && threadIdx.x == 0) db[n] += bacc;
 }
 
-int linear_wgrad(const float* dy, int ldy, const float* x, int ldx, float* dW, int ldw, float* db, int R, int N, int K, cudaStream_t st) {
-    dim3 grid(ceil_div(K, 256), N);
-    return launch_ex(linear_wgrad_kernel, dim3(grid), dim3(256), 0, st, dim3(1, 1, 1), true, dy, ldy, x, ldx, dW, ldw, db, R, N, K);
+int linear_wgrad(const float* dy, int ldy, const float* x, int ldx, float* dW, int ldw, float* db, int R, int N, int K, cudaStream_t st,
+                 int groups, int B, long long wstride) {
+    int bper = R, bstride = R, rows = R;
+    if (groups != 1) {
+        if (groups < 1 || B < 1 || B % groups != 0 || R % B != 0) return DBOA_ERR_SHAPE;
+        bper = B / groups; bstride = B; rows = R / groups;
+    }
+    dim3 grid(ceil_div(K, 256), N, groups);
+    return launch_ex(groups > 1 ? linear_wgrad_kernel<true> : linear_wgrad_kernel<false>, dim3(grid), dim3(256), 0, st, dim3(1, 1, 1), true,
+                     dy, ldy, x, ldx, dW, ldw, db, rows, N, K, bper, bstride, wstride);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -6,8 +6,12 @@
 
 namespace dboa {
 
+// Grouped convolutions (several independent videos in one launch): `groups` blocks of B samples each, stored one after the
+// other in the activations; group g uses the weights w + g * wstride (the weight gradient writes dw + g * wstride).
 struct ConvDims {
     int B, Hi, Wi, Cin, Ho, Wo, Cout, kh, kw, stride, pad, Kpitch;
+    int groups = 1;
+    long long wstride = 0;
 };
 
 // ---- conv.cu (fp32 CUDA-core implicit GEMM)
@@ -80,13 +84,18 @@ size_t gn_partial_floats(int B, int HW, int C);     // forward scratch (none; ke
 size_t gn_bwd_partial_floats(int B, int HW, int C); // backward scratch: per-sample dgamma / dbeta rows
 // out = relu?( gn(y) [+ res] ); writes (mean, rstd) to stats[B][4][2]
 // backward: dz = dout * (mask_src > 0 if mask_src else 1); dy = GN backward; dgamma/dbeta accumulate (+=)
+// Grouped (B = groups * bper samples): sample s uses gamma / beta + (s / bper) * pstride.  bper = B: one set for all.
 int gn_fwd_fused(const float* y, const float* gamma, const float* beta, const float* res, float* out, float* stats, float* partial,
-                 int B, int HW, int C, int relu, cudaStream_t st);
+                 int B, int HW, int C, int relu, cudaStream_t st, int bper = 0, long long pstride = 0);
 // defer = 1 (B > 1 only): leave the per-sample dgamma / dbeta rows in `partial` for gn_param_finish instead of reducing them here
+// (required when bper < B: the rows of each group then go to that group's gradient through gn_param_finish)
 int gn_bwd_fused(const float* dout, const float* mask_src, const float* y, const float* stats, const float* gamma, float* dy,
-                 float* dgamma, float* dbeta, float* partial, int B, int HW, int C, cudaStream_t st, int defer = 0);
+                 float* dgamma, float* dbeta, float* partial, int B, int HW, int C, cudaStream_t st, int defer = 0, int bper = 0,
+                 long long pstride = 0);
 struct GnFinishItem { long long g_off, b_off, cum_channels; int C; };
-int gn_param_finish(const GnFinishItem* items_dev, int n_items, const float* rows, float* G, int B, cudaStream_t st);
+// rows of samples [g * B / groups, (g + 1) * B / groups) are added to G + g * pstride
+int gn_param_finish(const GnFinishItem* items_dev, int n_items, const float* rows, float* G, int B, cudaStream_t st, int groups = 1,
+                    long long pstride = 0);
 // ---- norm_pool.cu
 int relu_mask(const float* dout, const float* mask_src, float* dz, size_t n, cudaStream_t st);
 int nchw_to_nhwc(const float* x, float* y, int B, int C, int H, int W, cudaStream_t st);
@@ -97,15 +106,18 @@ int avgpool_fwd(const float* x, float* out, int B, int HW, int C, int ld, int nc
 int avgpool_bwd(const float* dxf, int ld, float* dx, int B, int HW, int C, cudaStream_t st);
 
 // ---- head.cu
+// Grouped variants: B = groups * (B / groups) rows, row b uses W / bias + (b / (B / groups)) * wstride.
 // y[b][n] = (addend ? addend[b][n] : 0) + bias[n] + sum_k x[b][k] W[n][k];  pre <- y (before mask), post <- y*mask
 int linear_fwd(const float* x, int ldx, const float* W, int ldw, const float* bias, const float* addend, int ld_add,
                const float* mask, float* pre, float* post, int ld_out, float* post2, int ld_out2,
-               int B, int N, int K, cudaStream_t st);
+               int B, int N, int K, cudaStream_t st, int groups = 1, long long wstride = 0);
 // dx[b][k] = sum_n dy[b][n] W[n][k] (k < K)
 int linear_dgrad(const float* dy, int ldy, const float* W, int ldw, float* dx, int ldx, int B, int N, int K,
-                 float* ws, size_t ws_floats, cudaStream_t st);
-// dW[n][k] += sum_r dy[r][n] x[r][k];  db[n] += sum_r dy[r][n]
-int linear_wgrad(const float* dy, int ldy, const float* x, int ldx, float* dW, int ldw, float* db, int R, int N, int K, cudaStream_t st);
+                 float* ws, size_t ws_floats, cudaStream_t st, int groups = 1, long long wstride = 0);
+// dW[n][k] += sum_r dy[r][n] x[r][k];  db[n] += sum_r dy[r][n].  The R rows are `R / B` slabs of B rows; group g reduces the
+// rows g * B / groups .. (g + 1) * B / groups - 1 of every slab into dW / db + g * wstride (groups = 1: B is ignored)
+int linear_wgrad(const float* dy, int ldy, const float* x, int ldx, float* dW, int ldw, float* db, int R, int N, int K, cudaStream_t st,
+                 int groups = 1, int B = 0, long long wstride = 0);
 int rot6d_fwd_launch(const float* pose6d, float* rotmat, int n, cudaStream_t st);
 int rot6d_bwd_launch(const float* pose6d, const float* drot, float* dpose, int n, cudaStream_t st);
 int ew_mul(const float* a, const float* b, float* out, size_t n, cudaStream_t st);

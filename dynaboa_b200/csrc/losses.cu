@@ -153,12 +153,22 @@ int gmm_prior_launch(const float* pose69, const float* means, const float* prec,
 // terms: 0 s2d(masked, joints 25..48)  1 shape prior  2 pose prior (value only, from prior_b)
 //        3 target p2d MSE  4 target j3d MSE  5 target beta MSE  6 target R MSE  7 hip-centred 3D
 // ---------------------------------------------------------------------------------------------
+// grouped (a.groups > 1): block g computes video g's terms on its own rows
 __global__ void __launch_bounds__(256) loss_multi_kernel(LossArgs a) {
     pdl_wait();
     pdl_trigger();
     __shared__ float red[32];
     __shared__ float sterm[8];
-    const int t = threadIdx.x, B = a.B;
+    const int B = a.B / gridDim.x;
+    if (gridDim.x > 1) {
+        const size_t r = (size_t)blockIdx.x * B;
+        auto off = [&](auto& p, size_t per_row) { if (p != nullptr) p += r * per_row; };
+        off(a.p2d, 98); off(a.j3d, 147); off(a.R, 216); off(a.beta, 10); off(a.kp, 147); off(a.prior_b, 1); off(a.t_p2d, 98);
+        off(a.t_j3d, 147); off(a.t_beta, 10); off(a.t_R, 216); off(a.gt_s3d, 96); off(a.dp2d, 98); off(a.dj3d, 147); off(a.dR, 216);
+        off(a.dbeta, 10);
+        a.terms += 9 * blockIdx.x;
+    }
+    const int t = threadIdx.x;
     const int kf = a.kp_count > 0 ? a.kp_first : 25, kn = a.kp_count > 0 ? a.kp_count : 24;      // joints of the re-projection term
     float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 
@@ -257,9 +267,10 @@ __global__ void __launch_bounds__(256) loss_multi_kernel(LossArgs a) {
     }
 }
 int loss_multi_launch(const LossArgs& a, cudaStream_t st) {
-    if (a.B < 1 || a.B > 256) return DBOA_ERR_SHAPE;
+    const int groups = a.groups > 1 ? a.groups : 1;
+    if (a.B < 1 || a.B > 256 * groups || a.groups < 0 || a.B % groups != 0) return DBOA_ERR_SHAPE;
     if (a.kp_count < 0 || a.kp_first < 0 || a.kp_first + a.kp_count > 49) return DBOA_ERR_ARG;
-    return launch_ex(loss_multi_kernel, dim3(1), dim3(256), 0, st, dim3(1, 1, 1), true, a);
+    return launch_ex(loss_multi_kernel, dim3(groups), dim3(256), 0, st, dim3(1, 1, 1), true, a);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -273,6 +284,11 @@ __global__ void __launch_bounds__(256) loss_motion_kernel(const float* __restric
     pdl_wait();
     pdl_trigger();
     __shared__ float red[32];
+    B /= gridDim.x;                                          // grouped: block g takes video g's B rows
+    {
+        const size_t r = (size_t)blockIdx.x * B;
+        pa += r * 98; ph += r * 98; ka += r * 147; kh += r * 147; dpa += r * 98; dph += r * 98; term += blockIdx.x;
+    }
     float acc = 0.f;
     const float n = (float)(B * count * 2);
     for (int i = threadIdx.x; i < B * 98; i += 256) {
@@ -292,9 +308,11 @@ __global__ void __launch_bounds__(256) loss_motion_kernel(const float* __restric
     if (threadIdx.x == 0) term[0] = acc / n;
 }
 int loss_motion_launch(const float* pa, const float* ph, const float* ka, const float* kh, float w, float* term, float* dpa, float* dph,
-                       int B, int acc_a, int first, int count, cudaStream_t st) {
+                       int B, int acc_a, int first, int count, cudaStream_t st, int groups) {
     if (first < 0 || count < 1 || first + count > 49) return DBOA_ERR_ARG;
-    return launch_ex(loss_motion_kernel, dim3(1), dim3(256), 0, st, dim3(1, 1, 1), true, pa, ph, ka, kh, w, term, dpa, dph, B, acc_a, first, count);
+    if (groups < 1 || B % groups != 0) return DBOA_ERR_SHAPE;
+    return launch_ex(loss_motion_kernel, dim3(groups), dim3(256), 0, st, dim3(1, 1, 1), true, pa, ph, ka, kh, w, term, dpa, dph, B, acc_a, first,
+                     count);
 }
 
 }  // namespace dboa

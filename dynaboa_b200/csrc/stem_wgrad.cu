@@ -47,6 +47,8 @@ __global__ void __launch_bounds__(NT) stem_wgrad_kernel(const float* __restrict_
     for (int jj = 0; jj < JPT; ++jj) acc[jj] = 0.f;
     pdl_wait();
     pdl_trigger();
+    dy += (size_t)blockIdx.y * B * HO * HO * CO;            // grouped: blockIdx.y is the group, B its samples
+    x += (size_t)blockIdx.y * B * HI * HI * 3;
     const int total_rows = B * HO;
     const int row_begin = blockIdx.x * rows_per_cta, row_end = min(total_rows, row_begin + rows_per_cta);
     for (int row = row_begin; row < row_end; ++row) {
@@ -83,13 +85,16 @@ __global__ void __launch_bounds__(NT) stem_wgrad_kernel(const float* __restrict_
     for (int jj = 0; jj < JPT; ++jj)
         if (jj < nj) outs[co * KK + j0 + jj] = acc[jj];
     __syncthreads();
-    float* dst = part + (size_t)blockIdx.x * (CO * KK);
+    float* dst = part + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * (CO * KK);
     for (int i = tid; i < CO * KK; i += NT) dst[i] = outs[i];
 }
 
-__global__ void __launch_bounds__(256) stem_wgrad_reduce_kernel(const float* __restrict__ part, float* __restrict__ dw, int nparts, int kpitch) {
+__global__ void __launch_bounds__(256) stem_wgrad_reduce_kernel(const float* __restrict__ part, float* __restrict__ dw, int nparts, int kpitch,
+                                                                long long wstride) {
     pdl_wait();
     pdl_trigger();
+    part += (size_t)blockIdx.y * nparts * (CO * KK);          // grouped: group blockIdx.y's partials into its own gradient
+    dw += blockIdx.y * wstride;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= CO * KK) return;
     float s0 = 0.f, s1 = 0.f;
@@ -109,14 +114,14 @@ bool stem_wgrad_ok(const ConvDims& d) {
 
 int stem_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, float* ws, size_t ws_floats, cudaStream_t st) {
     if (!stem_wgrad_ok(d)) return DBOA_ERR_UNSUPPORTED;
-    const int rows = d.B * stem::HO;
-    const int max_parts = (int)std::min<size_t>(2 * num_sms(), ws_floats / (stem::CO * stem::KK));
+    const int rows = d.B * stem::HO;                     // per group
+    const int max_parts = (int)std::min<size_t>(2 * num_sms(), ws_floats / (stem::CO * stem::KK)) / std::max(d.groups, 1);
     if (ws == nullptr || max_parts < 1) return DBOA_ERR_UNSUPPORTED;
     const int rows_per = ceil_div(rows, max_parts), nparts = ceil_div(rows, rows_per);
-    DBOA_TRY(launch_ex(stem::stem_wgrad_kernel, dim3(nparts), dim3(stem::NT), (size_t)stem::SMEM_FLOATS * sizeof(float), st, dim3(1, 1, 1), true,
-                       dy, x, ws, d.B, rows_per));
-    return launch_ex(stem::stem_wgrad_reduce_kernel, dim3(ceil_div(stem::CO * stem::KK, 256)), dim3(256), 0, st, dim3(1, 1, 1), true,
-                     (const float*)ws, dw, nparts, d.Kpitch);
+    DBOA_TRY(launch_ex(stem::stem_wgrad_kernel, dim3(nparts, d.groups), dim3(stem::NT), (size_t)stem::SMEM_FLOATS * sizeof(float), st, dim3(1, 1, 1),
+                       true, dy, x, ws, d.B, rows_per));
+    return launch_ex(stem::stem_wgrad_reduce_kernel, dim3(ceil_div(stem::CO * stem::KK, 256), d.groups), dim3(256), 0, st, dim3(1, 1, 1), true,
+                     (const float*)ws, dw, nparts, d.Kpitch, d.wstride);
 }
 
 }  // namespace dboa

@@ -144,12 +144,23 @@ def scratch_for(B, device):
     return _SCRATCH[key]
 
 
-def raw_forward(arena, buffers, image, masks=None, tape=None):
-    """One ``dboa_hmr_forward`` call.  Returns (rotmat, shape, cam, pose6d, tape).  No autograd."""
+def _check_groups(arena, B, groups):
+    if groups < 1 or B % groups:
+        raise ValueError(f'{B} samples do not split into {groups} videos')
+    if groups > 1 and (not arena.is_contiguous() or arena.numel() != groups * layout().floats):
+        raise ValueError(f'a grouped call needs one contiguous ({groups}, {layout().floats}) arena stack')
+
+
+def raw_forward(arena, buffers, image, masks=None, tape=None, groups=1):
+    """One ``dboa_hmr_forward`` call.  Returns (rotmat, shape, cam, pose6d, tape).  No autograd.
+
+    ``groups`` > 1 runs ``dboa_hmr_forward_groups``: ``arena`` is a (groups, P) stack, and video g's weights ``arena[g]`` see
+    the samples [g * B / groups, (g + 1) * B / groups) of ``image`` (and of ``masks`` and the outputs)."""
     _lib.require_cuda(arena, image)
     B = image.shape[0]
     if tuple(image.shape[1:]) != (3, 224, 224):
         raise ValueError(f'HMR expects (B,3,224,224) images, got {tuple(image.shape)}')
+    _check_groups(arena, B, groups)
     image = image.contiguous().float()
     dev = image.device
     if tape is None:
@@ -162,18 +173,28 @@ def raw_forward(arena, buffers, image, masks=None, tape=None):
         masks = masks.contiguous().float()
         if tuple(masks.shape) != (3, 2, B, 1024):
             raise ValueError('dropout masks must be (3,2,B,1024)')
-    _lib.call('dboa_hmr_forward', ptr(arena), ptr(buffers['init_pose']), ptr(buffers['init_shape']), ptr(buffers['init_cam']),
-              ptr(image), B, ptr(masks), ptr(tape), ptr(scratch_for(B, dev)), ptr(rot), ptr(shape), ptr(cam), ptr(pose6d),
-              stream())
+    args = (ptr(arena), ptr(buffers['init_pose']), ptr(buffers['init_shape']), ptr(buffers['init_cam']), ptr(image), B, ptr(masks),
+            ptr(tape), ptr(scratch_for(B, dev)), ptr(rot), ptr(shape), ptr(cam), ptr(pose6d), stream())
+    if groups == 1:
+        _lib.call('dboa_hmr_forward', *args)
+    else:
+        _lib.call('dboa_hmr_forward_groups', *args, groups)
     return rot, shape, cam, pose6d, tape
 
 
-def raw_backward(arena, tape, B, masked, d_rot, d_shape, d_cam, grad_arena):
-    """One ``dboa_hmr_backward`` call: accumulates into ``grad_arena`` (flat, arena layout)."""
+def raw_backward(arena, tape, B, masked, d_rot, d_shape, d_cam, grad_arena, groups=1):
+    """One ``dboa_hmr_backward`` call: accumulates into ``grad_arena`` (flat, arena layout).  ``groups`` > 1: the grouped
+    backward, with ``arena`` and ``grad_arena`` both (groups, P) stacks (see ``raw_forward``)."""
+    _check_groups(arena, B, groups)
+    _check_groups(grad_arena, B, groups)
     c = lambda t: None if t is None else t.contiguous().float()
     d_rot, d_shape, d_cam = c(d_rot), c(d_shape), c(d_cam)
-    _lib.call('dboa_hmr_backward', ptr(arena), ptr(tape), B, int(masked), ptr(d_rot), ptr(d_shape), ptr(d_cam), ptr(grad_arena),
-              ptr(scratch_for(B, tape.device)), stream())
+    args = (ptr(arena), ptr(tape), B, int(masked), ptr(d_rot), ptr(d_shape), ptr(d_cam), ptr(grad_arena), ptr(scratch_for(B, tape.device)),
+            stream())
+    if groups == 1:
+        _lib.call('dboa_hmr_backward', *args)
+    else:
+        _lib.call('dboa_hmr_backward_groups', *args, groups)
 
 
 class _HMRFunction(torch.autograd.Function):

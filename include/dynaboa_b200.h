@@ -42,6 +42,7 @@ int dboa_get_fused_forward(void);
 /* the same switch for dboa_hmr_backward: 1 = fused data-gradient chain (GroupNorm backward on load), 0 (default) =
  * GroupNorm-backward and data-gradient launches per layer.  Environment: DBOA_FUSED_BWD. */
 int dboa_set_fused_backward(int enable);
+int dboa_get_fused_backward(void);
 
 /* ---- HMR regressor: parameter arena and tape layout ----------------------------------------
  * replaces: model/hmr.py:67-124 (HMR.__init__/_make_layer state_dict contract).
@@ -88,6 +89,20 @@ int dboa_hmr_forward(const float* arena, const float* init_pose, const float* in
 int dboa_hmr_backward(const float* arena, const float* tape, int B, int masked /* forward used drop_masks */,
                       const float* d_rotmat, const float* d_shape, const float* d_cam, float* grad_arena, float* scratch,
                       dboa_stream_t stream);
+/* Several independent videos in one launch sequence: the two calls above for `groups` videos of B / groups samples each.
+ * Video g owns the consecutive samples [g * B / groups, (g + 1) * B / groups) of every per-sample buffer (image, masks, outputs,
+ * d_* inputs; the tape and scratch are those of batch B) and the weights arena + g * dboa_hmr_arena_floats(); the backward
+ * accumulates into grad_arena + g * dboa_hmr_arena_floats().  Each video's arithmetic is the single-video plan's (the split-K
+ * slicing of a convolution may differ, since it is sized for all groups' tiles).  groups = 1 is exactly dboa_hmr_forward /
+ * dboa_hmr_backward.  Checked before any device access: DBOA_ERR_SHAPE for groups < 1, B outside 1..64 or B % groups != 0;
+ * DBOA_ERR_UNSUPPORTED for groups > 1 while the fused forward or backward plan is selected, and (backward) while
+ * dboa_hmr_backward_buckets is armed.  A grouped backward call (groups != 1) always consumes an armed bucket request. */
+int dboa_hmr_forward_groups(const float* arena, const float* init_pose, const float* init_shape, const float* init_cam,
+                            const float* image, int B, const float* drop_masks, float* tape, float* scratch,
+                            float* rotmat, float* shape, float* cam, float* pose6d, dboa_stream_t stream, int groups);
+int dboa_hmr_backward_groups(const float* arena, const float* tape, int B, int masked, const float* d_rotmat,
+                             const float* d_shape, const float* d_cam, float* grad_arena, float* scratch, dboa_stream_t stream,
+                             int groups);
 
 /* Gradient buckets of the NEXT dboa_hmr_backward call, for overlapping the data-parallel all-reduce with the backward
  * (SURVEY.md section 8e).  Bucket k spans the floats [dboa_hmr_bucket_offset(k), dboa_hmr_bucket_offset(k - 1)) of the gradient
@@ -230,6 +245,9 @@ typedef struct dboa_loss_args {
     int kp_first, kp_count;                 /* joints [kp_first, kp_first + kp_count) of the 49 carry the 2D re-projection term; 0, 0 = the
                                                benchmark's 24 ground-truth joints (25, 24); the webcam client compares the 25 OpenPose
                                                joints (0, 25), reference dynaboa_webcam.py:236,246,262 */
+    int groups;                             /* 0 or 1: one learner.  G > 1: B = G * b rows of G independent videos (video g: rows
+                                               [g b, (g+1) b) of every per-row buffer); means, gradient scaling and prior_b sums are
+                                               per video and `terms` is (G, 9).  B % G must be 0 */
 } dboa_loss_args;
 int dboa_loss_multi(const dboa_loss_args* args, dboa_stream_t stream);        /* :234-241,283-291,331-337,360-370,401,412-422 */
 int dboa_loss_motion(const float* p_cur, const float* p_hist, const float* kp_cur, const float* kp_hist, float weight, float* term,
@@ -237,6 +255,10 @@ int dboa_loss_motion(const float* p_cur, const float* p_hist, const float* kp_cu
 /* the same on joints [first, first + count): reference dynaboa_webcam.py:161-181 uses the 25 OpenPose joints (0, 25) */
 int dboa_loss_motion_joints(const float* p_cur, const float* p_hist, const float* kp_cur, const float* kp_hist, float weight, float* term,
                             float* dp_cur, float* dp_hist, int B, int accumulate_cur, int first, int count, dboa_stream_t stream);
+/* the same for `groups` independent videos of B / groups rows each: the mean is per video and term is (groups,) */
+int dboa_loss_motion_groups(const float* p_cur, const float* p_hist, const float* kp_cur, const float* kp_hist, float weight, float* term,
+                            float* dp_cur, float* dp_hist, int B, int accumulate_cur, int first, int count, int groups,
+                            dboa_stream_t stream);
 
 /* ---- whole-model sweeps, feature test, retrieval -------------------------------------------- */
 int dboa_sgd_update(const float* p, const float* g, float* out, float lr, long long n, dboa_stream_t stream);   /* l2l maml_update */
