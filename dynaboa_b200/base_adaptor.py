@@ -95,14 +95,9 @@ class BaseAdaptor:
 
     def retrieval(self, feature):
         """reference :82-96: nearest cluster centre by cosine distance, then ``random.sample`` inside it."""
-        f = feature.detach().reshape(-1)[:2048].contiguous()
-        _lib.call('dboa_retrieval_nearest', ptr(f), ptr(self.centers), self.centers.shape[0], 2048, ptr(self._best), ptr(self._dists),
-                  stream())
-        cluster = int(self._best.item())
-        picks = random.sample(self.index[cluster], self.options.sample_num)
-        self.last_retrieval = (cluster, picks)
-        idx = torch.as_tensor(picks, dtype=torch.long, device=self.device)
-        return {k: v.index_select(0, idx) for k, v in self.h36m_bank.items()}
+        from .fused import retrieve
+        (self.last_retrieval,), batch = retrieve(self, feature.detach().reshape(1, -1)[:, :2048], [random])
+        return batch
 
     def set_model_optim(self):
         checkpoint = torch.load(self.options.model_file, map_location='cpu', weights_only=False)

@@ -11,9 +11,14 @@ What changes relative to the autograd path (``Adaptor.adaptation``), none of it 
   applied to theta (SURVEY.md "facts": ``first_order=True``);
 * Adam and the mean-teacher EMA run as one fused sweep; frame and teacher-consistency terms share one loss-head
   launch; the only host syncs are retrieval's cluster index and the ``dynamic_boa`` decision.
+
+The same step adapts G videos at once (``multivideo.MultiVideoAdaptor``): their weight, teacher and gradient arenas are
+(G, P) stacks instead of flat arenas, video g owns the rows [g * b, (g + 1) * b) of every batch, and every network pass and
+loss head is one grouped call.  DESIGN.md section 10.
 """
 import ctypes as C
 import os
+import random
 
 import torch
 
@@ -40,9 +45,14 @@ def _mark(ad, name):
         ev_list.append((name, ev))
 
 
+def _groups(arena):
+    """Videos of a weight arena: one for a flat arena, G for a (G, P) stack."""
+    return arena.shape[0] if arena.dim() == 2 else 1
+
+
 class _Pred:
     """Everything one forward graph produces (kept for its backward)."""
-    __slots__ = ('image', 'rot', 'shape', 'cam', 'tape', 'verts', 'joints', 'smpl_tape', 'p2d', 'B', 'masked')
+    __slots__ = ('image', 'rot', 'shape', 'cam', 'tape', 'verts', 'joints', 'smpl_tape', 'p2d', 'B', 'masked', 'groups')
 
 
 def _smpl_fwd(smpl, betas, rot):
@@ -56,8 +66,8 @@ def _smpl_fwd(smpl, betas, rot):
 
 def forward_graph(ad, arena, buffers, image, masks=None):
     p = _Pred()
-    p.image, p.B, p.masked = image, image.shape[0], masks is not None
-    p.rot, p.shape, p.cam, _, p.tape = hmr_mod.raw_forward(arena, buffers, image, masks)
+    p.image, p.B, p.masked, p.groups = image, image.shape[0], masks is not None, _groups(arena)
+    p.rot, p.shape, p.cam, _, p.tape = hmr_mod.raw_forward(arena, buffers, image, masks, groups=p.groups)
     p.verts, p.joints, p.smpl_tape = _smpl_fwd(ad.smpl_neutral, p.shape, p.rot)
     p.p2d = torch.empty(p.B, 49, 2, dtype=torch.float32, device=image.device)
     _lib.call('dboa_project_fwd', ptr(p.cam), ptr(p.joints), ptr(p.p2d), p.B, 49, stream())
@@ -65,24 +75,24 @@ def forward_graph(ad, arena, buffers, image, masks=None):
 
 
 def _loss_head(ad, p, w, kp=None, t_p2d=None, t_j3d=None, t_beta=None, t_R=None, gt_s3d=None, grads=None, nb=None):
-    """Runs the (optional) pose prior and the multi-term head on the first ``nb`` samples of ``p``; returns
-    (terms[9], dp2d, dj3d, dR, dbeta).  ``grads``: preallocated (possibly larger-batch) gradient buffers whose leading
-    ``nb`` rows are written."""
-    B, dev = (p.B if nb is None else nb), p.rot.device
+    """Runs the (optional) pose prior and the multi-term head on the first ``nb`` samples of ``p``, each video's rows on their
+    own (per-video means and gradient scaling); returns (terms (G, 9), dp2d, dj3d, dR, dbeta).  ``grads``: preallocated
+    (possibly larger-batch) gradient buffers whose leading ``nb`` rows are written."""
+    B, dev, G = (p.B if nb is None else nb), p.rot.device, p.groups
     if grads is None:
         dp2d, dj3d = torch.empty_like(p.p2d), torch.empty_like(p.joints)
         dR, dbeta = torch.empty_like(p.rot), torch.empty_like(p.shape)
     else:
         dp2d, dj3d, dR, dbeta = grads
-    terms = torch.empty(9, dtype=torch.float32, device=dev)
+    terms = torch.empty(G, 9, dtype=torch.float32, device=dev)
     prior_b = None
     if w[2] != 0.0:
         prior_b = torch.empty(B, dtype=torch.float32, device=dev)
         g = ad.gmm_f
         _lib.call('dboa_pose_prior', ptr(p.rot), ptr(g.means), ptr(g.precisions), ptr(g.neg_log_weights), ptr(prior_b), ptr(dR),
-                  float(w[2]) / B, B, stream())
+                  float(w[2]) / (B // G), B, stream())                   # per-video mean: scale w / b
     a = _lib.LossArgsStruct()
-    a.B = B
+    a.B, a.groups = B, G
     keep = []
     for name, t in (('p2d', p.p2d), ('j3d', p.joints), ('R', p.rot), ('beta', p.shape), ('kp', kp), ('prior_b', prior_b), ('t_p2d', t_p2d),
                     ('t_j3d', t_j3d), ('t_beta', t_beta), ('t_R', t_R), ('gt_s3d', gt_s3d), ('terms', terms), ('dp2d', dp2d),
@@ -116,42 +126,56 @@ def backward_graph(ad, arena, p, dp2d, dj3d, dR, dbeta, grad_arena, sync=None):
               ptr(dbeta), 1, stream())
     if sync is not None:
         sync.arm()
-    hmr_mod.raw_backward(arena, p.tape, B, p.masked, dR, dbeta, dcam, grad_arena)
+    hmr_mod.raw_backward(arena, p.tape, B, p.masked, dR, dbeta, dcam, grad_arena, groups=p.groups)
     if sync is not None:
         sync.after_backward(grad_arena)
         ad.optimizer.reduced = True
 
 
+def retrieve(ad, rows, rngs):
+    """reference :82-96 for every video: the nearest cluster centre of video g's feature row ``rows[g]`` by cosine distance
+    (one host synchronisation for all videos), then ``rngs[g].sample`` inside that cluster.  Returns the (cluster, picks) of
+    every video and the picked exemplar rows, video after video."""
+    for g, f in enumerate(rows):
+        f = f.contiguous()
+        _lib.call('dboa_retrieval_nearest', ptr(f), ptr(ad.centers), ad.centers.shape[0], 2048, C.c_void_p(ad._best.data_ptr() + 4 * g),
+                  ptr(ad._dists), stream())
+    picked = [(c, rng.sample(ad.index[c], ad.options.sample_num)) for c, rng in zip(ad._best.tolist(), rngs)]
+    idx = torch.as_tensor([i for _, picks in picked for i in picks], dtype=torch.long, device=rows.device)
+    return picked, {k: v.index_select(0, idx) for k, v in ad.h36m_bank.items()}
+
+
 def level_backward(ad, arena, buffers, image, kp, lower, grad_arena, main=None, sync=None):
-    """One level of the bilevel problem (reference base_adaptor.py:222-317) on weights ``arena``: evaluates the
-    level's loss and accumulates its gradient into ``grad_arena`` (``sync``: data-parallel bucketed all-reduce to attach to
-    the last graph of the level).  ``main`` is an already computed forward of
-    ``image`` with these weights (re-used when given).  When the motion loss is live and no forward is supplied,
-    the current and the history frame go through ONE batched forward / backward (same weights, independent
-    samples).  Returns (loss as a device scalar, the forward whose first rows belong to ``image``)."""
+    """One level of the bilevel problem (reference base_adaptor.py:222-317) on weights ``arena``, a flat arena or a (G, P)
+    stack of G videos' arenas: evaluates the level's loss of every video and accumulates its gradient into ``grad_arena``
+    (same layout; ``sync``: data-parallel bucketed all-reduce to attach to the last graph of the level).  ``main`` is an
+    already computed forward of ``image`` with these weights (re-used when given).  Returns (the loss, a device scalar for
+    a flat arena and (G,) for a stack; the forward whose first rows belong to ``image``).
+
+    With one video, when the motion loss is live and no forward is supplied, the current and the history frame go through
+    ONE batched forward / backward (same weights, independent samples), and the teacher forward runs on a side stream.
+    With several, the history frame gets its own grouped pass and the teacher runs on the caller's stream."""
     o = ad.options
     tag = 'll' if lower else 'ul'
     nb = image.shape[0]
+    G = _groups(arena)
+    per_video = arena.shape[:-1]                                # shape of the losses recorded and returned: () or (G,)
     use_frame = o.use_frame_losses_lower if lower else o.use_frame_losses_upper
     use_temporal = o.use_temporal_losses_lower if lower else o.use_temporal_losses_upper
     motion = bool(use_temporal and o.use_motion and (ad.global_step - o.interval) > 0)
-    hist = None
     # the teacher forward is independent of the fast-weight forward: issue it on a side stream so that the two chains
     # of small, latency-bound kernels overlap on the GPU (each one alone leaves most SMs idle at batch 1)
     tpred, side = None, None
     if use_temporal and o.use_meanteacher:
         teacher = ad.teacher
-        if _TEACHER_OVERLAP:
-            cur = torch.cuda.current_stream()
+        if _TEACHER_OVERLAP and G == 1:
             side = _side_stream(image.device)
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):
-                tpred = forward_graph(ad, teacher.arena, teacher._buffers, image, teacher._masks(nb, image.device))
-        else:
+            side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):                           # None: the caller's stream
             tpred = forward_graph(ad, teacher.arena, teacher._buffers, image, teacher._masks(nb, image.device))
     if motion:
         hist_image, hist_kp = ad.get_hist()
-        if main is None:
+        if main is None and G == 1:
             pair = getattr(ad, '_pair', None)                   # persistent (2 nb, 3, 224, 224) staging: rows [nb:] = history frame
             if pair is None or pair.shape[0] != 2 * nb or pair.device != image.device:
                 pair = ad._pair = torch.empty(2 * nb, 3, 224, 224, dtype=torch.float32, device=image.device)
@@ -159,10 +183,10 @@ def level_backward(ad, arena, buffers, image, kp, lower, grad_arena, main=None, 
             _lib.call('dboa_copy_async', ptr(pair), ptr(image), half, stream())
             _lib.call('dboa_copy_async', C.c_void_p(pair.data_ptr() + half), ptr(hist_image.contiguous()), half, stream())
             main = forward_graph(ad, arena, buffers, pair)
-        else:
-            hist = forward_graph(ad, arena, buffers, hist_image)
-    elif main is None:
+    if main is None:
         main = forward_graph(ad, arena, buffers, image)
+    batched = main.B > nb
+    hist = forward_graph(ad, arena, buffers, hist_image) if motion and not batched else None
     w = [0.0] * 8
     targets = {}
     if use_frame:
@@ -178,7 +202,6 @@ def level_backward(ad, arena, buffers, image, kp, lower, grad_arena, main=None, 
         w[3], w[4], w[5], w[6] = 5 * tw, 5 * tw, 0.001 * tw, 1 * tw
         targets = dict(t_p2d=t.p2d, t_j3d=t.joints, t_beta=t.shape, t_R=t.rot)
     _mark(ad, f'{tag}: forward(s) issued')
-    batched = main.B > nb
     grads = None
     if batched:                                                 # gradients of the 2 nb rows in ONE zeroed buffer (rows [nb:] only get the motion term)
         Bm = main.B
@@ -190,29 +213,32 @@ def level_backward(ad, arena, buffers, image, kp, lower, grad_arena, main=None, 
         e = [0, sizes[0], sizes[0] + sizes[1], sizes[0] + sizes[1] + sizes[2]]
         grads = (flat[e[0]:e[1]].view(Bm, 49, 2), flat[e[1]:e[2]].view(Bm, 49, 3), flat[e[2]:e[3]].view(Bm, 24, 3, 3), flat[e[3]:].view(Bm, 10))
     terms, dp2d, dj3d, dR, dbeta = _loss_head(ad, main, w, kp=kp if use_frame else None, grads=grads, nb=nb, **targets)
-    total = terms[8]
+    terms = terms.view(*per_video, 9)
+    total = terms[..., 8]
     if use_frame:
-        ad.fit_losses[f'{tag}/s2dloss'], ad.fit_losses[f'{tag}/shape_prior'], ad.fit_losses[f'{tag}/pose_prior'] = terms[0], terms[1], terms[2]
-        (ad.kp2dlosses_lower.append(terms[0]) if lower else ad.kp2dlosses_upper.__setitem__(ad.global_step, terms[0]))
+        ad.fit_losses[f'{tag}/s2dloss'], ad.fit_losses[f'{tag}/shape_prior'], ad.fit_losses[f'{tag}/pose_prior'] = terms[..., 0], terms[..., 1], terms[..., 2]
+        (ad.kp2dlosses_lower.append(terms[..., 0]) if lower else ad.kp2dlosses_upper.__setitem__(ad.global_step, terms[..., 0]))
     if motion:
-        mterm = torch.empty(1, dtype=torch.float32, device=image.device)
+        mterm = torch.empty(per_video, dtype=torch.float32, device=image.device)
         p_hist = main.p2d[nb:] if batched else hist.p2d
         dph = dp2d[nb:] if batched else torch.empty_like(hist.p2d)
         kf, kn = getattr(ad, 'kp_range', (25, 24))
-        _lib.call('dboa_loss_motion_joints', ptr(main.p2d), ptr(p_hist), ptr(kp), ptr(hist_kp.contiguous()), float(o.motionloss_weight),
-                  ptr(mterm), ptr(dp2d), ptr(dph), nb, 1, kf, kn, stream())
+        _lib.call('dboa_loss_motion_groups', ptr(main.p2d), ptr(p_hist), ptr(kp), ptr(hist_kp.contiguous()), float(o.motionloss_weight),
+                  ptr(mterm), ptr(dp2d), ptr(dph), nb, 1, kf, kn, G, stream())
         if not batched:
             backward_graph(ad, arena, hist, dph, torch.zeros_like(hist.joints), torch.zeros_like(hist.rot), torch.zeros_like(hist.shape),
                            grad_arena)
-        total = total + mterm[0] * o.motionloss_weight
-        ad.fit_losses['ul/motion_loss'] = mterm[0]
+        total = total + mterm * o.motionloss_weight
+        ad.fit_losses['ul/motion_loss'] = mterm
     _mark(ad, f'{tag}: loss head')
     mix = bool(o.retrieval and (o.lower_level_mixtrain if lower else o.upper_level_mixtrain))
     backward_graph(ad, arena, main, dp2d, dj3d, dR, dbeta, grad_arena, sync=None if mix else sync)
     _mark(ad, f'{tag}: backward')
     if o.retrieval:
-        ex = ad.retrieval(hmr_mod._feature_views(main.tape, main.B)[5][:nb])
-        if (o.lower_level_mixtrain if lower else o.upper_level_mixtrain):
+        rows = hmr_mod._feature_views(main.tape, main.B)[5][:nb].reshape(G, -1, 2048)[:, 0]      # each video's first sample
+        picked, ex = retrieve(ad, rows, getattr(ad, 'rngs', [random]))
+        ad.last_retrieval = picked if per_video else picked[0]
+        if mix:
             e = forward_graph(ad, arena, buffers, ex['img'])
             n = e.B
             gt_R = torch.empty(n, 24, 3, 3, dtype=torch.float32, device=image.device)
@@ -221,8 +247,9 @@ def level_backward(ad, arena, buffers, image, kp, lower, grad_arena, main=None, 
             eterms, a, b, c, d = _loss_head(ad, e, [5 * lw, 0, 0, 0, 0, 0.001 * lw, 1 * lw, 5 * lw], kp=ex['keypoints'], t_beta=ex['betas'],
                                             t_R=gt_R, gt_s3d=ex['pose_3d'])
             backward_graph(ad, arena, e, a, b, c, d, grad_arena, sync=sync)
-            total = total + eterms[8]
-            ad.fit_losses[f'{tag}/labled_loss'] = eterms[8]
+            eterms = eterms.view(*per_video, 9)
+            total = total + eterms[..., 8]
+            ad.fit_losses[f'{tag}/labled_loss'] = eterms[..., 8]
     return total, main
 
 
@@ -232,13 +259,19 @@ def feature_cosines(ad, tape_a, tape_b, B):
 
 
 def fused_adapt(ad, batch):
+    """One adapted frame (reference dynaboa_benchmark.py:126-201) of every video of ``ad``: probe forward, ``inner_step`` SGD
+    steps of the lower level, the upper level, one Adam + EMA teacher sweep, then the optional ``dynamic_boa`` loop.
+
+    Reads from ``ad``: ``model`` (``arena``, ``_buffers``, ``grad_arena()``), ``teacher`` (``arena``, ``_buffers``,
+    ``_masks(B, device)``) and ``optimizer`` (``step(teacher=, alpha=)``, ``grad_sync``), whose arenas are flat for one video
+    and (G, P) stacks for G videos; ``save_hist`` / ``get_hist``; ``global_step``; the records the level writes."""
     o = ad.options
     image, kp = batch['image'].contiguous().float(), batch['smpl_j2d'].contiguous().float()
     ad.save_hist(image, kp)
     model = getattr(ad.model, 'module', ad.model)
     theta, buffers = model.arena, model._buffers
     opt = ad.optimizer
-    G = model.grad_arena()
+    grad = model.grad_arena()
     teacher = ad.teacher if o.use_meanteacher else None
     evaluate = getattr(ad, 'fused_eval', 'final')
     with torch.no_grad():
@@ -248,8 +281,8 @@ def fused_adapt(ad, batch):
         import torch.distributed as tdist
         sync = opt.grad_sync if (opt.grad_sync is not None and tdist.is_initialized() and tdist.get_world_size() > 1) else None
         if not o.use_boa:
-            _zero(G)
-            ad.last_upper_loss, _ = level_backward(ad, theta, buffers, image, kp, True, G, main=probe, sync=sync)
+            _zero(grad)
+            ad.last_upper_loss, _ = level_backward(ad, theta, buffers, image, kp, True, grad, main=probe, sync=sync)
             opt.step()
             return ad.inference(batch, ad.model) if evaluate != 'none' else None
         fast, cur = theta, probe
@@ -266,8 +299,8 @@ def fused_adapt(ad, batch):
             _mark(ad, 'inner SGD step')
             if evaluate == 'all':
                 ad.inference(batch, _ArenaModel(model, fast))
-        _zero(G)
-        ad.last_upper_loss, _ = level_backward(ad, fast, buffers, image, kp, False, G, sync=sync)
+        _zero(grad)
+        ad.last_upper_loss, _ = level_backward(ad, fast, buffers, image, kp, False, grad, sync=sync)
         _mark(ad, 'upper level (forward + loss + backward)')
         opt.step(teacher=teacher, alpha=o.alpha)                    # Adam + EMA teacher, one sweep
         _mark(ad, 'Adam + EMA')
@@ -283,8 +316,8 @@ def fused_adapt(ad, batch):
                 steps += 1
                 if steps > o.optim_steps:
                     break
-                _zero(G)
-                level_backward(ad, theta, buffers, image, kp, False, G, main=after, sync=sync)   # 'after' was computed with the current theta
+                _zero(grad)
+                level_backward(ad, theta, buffers, image, kp, False, grad, main=after, sync=sync)   # 'after' was computed with the current theta
                 opt.step(teacher=teacher, alpha=o.alpha)
                 before, after = after, forward_graph(ad, theta, buffers, image)
                 sims = feature_cosines(ad, before.tape, after.tape, probe.B)

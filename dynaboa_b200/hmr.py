@@ -152,10 +152,10 @@ def _check_groups(arena, B, groups):
 
 
 def raw_forward(arena, buffers, image, masks=None, tape=None, groups=1):
-    """One ``dboa_hmr_forward`` call.  Returns (rotmat, shape, cam, pose6d, tape).  No autograd.
+    """One ``dboa_hmr_forward_groups`` call.  Returns (rotmat, shape, cam, pose6d, tape).  No autograd.
 
-    ``groups`` > 1 runs ``dboa_hmr_forward_groups``: ``arena`` is a (groups, P) stack, and video g's weights ``arena[g]`` see
-    the samples [g * B / groups, (g + 1) * B / groups) of ``image`` (and of ``masks`` and the outputs)."""
+    ``groups`` > 1: ``arena`` is a (groups, P) stack, and video g's weights ``arena[g]`` see the samples
+    [g * B / groups, (g + 1) * B / groups) of ``image`` (and of ``masks`` and the outputs)."""
     _lib.require_cuda(arena, image)
     B = image.shape[0]
     if tuple(image.shape[1:]) != (3, 224, 224):
@@ -173,28 +173,20 @@ def raw_forward(arena, buffers, image, masks=None, tape=None, groups=1):
         masks = masks.contiguous().float()
         if tuple(masks.shape) != (3, 2, B, 1024):
             raise ValueError('dropout masks must be (3,2,B,1024)')
-    args = (ptr(arena), ptr(buffers['init_pose']), ptr(buffers['init_shape']), ptr(buffers['init_cam']), ptr(image), B, ptr(masks),
-            ptr(tape), ptr(scratch_for(B, dev)), ptr(rot), ptr(shape), ptr(cam), ptr(pose6d), stream())
-    if groups == 1:
-        _lib.call('dboa_hmr_forward', *args)
-    else:
-        _lib.call('dboa_hmr_forward_groups', *args, groups)
+    _lib.call('dboa_hmr_forward_groups', ptr(arena), ptr(buffers['init_pose']), ptr(buffers['init_shape']), ptr(buffers['init_cam']),
+              ptr(image), B, ptr(masks), ptr(tape), ptr(scratch_for(B, dev)), ptr(rot), ptr(shape), ptr(cam), ptr(pose6d), stream(), groups)
     return rot, shape, cam, pose6d, tape
 
 
 def raw_backward(arena, tape, B, masked, d_rot, d_shape, d_cam, grad_arena, groups=1):
-    """One ``dboa_hmr_backward`` call: accumulates into ``grad_arena`` (flat, arena layout).  ``groups`` > 1: the grouped
-    backward, with ``arena`` and ``grad_arena`` both (groups, P) stacks (see ``raw_forward``)."""
+    """One ``dboa_hmr_backward_groups`` call: accumulates into ``grad_arena`` (flat, arena layout).  ``groups`` > 1: ``arena``
+    and ``grad_arena`` are both (groups, P) stacks (see ``raw_forward``)."""
     _check_groups(arena, B, groups)
     _check_groups(grad_arena, B, groups)
     c = lambda t: None if t is None else t.contiguous().float()
     d_rot, d_shape, d_cam = c(d_rot), c(d_shape), c(d_cam)
-    args = (ptr(arena), ptr(tape), B, int(masked), ptr(d_rot), ptr(d_shape), ptr(d_cam), ptr(grad_arena), ptr(scratch_for(B, tape.device)),
-            stream())
-    if groups == 1:
-        _lib.call('dboa_hmr_backward', *args)
-    else:
-        _lib.call('dboa_hmr_backward_groups', *args, groups)
+    _lib.call('dboa_hmr_backward_groups', ptr(arena), ptr(tape), B, int(masked), ptr(d_rot), ptr(d_shape), ptr(d_cam), ptr(grad_arena),
+              ptr(scratch_for(B, tape.device)), stream(), groups)
 
 
 class _HMRFunction(torch.autograd.Function):

@@ -2,7 +2,7 @@
 (rank 0, the golden stream) is held to tests/golden/adapt_{c2,c3}.npz directly; videos 1..3 to their own single-video
 ``Adaptor.adapt`` runs given the same teacher masks and retrieval picks.  Criteria of test_gpu_adapt.run_and_compare: upper
 loss within 1e-3 (2e-4 on the first frame against the golden), outputs within 1e-3, theta within 4 * lr * n_outer.  Two
-grouped runs give bit-identical theta."""
+grouped runs give bit-identical theta, and one video takes the single-video schedule bit for bit."""
 import ast
 import random
 
@@ -29,10 +29,10 @@ def seed_for(g, t):
     return 1000 + t if g == 0 else 1000 * (g + 1) + t
 
 
-def grouped(opts, gd):
+def grouped(opts, gd, n_videos=G):
     from dynaboa_b200.multivideo import MultiVideoAdaptor
-    mv = MultiVideoAdaptor(opts, G)
-    calls = [0] * G
+    mv = MultiVideoAdaptor(opts, n_videos)
+    calls = [0] * n_videos
 
     def provider(g, B, dev):
         m = masks_for(g, mv.global_step, calls[g], gd)
@@ -41,7 +41,7 @@ def grouped(opts, gd):
     mv.mask_provider = provider
 
     def step(batches):
-        for g in range(G):
+        for g in range(n_videos):
             calls[g] = 0
             mv.rngs[g].seed(seed_for(g, mv.global_step))
         mv.adapt(batches)
@@ -127,3 +127,33 @@ def test_grouped_adaptation_is_bit_reproducible(asset_dir, tmp_path, golden):
         thetas.append(mv.thetas.clone())
         del mv
     assert torch.equal(thetas[0], thetas[1])
+
+
+def test_one_video_is_bit_identical_to_the_single_video_step(asset_dir, tmp_path, golden):
+    """With one video the grouped adaptor runs ``Adaptor.adapt``'s schedule (history frame paired with the current frame,
+    teacher forward on the side stream): given the same teacher masks, theta, teacher and upper loss are bit-identical after
+    8 frames at C2."""
+    from dynaboa_b200 import config, synthetic
+    from dynaboa_b200.adaptor import Adaptor
+    gd = golden('adapt_c2')
+    mv, step = grouped(make_options(tmp_path / 'mv', str(gd['options']), model_file=config.BASE_MODEL), gd, n_videos=1)
+    ad = Adaptor(make_options(tmp_path / 'ad', str(gd['options']), model_file=config.BASE_MODEL))
+    ad.fused_eval = 'none'
+    stream = synthetic.SyntheticStream(length=8, batch_size=1)
+    for t in range(8):
+        batches = frame([stream], t)
+        step(batches)
+        calls = {'i': 0}
+
+        def provider(B, dev, t=t, calls=calls):
+            m = masks_for(0, t, calls['i'], gd)
+            calls['i'] += 1
+            return m.to(dev)
+        ad.teacher.mask_provider = provider
+        random.seed(seed_for(0, t))
+        ad.global_step, ad.fit_losses = t, {}
+        ad.model.eval()
+        ad.adapt(batches[0])
+        assert torch.equal(mv.last_upper_loss[0], ad.last_upper_loss), t
+    assert torch.equal(mv.theta(0), ad.model.module.arena)
+    assert torch.equal(mv.teachers[0], ad.teacher.arena)
