@@ -64,6 +64,8 @@ SIGNATURES = {
     'dboa_hmr_backward': (I, [P, P, I, I, P, P, P, P, P, P]),
     'dboa_hmr_forward_groups': (I, [P, P, P, P, P, I, P, P, P, P, P, P, P, P, I]),
     'dboa_hmr_backward_groups': (I, [P, P, I, I, P, P, P, P, P, P, I]),
+    'dboa_hmr_forward_active': (I, [P, P, P, P, P, I, P, P, P, P, P, P, P, P, I, C.c_ulonglong]),
+    'dboa_hmr_backward_active': (I, [P, P, I, I, P, P, P, P, P, P, I, C.c_ulonglong]),
     'dboa_conv2d_fwd': (I, [P, P, P, I, I, I, I, I, I, I, I, I, P, L, P]),
     'dboa_conv2d_dgrad': (I, [P, P, P, I, I, I, I, I, I, I, I, I, I, P, L, P]),
     'dboa_conv2d_wgrad': (I, [P, P, P, I, I, I, I, I, I, I, I, I, P, L, P]),
@@ -94,6 +96,7 @@ SIGNATURES = {
     'dboa_loss_motion': (I, [P, P, P, P, F, P, P, P, I, I, P]),
     'dboa_loss_motion_joints': (I, [P, P, P, P, F, P, P, P, I, I, I, I, P]),
     'dboa_loss_motion_groups': (I, [P, P, P, P, F, P, P, P, I, I, I, I, I, P]),
+    'dboa_loss_motion_active': (I, [P, P, P, P, F, P, P, P, I, I, I, I, I, C.c_ulonglong, P]),
     'dboa_sgd_update': (I, [P, P, P, F, L, P]),
     'dboa_adam_ema': (I, [P, P, P, P, P, L, F, F, F, F, I, F, P]),
     'dboa_ema_update': (I, [P, P, L, F, P]),

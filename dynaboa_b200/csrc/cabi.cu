@@ -12,9 +12,9 @@
 namespace dboa {
 int hmr_forward(const float* P, const float* init_pose, const float* init_shape, const float* init_cam, const float* image, int B,
                 const float* drop_masks, float* T, float* scratch, float* rotmat, float* shape, float* cam, float* pose6d,
-                cudaStream_t st, int groups);
+                cudaStream_t st, int groups, unsigned long long active);
 int hmr_backward(const float* P, const float* T, int B, int masked, const float* d_rotmat, const float* d_shape, const float* d_cam,
-                 float* G, float* scratch, cudaStream_t st, int groups);
+                 float* G, float* scratch, cudaStream_t st, int groups, unsigned long long active);
 void hmr_arm_bucket_events(cudaEvent_t e0, cudaEvent_t e1, cudaEvent_t e2);
 long long hmr_bucket_offset(int k);
 void hmr_set_fused_forward(bool on);
@@ -95,24 +95,36 @@ int dboa_hmr_forward(const float* arena, const float* init_pose, const float* in
                      int B, const float* drop_masks, float* tape, float* scratch, float* rotmat, float* shape, float* cam, float* pose6d,
                      dboa_stream_t stream) {
     if (!arena || !init_pose || !init_shape || !init_cam || !image || !tape || !scratch || !rotmat || !shape || !cam) return DBOA_ERR_ARG;
-    return hmr_forward(arena, init_pose, init_shape, init_cam, image, B, drop_masks, tape, scratch, rotmat, shape, cam, pose6d, ST(stream), 1);
+    return hmr_forward(arena, init_pose, init_shape, init_cam, image, B, drop_masks, tape, scratch, rotmat, shape, cam, pose6d, ST(stream), 1, 1ULL);
 }
 int dboa_hmr_backward(const float* arena, const float* tape, int B, int masked, const float* d_rotmat, const float* d_shape,
                       const float* d_cam, float* grad_arena, float* scratch, dboa_stream_t stream) {
     if (!arena || !tape || !grad_arena || !scratch) return DBOA_ERR_ARG;
-    return hmr_backward(arena, tape, B, masked, d_rotmat, d_shape, d_cam, grad_arena, scratch, ST(stream), 1);
+    return hmr_backward(arena, tape, B, masked, d_rotmat, d_shape, d_cam, grad_arena, scratch, ST(stream), 1, 1ULL);
 }
+// every one of `groups` videos (groups outside 1..64 is refused by the plan's shape check before the mask is looked at)
+static unsigned long long all_videos(int groups) { return groups >= 64 ? ~0ULL : (groups < 1 ? 0ULL : (1ULL << groups) - 1); }
 int dboa_hmr_forward_groups(const float* arena, const float* init_pose, const float* init_shape, const float* init_cam, const float* image,
                             int B, const float* drop_masks, float* tape, float* scratch, float* rotmat, float* shape, float* cam,
                             float* pose6d, dboa_stream_t stream, int groups) {
-    if (!arena || !init_pose || !init_shape || !init_cam || !image || !tape || !scratch || !rotmat || !shape || !cam) return DBOA_ERR_ARG;
-    return hmr_forward(arena, init_pose, init_shape, init_cam, image, B, drop_masks, tape, scratch, rotmat, shape, cam, pose6d, ST(stream),
-                       groups);
+    return dboa_hmr_forward_active(arena, init_pose, init_shape, init_cam, image, B, drop_masks, tape, scratch, rotmat, shape, cam, pose6d,
+                                   stream, groups, all_videos(groups));
 }
 int dboa_hmr_backward_groups(const float* arena, const float* tape, int B, int masked, const float* d_rotmat, const float* d_shape,
                              const float* d_cam, float* grad_arena, float* scratch, dboa_stream_t stream, int groups) {
+    return dboa_hmr_backward_active(arena, tape, B, masked, d_rotmat, d_shape, d_cam, grad_arena, scratch, stream, groups, all_videos(groups));
+}
+int dboa_hmr_forward_active(const float* arena, const float* init_pose, const float* init_shape, const float* init_cam, const float* image,
+                            int B, const float* drop_masks, float* tape, float* scratch, float* rotmat, float* shape, float* cam,
+                            float* pose6d, dboa_stream_t stream, int groups, unsigned long long active) {
+    if (!arena || !init_pose || !init_shape || !init_cam || !image || !tape || !scratch || !rotmat || !shape || !cam) return DBOA_ERR_ARG;
+    return hmr_forward(arena, init_pose, init_shape, init_cam, image, B, drop_masks, tape, scratch, rotmat, shape, cam, pose6d, ST(stream),
+                       groups, active);
+}
+int dboa_hmr_backward_active(const float* arena, const float* tape, int B, int masked, const float* d_rotmat, const float* d_shape,
+                             const float* d_cam, float* grad_arena, float* scratch, dboa_stream_t stream, int groups, unsigned long long active) {
     if (!arena || !tape || !grad_arena || !scratch) return DBOA_ERR_ARG;
-    return hmr_backward(arena, tape, B, masked, d_rotmat, d_shape, d_cam, grad_arena, scratch, ST(stream), groups);
+    return hmr_backward(arena, tape, B, masked, d_rotmat, d_shape, d_cam, grad_arena, scratch, ST(stream), groups, active);
 }
 
 int dboa_conv2d_fwd(const float* x, const float* w, float* y, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad, int Kpitch,
@@ -288,6 +300,15 @@ int dboa_loss_motion_groups(const float* p_cur, const float* p_hist, const float
     if (!p_cur || !p_hist || !kp_cur || !kp_hist || !term || !dp_cur || !dp_hist || B < 1) return DBOA_ERR_ARG;
     return loss_motion_launch(p_cur, p_hist, kp_cur, kp_hist, weight, term, dp_cur, dp_hist, B, accumulate_cur, first, count, ST(stream),
                               groups);
+}
+int dboa_loss_motion_active(const float* p_cur, const float* p_hist, const float* kp_cur, const float* kp_hist, float weight, float* term,
+                            float* dp_cur, float* dp_hist, int B, int accumulate_cur, int first, int count, int groups,
+                            unsigned long long active, dboa_stream_t stream) {
+    if (!p_cur || !p_hist || !kp_cur || !kp_hist || !term || !dp_cur || !dp_hist || B < 1) return DBOA_ERR_ARG;
+    if (groups < 1 || groups > 64 || B % groups != 0) return DBOA_ERR_SHAPE;
+    if (active == 0 || (groups < 64 && (active >> groups) != 0)) return DBOA_ERR_ARG;
+    return loss_motion_launch(p_cur, p_hist, kp_cur, kp_hist, weight, term, dp_cur, dp_hist, B, accumulate_cur, first, count, ST(stream),
+                              groups, active);
 }
 
 int dboa_sgd_update(const float* p, const float* g, float* out, float lr, long long n, dboa_stream_t stream) {

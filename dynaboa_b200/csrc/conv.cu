@@ -98,7 +98,9 @@ __device__ __forceinline__ void cluster_reduce_store(const float acc[4][4], floa
 // forward:  y[m][n] = sum_k xcol[m][k] * w[n][k],   m = (b,ho,wo), k = (r,s,ci)
 // grid (ceil(M/64), Cout/64, nsplit); each z-slice covers k in [z*klen, (z+1)*klen)
 // ---------------------------------------------------------------------------------------------
-// GROUPED (all three kernels): a call over d.groups > 1 groups; the group arithmetic is compiled only into that instantiation
+// GROUPED (all three kernels): a call over d.groups > 1 groups; the group arithmetic is compiled only into that instantiation.
+// The CTAs of an idle group (d.active bit clear) return before the cluster reduction, so a split-K cluster (along z, inside one
+// group) exits as a whole.
 template <int VEC, bool GROUPED>
 __global__ void __launch_bounds__(NT) conv_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                       float* __restrict__ out, ConvDims d, int klen) {
@@ -110,7 +112,8 @@ __global__ void __launch_bounds__(NT) conv_fwd_kernel(const float* __restrict__ 
     int bx = blockIdx.x;
     if (GROUPED) {                                                       // the row tiles of group grp
         const int gx = gridDim.x / d.groups, grp = blockIdx.x / gx;
-        x += (size_t)grp * d.B * d.Hi * d.Wi * d.Cin; w += grp * d.wstride; out += (size_t)grp * M * d.Cout;
+        if (!((d.active >> grp) & 1ULL)) return;
+        x +=(size_t)grp * d.B * d.Hi * d.Wi * d.Cin; w += grp * d.wstride; out += (size_t)grp * M * d.Cout;
         bx -= grp * gx;
     }
     const int m0 = bx * BM, n0 = blockIdx.y * BN;
@@ -204,6 +207,7 @@ __global__ void __launch_bounds__(NT) conv_dgrad_kernel(const float* __restrict_
     int bx = blockIdx.x;
     if (GROUPED) {
         const int gx = gridDim.x / d.groups, grp = blockIdx.x / gx;
+        if (!((d.active >> grp) & 1ULL)) return;
         dy += (size_t)grp * d.B * d.Ho * d.Wo * d.Cout; w += grp * d.wstride; out += (size_t)grp * M * d.Cin;
         bx -= grp * gx;
     }
@@ -285,6 +289,7 @@ __global__ void __launch_bounds__(NT) conv_wgrad_kernel(const float* __restrict_
     int bx = blockIdx.x;
     if (GROUPED) {                                                       // K' = this group's B*Ho*Wo pixels
         const int gx = gridDim.x / d.groups, grp = blockIdx.x / gx;
+        if (!((d.active >> grp) & 1ULL)) return;
         dy += (size_t)grp * Mpix * d.Cout; x += (size_t)grp * d.B * d.Hi * d.Wi * d.Cin; out += grp * d.wstride;
         bx -= grp * gx;
     }

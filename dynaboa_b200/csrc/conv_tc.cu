@@ -194,9 +194,12 @@ __global__ void __launch_bounds__(NT, 1) conv_tf32x3_kernel(const float* __restr
     const int Ktaps = d.kh * d.kw, Kfull = Ktaps * d.Cin;
     // Grouped call: blockIdx.x = group * gx + tile, and group grp reads / writes only its own samples and weights (no tile
     // straddles two groups, since the weight operand differs per group).  groups == 1: grp = 0, bx = blockIdx.x.
+    // The CTAs of an idle group (its `d.active` bit clear) return here: the split-K cluster lies along z inside one group, so the
+    // exit is uniform over the cluster and comes before any barrier, DSMEM access or dependency wait.
     int gx = gridDim.x, bx = blockIdx.x;
     if (GROUPED) {
         const int grp = blockIdx.x / (gridDim.x / d.groups);
+        if (!((d.active >> grp) & 1ULL)) return;
         gx = gridDim.x / d.groups; bx = blockIdx.x - grp * gx;
         const size_t xin = (size_t)grp * d.B * d.Hi * d.Wi * d.Cin, yout = (size_t)grp * d.B * d.Ho * d.Wo * d.Cout;
         if (MODE == FWD) { P += xin; Q += grp * d.wstride; O += yout; }

@@ -324,9 +324,11 @@ int gn_bwd_fused(const float* dout, const float* mask_src, const float* y, const
 // Deferred affine-parameter gradients of a whole network (B > 1): every GroupNorm backward left its per-sample rows
 // [B][C] (dgamma) | [B][C] (dbeta) at rows + 2 * B * item.cum_channels; ONE launch adds them to the gradient arena in sample
 // order.  This keeps the per-layer kernels free of the fence + ticket + last-CTA pass that B > 1 otherwise needs.
-// Grouped (gridDim.y groups of B / groups samples): group blockIdx.y sums its own rows into G + blockIdx.y * pstride.
+// Grouped (gridDim.y groups of B / groups samples): group blockIdx.y sums its own rows into G + blockIdx.y * pstride, if its
+// `active` bit is set.
 __global__ void __launch_bounds__(256) gn_param_finish_kernel(const GnFinishItem* __restrict__ items, const float* __restrict__ rows,
-                                                              float* __restrict__ G, int B, long long pstride) {
+                                                              float* __restrict__ G, int B, long long pstride, unsigned long long active) {
+    if (!((active >> blockIdx.y) & 1ULL)) return;
     pdl_wait();
     pdl_trigger();
     const GnFinishItem it = items[blockIdx.x];
@@ -342,9 +344,9 @@ __global__ void __launch_bounds__(256) gn_param_finish_kernel(const GnFinishItem
 }
 
 int gn_param_finish(const GnFinishItem* items_dev, int n_items, const float* rows, float* G, int B, cudaStream_t st, int groups,
-                    long long pstride) {
+                    long long pstride, unsigned long long active) {
     if (groups < 1 || B % groups != 0) return DBOA_ERR_SHAPE;
-    return launch_ex(gn_param_finish_kernel, dim3(n_items, groups), dim3(256), 0, st, dim3(1, 1, 1), true, items_dev, rows, G, B, pstride);
+    return launch_ex(gn_param_finish_kernel, dim3(n_items, groups), dim3(256), 0, st, dim3(1, 1, 1), true, items_dev, rows, G, B, pstride, active);
 }
 
 }  // namespace dboa

@@ -19,8 +19,10 @@ __global__ void __launch_bounds__(256) linear_fwd_kernel(const float* __restrict
                                                          const float* __restrict__ bias, const float* __restrict__ addend, int ld_add,
                                                          const float* __restrict__ mask, float* __restrict__ pre,
                                                          float* __restrict__ post, int ld_out, float* __restrict__ post2, int ld_out2,
-                                                         int b0, int nb, int N, int K, int bper, long long wstride) {
+                                                         int b0, int nb, int N, int K, int bper, long long wstride,
+                                                         unsigned long long active) {
     __shared__ float sred[8][BT];
+    if (!((active >> blockIdx.y) & 1ULL)) return;           // grouped: an idle group's rows are not computed
     pdl_wait();
     pdl_trigger();
     b0 += blockIdx.y * bper;                                // grouped: rows of group blockIdx.y, its own weights
@@ -89,12 +91,12 @@ __global__ void __launch_bounds__(256) linear_fwd_kernel(const float* __restrict
 
 int linear_fwd(const float* x, int ldx, const float* W, int ldw, const float* bias, const float* addend, int ld_add, const float* mask,
                float* pre, float* post, int ld_out, float* post2, int ld_out2, int B, int N, int K, cudaStream_t st, int groups,
-               long long wstride) {
+               long long wstride, unsigned long long active) {
     if (groups < 1 || B % groups != 0) return DBOA_ERR_SHAPE;
     const int bper = B / groups;
     for (int b0 = 0; b0 < bper; b0 += 8) {
         int nb = bper - b0 < 8 ? bper - b0 : 8;
-        DBOA_TRY(launch_ex(linear_fwd_kernel<8>, dim3(ceil_div(N, 2), groups), dim3(256), 0, st, dim3(1, 1, 1), true, x, ldx, W, ldw, bias, addend, ld_add, mask, pre, post, ld_out, post2, ld_out2, b0, nb, N, K, bper, wstride));
+        DBOA_TRY(launch_ex(linear_fwd_kernel<8>, dim3(ceil_div(N, 2), groups), dim3(256), 0, st, dim3(1, 1, 1), true, x, ldx, W, ldw, bias, addend, ld_add, mask, pre, post, ld_out, post2, ld_out2, b0, nb, N, K, bper, wstride, active));
     }
     return DBOA_OK;
 }
@@ -104,7 +106,8 @@ int linear_fwd(const float* x, int ldx, const float* W, int ldw, const float* bi
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) linear_dgrad_kernel(const float* __restrict__ dy, int ldy, const float* __restrict__ W, int ldw,
                                                            float* __restrict__ part, int b0, int nb, int B, int N, int K, int nlen,
-                                                           int bper, long long wstride) {
+                                                           int bper, long long wstride, unsigned long long active) {
+    if (!((active >> blockIdx.z) & 1ULL)) return;           // grouped: an idle group's partial rows are not computed
     pdl_wait();
     pdl_trigger();
     b0 += blockIdx.z * bper;                                // grouped: rows of group blockIdx.z, its own weights
@@ -147,7 +150,7 @@ __global__ void linear_dgrad_reduce_kernel(const float* __restrict__ part, float
 }
 
 int linear_dgrad(const float* dy, int ldy, const float* W, int ldw, float* dx, int ldx, int B, int N, int K, float* ws, size_t ws_floats,
-                 cudaStream_t st, int groups, long long wstride) {
+                 cudaStream_t st, int groups, long long wstride, unsigned long long active) {
     if (groups < 1 || B % groups != 0) return DBOA_ERR_SHAPE;
     const int bper = B / groups;
     // 32 rows of W per CTA: at batch 1-3 the kernel is a chain of dependent weight loads, so many short CTAs beat few long ones
@@ -161,7 +164,7 @@ int linear_dgrad(const float* dy, int ldy, const float* W, int ldw, float* dx, i
         int nb = bper - b0 < 8 ? bper - b0 : 8;
         dim3 grid(ceil_div(K, 256), nsplit, groups);
         DBOA_TRY(launch_ex(linear_dgrad_kernel, dim3(grid), dim3(256), 0, st, dim3(1, 1, 1), true, dy, ldy, W, ldw, ws, b0, nb, B, N, K, nlen,
-                           bper, wstride));
+                           bper, wstride, active));
     }
     return launch_ex(linear_dgrad_reduce_kernel, dim3(ceil_div(B * K, 256)), dim3(256), 0, st, dim3(1, 1, 1), true, ws, dx, ldx, B, K, nsplit);
 }
@@ -174,13 +177,15 @@ int linear_dgrad(const float* dy, int ldy, const float* W, int ldw, float* dx, i
 template <bool GROUPED>
 __global__ void __launch_bounds__(256) linear_wgrad_kernel(const float* __restrict__ dy, int ldy, const float* __restrict__ x, int ldx,
                                                            float* __restrict__ dW, int ldw, float* __restrict__ db, int R, int N, int K,
-                                                           int bper, int bstride, long long wstride) {
+                                                           int bper, int bstride, long long wstride,
+                                                           unsigned long long active) {
+    const int g = blockIdx.z;
+    if (GROUPED && !((active >> g) & 1ULL)) return;         // nothing is added to an idle group's gradient
     pdl_wait();
     pdl_trigger();
     __shared__ float sdy[64];
     const int n = blockIdx.y;
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
-    const int g = blockIdx.z;
     if (GROUPED) {
         dW += g * wstride;
         if (db != nullptr) db += g * wstride;
@@ -206,7 +211,7 @@ __global__ void __launch_bounds__(256) linear_wgrad_kernel(const float* __restri
 }
 
 int linear_wgrad(const float* dy, int ldy, const float* x, int ldx, float* dW, int ldw, float* db, int R, int N, int K, cudaStream_t st,
-                 int groups, int B, long long wstride) {
+                 int groups, int B, long long wstride, unsigned long long active) {
     int bper = R, bstride = R, rows = R;
     if (groups != 1) {
         if (groups < 1 || B < 1 || B % groups != 0 || R % B != 0) return DBOA_ERR_SHAPE;
@@ -214,7 +219,7 @@ int linear_wgrad(const float* dy, int ldy, const float* x, int ldx, float* dW, i
     }
     dim3 grid(ceil_div(K, 256), N, groups);
     return launch_ex(groups > 1 ? linear_wgrad_kernel<true> : linear_wgrad_kernel<false>, dim3(grid), dim3(256), 0, st, dim3(1, 1, 1), true,
-                     dy, ldy, x, ldx, dW, ldw, db, rows, N, K, bper, bstride, wstride);
+                     dy, ldy, x, ldx, dW, ldw, db, rows, N, K, bper, bstride, wstride, active);
 }
 
 // ---------------------------------------------------------------------------------------------

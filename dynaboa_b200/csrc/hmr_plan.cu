@@ -267,7 +267,7 @@ void hmr_set_async_wgrad(bool on) { g_async_enabled = on; }
 // DBOA_WGRAD_STREAMS=1|2: how many side streams the weight gradients alternate over
 static const int g_wgrad_streams = [] { const char* e = getenv("DBOA_WGRAD_STREAMS"); return (e && e[0] == '1') ? 1 : BwdAsync::NSIDE; }();
 
-static ConvDims dims_of(const ConvLayer& c, int B, int groups = 1);
+static ConvDims dims_of(const ConvLayer& c, int B, int groups = 1, unsigned long long active = ~0ULL);
 
 // Fused plan (conv_tc.cu with an operand transform): every convolution applies the GroupNorm (+ residual, ReLU) of its operand on
 // load and leaves the statistics of its output as fixed-point sums; the fused data gradient applies GroupNorm backward on load
@@ -303,49 +303,58 @@ static const GnItems& gn_items() {
     return gi;
 }
 // backward convolutions: wgmma implicit GEMM when enabled and the shape is taken, else the fp32 CUDA-core kernels
-static int conv_backward_data(const ConvLayer& c, int B, int groups, const float* dy, const float* w, float* dx, int accumulate, float* ws,
-                              cudaStream_t st);
-static int conv_backward_weight(const ConvLayer& c, int B, int groups, const float* dy, const float* x, float* dw, float* ws, cudaStream_t st);
+static int conv_backward_data(const ConvLayer& c, int B, int groups, unsigned long long active, const float* dy, const float* w, float* dx,
+                              int accumulate, float* ws, cudaStream_t st);
+static int conv_backward_weight(const ConvLayer& c, int B, int groups, unsigned long long active, const float* dy, const float* x, float* dw,
+                                float* ws, cudaStream_t st);
 
-// B samples in `groups` videos of B / groups consecutive samples; video g's weights (and weight gradients) are one arena further on
-static ConvDims dims_of(const ConvLayer& c, int B, int groups) {
+// B samples in `groups` videos of B / groups consecutive samples; video g's weights (and weight gradients) are one arena further on;
+// the videos whose `active` bit is clear are skipped
+static ConvDims dims_of(const ConvLayer& c, int B, int groups, unsigned long long active) {
     ConvDims d;
-    d.B = B / groups; d.groups = groups; d.wstride = net().arena_floats;
+    d.B = B / groups; d.groups = groups; d.wstride = net().arena_floats; d.active = active;
     d.Hi = c.hin; d.Wi = c.hin; d.Cin = c.cin; d.Ho = c.hout; d.Wo = c.hout; d.Cout = c.cout;
     d.kh = c.k; d.kw = c.k; d.stride = c.stride; d.pad = c.pad; d.Kpitch = c.kpitch;
     return d;
 }
 
 // conv forward: wgmma implicit GEMM when enabled and the shape is taken (Cin % 64 == 0, Cout % 64 == 0), else the fp32 CUDA-core kernel
-static int conv_forward(const ConvLayer& c, int B, int groups, const float* x, const float* w, float* y, float* ws, cudaStream_t st) {
+static int conv_forward(const ConvLayer& c, int B, int groups, unsigned long long active, const float* x, const float* w, float* y, float* ws,
+                        cudaStream_t st) {
+    const ConvDims d = dims_of(c, B, groups, active);
     if (conv_tc_enabled()) {
-        int s = conv_tc_fwd(x, w, y, dims_of(c, B, groups), st);
+        int s = conv_tc_fwd(x, w, y, d, st);
         if (s != DBOA_ERR_UNSUPPORTED) return s;
     }
-    return conv_fwd(x, w, y, dims_of(c, B, groups), ws, (size_t)kConvWs, st);
+    return conv_fwd(x, w, y, d, ws, (size_t)kConvWs, st);
 }
 
-static int conv_backward_data(const ConvLayer& c, int B, int groups, const float* dy, const float* w, float* dx, int accumulate, float* ws,
-                              cudaStream_t st) {
+static int conv_backward_data(const ConvLayer& c, int B, int groups, unsigned long long active, const float* dy, const float* w, float* dx,
+                              int accumulate, float* ws, cudaStream_t st) {
+    const ConvDims d = dims_of(c, B, groups, active);
     if (conv_tc_bwd_enabled()) {
-        int s = conv_tc_dgrad(dy, w, dx, dims_of(c, B, groups), accumulate, st);
+        int s = conv_tc_dgrad(dy, w, dx, d, accumulate, st);
         if (s != DBOA_ERR_UNSUPPORTED) return s;
     }
-    return conv_dgrad(dy, w, dx, dims_of(c, B, groups), accumulate, ws, (size_t)kConvWs, st);
+    return conv_dgrad(dy, w, dx, d, accumulate, ws, (size_t)kConvWs, st);
 }
-static int conv_backward_weight(const ConvLayer& c, int B, int groups, const float* dy, const float* x, float* dw, float* ws, cudaStream_t st) {
+static int conv_backward_weight(const ConvLayer& c, int B, int groups, unsigned long long active, const float* dy, const float* x, float* dw,
+                                float* ws, cudaStream_t st) {
+    const ConvDims d = dims_of(c, B, groups, active);
     if (conv_tc_wgrad_enabled()) {
-        int s = conv_tc_wgrad(dy, x, dw, dims_of(c, B, groups), st);
+        int s = conv_tc_wgrad(dy, x, dw, d, st);
         if (s != DBOA_ERR_UNSUPPORTED) return s;
     }
-    return conv_wgrad(dy, x, dw, dims_of(c, B, groups), ws, (size_t)kConvWs, st);
+    return conv_wgrad(dy, x, dw, d, ws, (size_t)kConvWs, st);
 }
 
 // Argument checks of a grouped call (host only, before any device access).  Video g owns samples [g * B / groups, (g + 1) * B /
 // groups) and the arena, gradient arena and weights one arena_floats apart; only the default plan serves several videos, and the
-// data-parallel gradient buckets (one arena, all-reduced across ranks) do not apply to them.
-static int groups_check(int B, int groups) {
+// data-parallel gradient buckets (one arena, all-reduced across ranks) do not apply to them.  `active` (bit g: video g takes part)
+// must name at least one video and none past `groups`.
+static int groups_check(int B, int groups, unsigned long long active) {
     if (groups < 1 || B < 1 || B > 64 || B % groups != 0) return DBOA_ERR_SHAPE;
+    if (active == 0 || (groups < 64 && (active >> groups) != 0)) return DBOA_ERR_ARG;
     if (groups > 1 && (g_fused_fwd || g_fused_bwd)) return DBOA_ERR_UNSUPPORTED;
     return DBOA_OK;
 }
@@ -421,8 +430,8 @@ __global__ void rot6d_rows_bwd_kernel(const float* __restrict__ params3, const f
 // ---------------------------------------------------------------------------------------------
 int hmr_forward(const float* P, const float* init_pose, const float* init_shape, const float* init_cam, const float* image, int B,
                 const float* drop_masks, float* T, float* scratch, float* rotmat, float* shape, float* cam, float* pose6d,
-                cudaStream_t st, int groups) {
-    DBOA_TRY(groups_check(B, groups));
+                cudaStream_t st, int groups, unsigned long long active) {
+    DBOA_TRY(groups_check(B, groups, active));
     DBOA_TRY(device_guard());
     const Net& n = net();
     const long long PS = n.arena_floats;
@@ -437,7 +446,7 @@ int hmr_forward(const float* P, const float* init_pose, const float* init_shape,
     if (g_fused_fwd && conv_tc_enabled())
         cudaMemsetAsync(T + t.acc, 0, n.convs.size() * (size_t)B * 16 * sizeof(float), st);      // statistics accumulators of this forward
     DBOA_TRY(nchw_to_nhwc(image, T + t.x0, B, 3, 224, 224, st));
-    DBOA_TRY(conv_forward(n.convs[0], B, groups, T + t.x0, P + n.convs[0].w_off, T + t.conv[0].y, sc.ws, st));
+    DBOA_TRY(conv_forward(n.convs[0], B, groups, active, T + t.x0, P + n.convs[0].w_off, T + t.conv[0].y, sc.ws, st));
     DBOA_TRY(gn_plain(0, T + t.conv[0].a, 1, nullptr));
     DBOA_TRY(maxpool3x3s2_fwd(T + t.conv[0].a, T + t.p0, reinterpret_cast<unsigned char*>(T + t.p0_idx), B, 112, 112, 64, st));
     const float* x = T + t.p0;
@@ -495,15 +504,15 @@ int hmr_forward(const float* P, const float* init_pose, const float* init_shape,
     } else {
     for (const Block& b : n.blocks) {
         const ConvLayer &c1 = n.convs[b.c1], &c2 = n.convs[b.c2], &c3 = n.convs[b.c3];
-        DBOA_TRY(conv_forward(c1, B, groups, x, P + c1.w_off, T + t.conv[b.c1].y, sc.ws, st));
+        DBOA_TRY(conv_forward(c1, B, groups, active, x, P + c1.w_off, T + t.conv[b.c1].y, sc.ws, st));
         DBOA_TRY(gn_plain(b.c1, T + t.conv[b.c1].a, 1, nullptr));
-        DBOA_TRY(conv_forward(c2, B, groups, T + t.conv[b.c1].a, P + c2.w_off, T + t.conv[b.c2].y, sc.ws, st));
+        DBOA_TRY(conv_forward(c2, B, groups, active, T + t.conv[b.c1].a, P + c2.w_off, T + t.conv[b.c2].y, sc.ws, st));
         DBOA_TRY(gn_plain(b.c2, T + t.conv[b.c2].a, 1, nullptr));
-        DBOA_TRY(conv_forward(c3, B, groups, T + t.conv[b.c2].a, P + c3.w_off, T + t.conv[b.c3].y, sc.ws, st));
+        DBOA_TRY(conv_forward(c3, B, groups, active, T + t.conv[b.c2].a, P + c3.w_off, T + t.conv[b.c3].y, sc.ws, st));
         const int HW = c3.hout * c3.hout;
         if (b.cd >= 0) {
             const ConvLayer& cd = n.convs[b.cd];
-            DBOA_TRY(conv_forward(cd, B, groups, x, P + cd.w_off, T + t.conv[b.cd].y, sc.ws, st));
+            DBOA_TRY(conv_forward(cd, B, groups, active, x, P + cd.w_off, T + t.conv[b.cd].y, sc.ws, st));
             (void)HW;
             DBOA_TRY(gn_plain(b.cd, sc.t1, 0, nullptr));                 // normalised shortcut -> scratch
             DBOA_TRY(gn_plain(b.c3, T + t.conv[b.c3].a, 1, sc.t1));      // relu(gn(y3) + shortcut)
@@ -524,13 +533,13 @@ int hmr_forward(const float* P, const float* init_pose, const float* init_shape,
         float* h1pre = T + t.h1pre + (size_t)it * B * HID; float* h1post = T + t.h1post + (size_t)it * B * HID;
         float* h2pre = T + t.h2pre + (size_t)it * B * HID; float* h2post = T + t.h2post + (size_t)it * B * HID;
         DBOA_TRY(linear_fwd(xc, HEAD_LD, P + n.fc1_w, HEAD_LD, P + n.fc1_b, nullptr, 0, m1, h1pre, h1post, HID, nullptr, 0, B, HID, HEAD_IN, st,
-                            groups, PS));
-        DBOA_TRY(linear_fwd(h1post, HID, P + n.fc2_w, HID, P + n.fc2_b, nullptr, 0, m2, h2pre, h2post, HID, nullptr, 0, B, HID, HID, st, groups, PS));
+                            groups, PS, active));
+        DBOA_TRY(linear_fwd(h1post, HID, P + n.fc2_w, HID, P + n.fc2_b, nullptr, 0, m2, h2pre, h2post, HID, nullptr, 0, B, HID, HID, st, groups, PS, active));
         float* pin = T + t.params + (size_t)it * B * DEC_LD;
         float* pout = T + t.params + (size_t)(it + 1) * B * DEC_LD;
         float* xnext = it < 2 ? T + t.xc + (size_t)(it + 1) * B * HEAD_LD + 2048 : nullptr;
         DBOA_TRY(linear_fwd(h2post, HID, P + n.dec_w, HID, P + n.dec_b, pin, DEC_LD, nullptr, nullptr, pout, DEC_LD, xnext, HEAD_LD, B, NDEC,
-                            HID, st, groups, PS));
+                            HID, st, groups, PS, active));
     }
     const float* p3 = T + t.params + 3ULL * B * DEC_LD;
     DBOA_TRY(launch_ex(rot6d_rows_fwd_kernel, dim3(ceil_div(B * 24, 128)), dim3(128), 0, st, dim3(1, 1, 1), true, p3, rotmat, B));
@@ -541,10 +550,10 @@ int hmr_forward(const float* P, const float* init_pose, const float* init_shape,
 // backward (accumulates into the flat gradient arena G, same layout as P)
 // ---------------------------------------------------------------------------------------------
 int hmr_backward(const float* P, const float* T, int B, int masked_in, const float* d_rotmat, const float* d_shape, const float* d_cam,
-                 float* G, float* scratch, cudaStream_t st, int groups) {
+                 float* G, float* scratch, cudaStream_t st, int groups, unsigned long long active) {
     const bool bucketed = g_bucket_req.armed;
     if (groups != 1) g_bucket_req.armed = false;         // a request armed for a grouped call is consumed by it, whatever it returns
-    DBOA_TRY(groups_check(B, groups));
+    DBOA_TRY(groups_check(B, groups, active));
     if (groups > 1 && bucketed) return DBOA_ERR_UNSUPPORTED;
     DBOA_TRY(device_guard());
     const Net& n = net();
@@ -572,21 +581,21 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
         float* d_h1 = sc.d_h1 + (size_t)it * B * HID;
         cudaMemcpyAsync(dy_dec, sc.dP, (size_t)B * DEC_LD * sizeof(float), cudaMemcpyDeviceToDevice, st);
         if (masked) {
-            DBOA_TRY(linear_dgrad(dy_dec, DEC_LD, P + n.dec_w, HID, sc.tmp1024, HID, B, NDEC, HID, sc.lin_ws, sc.lin_ws_floats, st, groups, PS));
+            DBOA_TRY(linear_dgrad(dy_dec, DEC_LD, P + n.dec_w, HID, sc.tmp1024, HID, B, NDEC, HID, sc.lin_ws, sc.lin_ws_floats, st, groups, PS, active));
             DBOA_TRY(ew_mul(sc.tmp1024, T + t.masks + (size_t)(it * 2 + 1) * B * HID, d_h2, (size_t)B * HID, st));
-            DBOA_TRY(linear_dgrad(d_h2, HID, P + n.fc2_w, HID, sc.tmp1024, HID, B, HID, HID, sc.lin_ws, sc.lin_ws_floats, st, groups, PS));
+            DBOA_TRY(linear_dgrad(d_h2, HID, P + n.fc2_w, HID, sc.tmp1024, HID, B, HID, HID, sc.lin_ws, sc.lin_ws_floats, st, groups, PS, active));
             DBOA_TRY(ew_mul(sc.tmp1024, T + t.masks + (size_t)(it * 2 + 0) * B * HID, d_h1, (size_t)B * HID, st));
         } else {
-            DBOA_TRY(linear_dgrad(dy_dec, DEC_LD, P + n.dec_w, HID, d_h2, HID, B, NDEC, HID, sc.lin_ws, sc.lin_ws_floats, st, groups, PS));
-            DBOA_TRY(linear_dgrad(d_h2, HID, P + n.fc2_w, HID, d_h1, HID, B, HID, HID, sc.lin_ws, sc.lin_ws_floats, st, groups, PS));
+            DBOA_TRY(linear_dgrad(dy_dec, DEC_LD, P + n.dec_w, HID, d_h2, HID, B, NDEC, HID, sc.lin_ws, sc.lin_ws_floats, st, groups, PS, active));
+            DBOA_TRY(linear_dgrad(d_h2, HID, P + n.fc2_w, HID, d_h1, HID, B, HID, HID, sc.lin_ws, sc.lin_ws_floats, st, groups, PS, active));
         }
-        DBOA_TRY(linear_dgrad(d_h1, HID, P + n.fc1_w, HEAD_LD, sc.dxc, HEAD_LD, B, HID, HEAD_IN, sc.lin_ws, sc.lin_ws_floats, st, groups, PS));
+        DBOA_TRY(linear_dgrad(d_h1, HID, P + n.fc1_w, HEAD_LD, sc.dxc, HEAD_LD, B, HID, HEAD_IN, sc.lin_ws, sc.lin_ws_floats, st, groups, PS, active));
         DBOA_TRY(ew_add_rows(sc.dxf, 2048, sc.dxf, 2048, sc.dxc, HEAD_LD, B, 2048, st));
         DBOA_TRY(ew_add_rows(sc.dP, DEC_LD, sc.dP, DEC_LD, sc.dxc + 2048, HEAD_LD, B, NDEC, st));
     }
-    DBOA_TRY(linear_wgrad(sc.dy_dec, DEC_LD, T + t.h2post, HID, G + n.dec_w, HID, G + n.dec_b, 3 * B, NDEC, HID, st, groups, B, PS));
-    DBOA_TRY(linear_wgrad(sc.d_h2, HID, T + t.h1post, HID, G + n.fc2_w, HID, G + n.fc2_b, 3 * B, HID, HID, st, groups, B, PS));
-    DBOA_TRY(linear_wgrad(sc.d_h1, HID, T + t.xc, HEAD_LD, G + n.fc1_w, HEAD_LD, G + n.fc1_b, 3 * B, HID, HEAD_IN, st, groups, B, PS));
+    DBOA_TRY(linear_wgrad(sc.dy_dec, DEC_LD, T + t.h2post, HID, G + n.dec_w, HID, G + n.dec_b, 3 * B, NDEC, HID, st, groups, B, PS, active));
+    DBOA_TRY(linear_wgrad(sc.d_h2, HID, T + t.h1post, HID, G + n.fc2_w, HID, G + n.fc2_b, 3 * B, HID, HID, st, groups, B, PS, active));
+    DBOA_TRY(linear_wgrad(sc.d_h1, HID, T + t.xc, HEAD_LD, G + n.fc1_w, HEAD_LD, G + n.fc1_b, 3 * B, HID, HEAD_IN, st, groups, B, PS, active));
 
     // ---- backbone
     float* dOut = sc.g0;
@@ -613,13 +622,13 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
     };
     // weight gradient of conv `c` from dy held in temp k
     auto wgrad = [&](const ConvLayer& c, int k, const float* xin_) {
-        if (!async) return conv_backward_weight(c, B, groups, tmp[k], xin_, G + c.w_off, sc.ws, st);
+        if (!async) return conv_backward_weight(c, B, groups, active, tmp[k], xin_, G + c.w_off, sc.ws, st);
         cudaStream_t ss = A.side[A.next_side];
         A.next_side = (A.next_side + 1) % g_wgrad_streams;
         cudaEventRecord(A.ev_ready[A.ring], st);
         cudaStreamWaitEvent(ss, A.ev_ready[A.ring], 0);
         A.ring = (A.ring + 1) & 7;
-        int s_ = conv_backward_weight(c, B, groups, tmp[k], xin_, G + c.w_off, sc.ws, ss);
+        int s_ = conv_backward_weight(c, B, groups, active, tmp[k], xin_, G + c.w_off, sc.ws, ss);
         cudaEventRecord(A.ev_read[k], ss);
         A.pending[k] = true;
         return s_;
@@ -630,7 +639,7 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
         if (B > 1 && first_conv < finished_from) {
             const GnItems& gi = gn_items();
             if (gi.dev == nullptr) return DBOA_ERR_CUDA;
-            DBOA_TRY(gn_param_finish(gi.dev + first_conv, finished_from - first_conv, sc.gnp, G, B, st, groups, PS));
+            DBOA_TRY(gn_param_finish(gi.dev + first_conv, finished_from - first_conv, sc.gnp, G, B, st, groups, PS, active));
             finished_from = first_conv;
         }
         if (!breq.armed) return DBOA_OK;
@@ -717,13 +726,13 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
                 const ConvLayer& cd = n.convs[b.cd];
                 DBOA_TRY(gnb(b.cd, dzo, a3, claim(1)));
                 DBOA_TRY(wgrad(cd, 1, xin));
-                DBOA_TRY(conv_backward_data(cd, B, groups, tmp[1], P + cd.w_off, dIn, 0, sc.ws, st));
+                DBOA_TRY(conv_backward_data(cd, B, groups, active, tmp[1], P + cd.w_off, dIn, 0, sc.ws, st));
                 DBOA_TRY(gnb(b.c2, tmp[2], T + t.conv[b.c2].a, claim(3)));
                 DBOA_TRY(wgrad(c2, 3, T + t.conv[b.c1].a));
-                DBOA_TRY(conv_backward_data(c2, B, groups, tmp[3], P + c2.w_off, claim(4), 0, sc.ws, st));
+                DBOA_TRY(conv_backward_data(c2, B, groups, active, tmp[3], P + c2.w_off, claim(4), 0, sc.ws, st));
                 DBOA_TRY(gnb(b.c1, tmp[4], T + t.conv[b.c1].a, claim(5)));
                 DBOA_TRY(wgrad(c1, 5, xin));
-                DBOA_TRY(conv_backward_data(c1, B, groups, tmp[5], P + c1.w_off, dIn, 1, sc.ws, st));
+                DBOA_TRY(conv_backward_data(c1, B, groups, active, tmp[5], P + c1.w_off, dIn, 1, sc.ws, st));
                 const Block& pb = n.blocks[bi - 1];             // seam: the previous block (last of its layer) has an identity shortcut
                 const ConvLayer& p3 = n.convs[pb.c3];
                 DBOA_TRY(gn_bwd_prep(dIn, T + t.conv[pb.c3].a, dIn, prep_of(pb.c3), B, p3.hout * p3.hout, p3.cout, st));
@@ -746,24 +755,24 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
             const ConvLayer& cd = n.convs[b.cd];
             DBOA_TRY(gnb(b.cd, dOut, a3, claim(1)));
             DBOA_TRY(wgrad(cd, 1, xin));
-            DBOA_TRY(conv_backward_data(cd, B, groups, tmp[1], P + cd.w_off, dIn, 0, sc.ws, st));
+            DBOA_TRY(conv_backward_data(cd, B, groups, active, tmp[1], P + cd.w_off, dIn, 0, sc.ws, st));
         } else {
             DBOA_TRY(relu_mask(dOut, a3, dIn, (size_t)B * c3.hout * c3.hout * c3.cout, st));
         }
-        DBOA_TRY(conv_backward_data(c3, B, groups, tmp[0], P + c3.w_off, claim(2), 0, sc.ws, st));
+        DBOA_TRY(conv_backward_data(c3, B, groups, active, tmp[0], P + c3.w_off, claim(2), 0, sc.ws, st));
         DBOA_TRY(gnb(b.c2, tmp[2], T + t.conv[b.c2].a, claim(3)));
         DBOA_TRY(wgrad(c2, 3, T + t.conv[b.c1].a));
-        DBOA_TRY(conv_backward_data(c2, B, groups, tmp[3], P + c2.w_off, claim(4), 0, sc.ws, st));
+        DBOA_TRY(conv_backward_data(c2, B, groups, active, tmp[3], P + c2.w_off, claim(4), 0, sc.ws, st));
         DBOA_TRY(gnb(b.c1, tmp[4], T + t.conv[b.c1].a, claim(5)));
         DBOA_TRY(wgrad(c1, 5, xin));
-        DBOA_TRY(conv_backward_data(c1, B, groups, tmp[5], P + c1.w_off, dIn, 1, sc.ws, st));
+        DBOA_TRY(conv_backward_data(c1, B, groups, active, tmp[5], P + c1.w_off, dIn, 1, sc.ws, st));
         float* sw = dOut; dOut = dIn; dIn = sw;
     }
     }
     // ---- stem: maxpool, GroupNorm+ReLU, conv (weight gradient only; the image needs none)
     DBOA_TRY(maxpool3x3s2_bwd(dOut, reinterpret_cast<const unsigned char*>(T + t.p0_idx), dIn, B, 112, 112, 64, st));
     DBOA_TRY(gnb(0, dIn, T + t.conv[0].a, claim(0)));
-    int rc = conv_wgrad(tmp[0], T + t.x0, G + n.convs[0].w_off, dims_of(n.convs[0], B, groups), sc.ws, (size_t)kConvWs, st);
+    int rc = conv_wgrad(tmp[0], T + t.x0, G + n.convs[0].w_off, dims_of(n.convs[0], B, groups, active), sc.ws, (size_t)kConvWs, st);
     if (rc == DBOA_OK) rc = bucket_done(2, 0);               // stem, layer1, layer2 (and, for B > 1, their GroupNorm affine rows)
     if (async) {                                   // join: nothing of this call is left running when the caller's stream continues
         for (int i = 0; i < BwdAsync::NSIDE; ++i) {

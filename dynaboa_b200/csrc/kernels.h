@@ -8,10 +8,12 @@ namespace dboa {
 
 // Grouped convolutions (several independent videos in one launch): `groups` blocks of B samples each, stored one after the
 // other in the activations; group g uses the weights w + g * wstride (the weight gradient writes dw + g * wstride).
+// `active`: bit g set means group g takes part; the CTAs of an idle group return before touching memory (grouped calls only).
 struct ConvDims {
     int B, Hi, Wi, Cin, Ho, Wo, Cout, kh, kw, stride, pad, Kpitch;
     int groups = 1;
     long long wstride = 0;
+    unsigned long long active = ~0ULL;
 };
 
 // ---- conv.cu (fp32 CUDA-core implicit GEMM)
@@ -93,9 +95,9 @@ int gn_bwd_fused(const float* dout, const float* mask_src, const float* y, const
                  float* dgamma, float* dbeta, float* partial, int B, int HW, int C, cudaStream_t st, int defer = 0, int bper = 0,
                  long long pstride = 0);
 struct GnFinishItem { long long g_off, b_off, cum_channels; int C; };
-// rows of samples [g * B / groups, (g + 1) * B / groups) are added to G + g * pstride
+// rows of samples [g * B / groups, (g + 1) * B / groups) are added to G + g * pstride (groups whose `active` bit is set)
 int gn_param_finish(const GnFinishItem* items_dev, int n_items, const float* rows, float* G, int B, cudaStream_t st, int groups = 1,
-                    long long pstride = 0);
+                    long long pstride = 0, unsigned long long active = ~0ULL);
 // ---- norm_pool.cu
 int relu_mask(const float* dout, const float* mask_src, float* dz, size_t n, cudaStream_t st);
 int nchw_to_nhwc(const float* x, float* y, int B, int C, int H, int W, cudaStream_t st);
@@ -106,18 +108,19 @@ int avgpool_fwd(const float* x, float* out, int B, int HW, int C, int ld, int nc
 int avgpool_bwd(const float* dxf, int ld, float* dx, int B, int HW, int C, cudaStream_t st);
 
 // ---- head.cu
-// Grouped variants: B = groups * (B / groups) rows, row b uses W / bias + (b / (B / groups)) * wstride.
+// Grouped variants: B = groups * (B / groups) rows, row b uses W / bias + (b / (B / groups)) * wstride.  Only the groups whose
+// `active` bit is set are computed; the rows of the others are left as they were (linear_dgrad: unspecified).
 // y[b][n] = (addend ? addend[b][n] : 0) + bias[n] + sum_k x[b][k] W[n][k];  pre <- y (before mask), post <- y*mask
 int linear_fwd(const float* x, int ldx, const float* W, int ldw, const float* bias, const float* addend, int ld_add,
                const float* mask, float* pre, float* post, int ld_out, float* post2, int ld_out2,
-               int B, int N, int K, cudaStream_t st, int groups = 1, long long wstride = 0);
+               int B, int N, int K, cudaStream_t st, int groups = 1, long long wstride = 0, unsigned long long active = ~0ULL);
 // dx[b][k] = sum_n dy[b][n] W[n][k] (k < K)
 int linear_dgrad(const float* dy, int ldy, const float* W, int ldw, float* dx, int ldx, int B, int N, int K,
-                 float* ws, size_t ws_floats, cudaStream_t st, int groups = 1, long long wstride = 0);
+                 float* ws, size_t ws_floats, cudaStream_t st, int groups = 1, long long wstride = 0, unsigned long long active = ~0ULL);
 // dW[n][k] += sum_r dy[r][n] x[r][k];  db[n] += sum_r dy[r][n].  The R rows are `R / B` slabs of B rows; group g reduces the
 // rows g * B / groups .. (g + 1) * B / groups - 1 of every slab into dW / db + g * wstride (groups = 1: B is ignored)
 int linear_wgrad(const float* dy, int ldy, const float* x, int ldx, float* dW, int ldw, float* db, int R, int N, int K, cudaStream_t st,
-                 int groups = 1, int B = 0, long long wstride = 0);
+                 int groups = 1, int B = 0, long long wstride = 0, unsigned long long active = ~0ULL);
 int rot6d_fwd_launch(const float* pose6d, float* rotmat, int n, cudaStream_t st);
 int rot6d_bwd_launch(const float* pose6d, const float* drot, float* dpose, int n, cudaStream_t st);
 int ew_mul(const float* a, const float* b, float* out, size_t n, cudaStream_t st);

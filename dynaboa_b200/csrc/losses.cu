@@ -276,15 +276,20 @@ int loss_multi_launch(const LossArgs& a, cudaStream_t st) {
 // ---------------------------------------------------------------------------------------------
 // motion loss between the current prediction (a) and the prediction on the history frame (h)
 //   L = mean_{B*count*2} [conf_a + conf_h == 2] * ((pa - ph) - (ka - kh))^2   on joints [first, first + count)  (benchmark: 25..48)
+// A video whose `active` bit is clear gets term 0 and leaves its rows of dpa and dph untouched.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) loss_motion_kernel(const float* __restrict__ pa, const float* __restrict__ ph,
                                                           const float* __restrict__ ka, const float* __restrict__ kh, float w,
                                                           float* __restrict__ term, float* __restrict__ dpa, float* __restrict__ dph,
-                                                          int B, int acc_a, int first, int count) {
+                                                          int B, int acc_a, int first, int count, unsigned long long active) {
     pdl_wait();
     pdl_trigger();
     __shared__ float red[32];
     B /= gridDim.x;                                          // grouped: block g takes video g's B rows
+    if (blockIdx.x < 64 && !((active >> blockIdx.x) & 1ULL)) {
+        if (threadIdx.x == 0) term[blockIdx.x] = 0.f;
+        return;
+    }
     {
         const size_t r = (size_t)blockIdx.x * B;
         pa += r * 98; ph += r * 98; ka += r * 147; kh += r * 147; dpa += r * 98; dph += r * 98; term += blockIdx.x;
@@ -308,11 +313,11 @@ __global__ void __launch_bounds__(256) loss_motion_kernel(const float* __restric
     if (threadIdx.x == 0) term[0] = acc / n;
 }
 int loss_motion_launch(const float* pa, const float* ph, const float* ka, const float* kh, float w, float* term, float* dpa, float* dph,
-                       int B, int acc_a, int first, int count, cudaStream_t st, int groups) {
+                       int B, int acc_a, int first, int count, cudaStream_t st, int groups, unsigned long long active) {
     if (first < 0 || count < 1 || first + count > 49) return DBOA_ERR_ARG;
     if (groups < 1 || B % groups != 0) return DBOA_ERR_SHAPE;
     return launch_ex(loss_motion_kernel, dim3(groups), dim3(256), 0, st, dim3(1, 1, 1), true, pa, ph, ka, kh, w, term, dpa, dph, B, acc_a, first,
-                     count);
+                     count, active);
 }
 
 }  // namespace dboa

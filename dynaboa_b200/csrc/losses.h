@@ -16,6 +16,6 @@ int gmm_prior_launch(const float* pose69, const float* means, const float* prec,
                      float scale, int B, cudaStream_t st);
 int loss_multi_launch(const LossArgs& a, cudaStream_t st);
 int loss_motion_launch(const float* pa, const float* ph, const float* ka, const float* kh, float w, float* term, float* dpa, float* dph,
-                       int B, int acc_a, int first, int count, cudaStream_t st, int groups = 1);
+                       int B, int acc_a, int first, int count, cudaStream_t st, int groups = 1, unsigned long long active = ~0ULL);
 
 }  // namespace dboa

@@ -29,7 +29,8 @@ __device__ __forceinline__ float lds_imm(uint32_t a) {
 }
 
 __global__ void __launch_bounds__(NT) stem_wgrad_kernel(const float* __restrict__ dy, const float* __restrict__ x, float* __restrict__ part,
-                                                        int B, int rows_per_cta) {
+                                                        int B, int rows_per_cta, unsigned long long active) {
+    if (!((active >> blockIdx.y) & 1ULL)) return;           // grouped: an idle group computes no partials
     extern __shared__ __align__(16) float sm[];
     float* dys = sm;                        // [112][64]
     float* xs = sm + HO * CO;               // [7][ROWF]: xs[r][(wi + 3) * 3 + ci], rows hi = 2 ho - 3 + r
@@ -90,7 +91,8 @@ __global__ void __launch_bounds__(NT) stem_wgrad_kernel(const float* __restrict_
 }
 
 __global__ void __launch_bounds__(256) stem_wgrad_reduce_kernel(const float* __restrict__ part, float* __restrict__ dw, int nparts, int kpitch,
-                                                                long long wstride) {
+                                                                long long wstride, unsigned long long active) {
+    if (!((active >> blockIdx.y) & 1ULL)) return;           // grouped: nothing is added to an idle group's gradient
     pdl_wait();
     pdl_trigger();
     part += (size_t)blockIdx.y * nparts * (CO * KK);          // grouped: group blockIdx.y's partials into its own gradient
@@ -119,9 +121,9 @@ int stem_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, fl
     if (ws == nullptr || max_parts < 1) return DBOA_ERR_UNSUPPORTED;
     const int rows_per = ceil_div(rows, max_parts), nparts = ceil_div(rows, rows_per);
     DBOA_TRY(launch_ex(stem::stem_wgrad_kernel, dim3(nparts, d.groups), dim3(stem::NT), (size_t)stem::SMEM_FLOATS * sizeof(float), st, dim3(1, 1, 1),
-                       true, dy, x, ws, d.B, rows_per));
+                       true, dy, x, ws, d.B, rows_per, d.active));
     return launch_ex(stem::stem_wgrad_reduce_kernel, dim3(ceil_div(stem::CO * stem::KK, 256), d.groups), dim3(256), 0, st, dim3(1, 1, 1), true,
-                     (const float*)ws, dw, nparts, d.Kpitch, d.wstride);
+                     (const float*)ws, dw, nparts, d.Kpitch, d.wstride, d.active);
 }
 
 }  // namespace dboa

@@ -14,7 +14,9 @@ What changes relative to the autograd path (``Adaptor.adaptation``), none of it 
 
 The same step adapts G videos at once (``multivideo.MultiVideoAdaptor``): their weight, teacher and gradient arenas are
 (G, P) stacks instead of flat arenas, video g owns the rows [g * b, (g + 1) * b) of every batch, and every network pass and
-loss head is one grouped call.  DESIGN.md section 10.
+loss head is one grouped call.  When only some of the videos advance this frame (``ad.active``, an int whose bit g means video
+g takes part; None: all), the network passes skip the others and the element-wise sweeps touch only the active videos' rows of
+the stacks.  DESIGN.md section 10.
 """
 import ctypes as C
 import os
@@ -50,9 +52,28 @@ def _groups(arena):
     return arena.shape[0] if arena.dim() == 2 else 1
 
 
+def runs(mask, G, key=lambda g: 0):
+    """[a, b) ranges of consecutive videos whose bit is set in ``mask`` and that share ``key(g)``."""
+    out = []
+    for g in range(G):
+        if (mask >> g) & 1:
+            if out and out[-1][1] == g and key(out[-1][0]) == key(g):
+                out[-1][1] = g + 1
+            else:
+                out.append([g, g + 1])
+    return out
+
+
+def _active_rows(ad, t):
+    """``t`` itself, or, for a (G, P) stack while only some videos take part, the views of its runs of active videos: element-wise
+    sweeps over them leave the idle videos' rows untouched, and with every video active they are one sweep as before."""
+    act = getattr(ad, 'active', None)
+    return [t] if act is None else [t[a:b] for a, b in runs(act, t.shape[0])]
+
+
 class _Pred:
     """Everything one forward graph produces (kept for its backward)."""
-    __slots__ = ('image', 'rot', 'shape', 'cam', 'tape', 'verts', 'joints', 'smpl_tape', 'p2d', 'B', 'masked', 'groups')
+    __slots__ = ('image', 'rot', 'shape', 'cam', 'tape', 'verts', 'joints', 'smpl_tape', 'p2d', 'B', 'masked', 'groups', 'active')
 
 
 def _smpl_fwd(smpl, betas, rot):
@@ -64,10 +85,10 @@ def _smpl_fwd(smpl, betas, rot):
     return verts, joints, tape
 
 
-def forward_graph(ad, arena, buffers, image, masks=None):
+def forward_graph(ad, arena, buffers, image, masks=None, active=None):
     p = _Pred()
-    p.image, p.B, p.masked, p.groups = image, image.shape[0], masks is not None, _groups(arena)
-    p.rot, p.shape, p.cam, _, p.tape = hmr_mod.raw_forward(arena, buffers, image, masks, groups=p.groups)
+    p.image, p.B, p.masked, p.groups, p.active = image, image.shape[0], masks is not None, _groups(arena), active
+    p.rot, p.shape, p.cam, _, p.tape = hmr_mod.raw_forward(arena, buffers, image, masks, groups=p.groups, active=active)
     p.verts, p.joints, p.smpl_tape = _smpl_fwd(ad.smpl_neutral, p.shape, p.rot)
     p.p2d = torch.empty(p.B, 49, 2, dtype=torch.float32, device=image.device)
     _lib.call('dboa_project_fwd', ptr(p.cam), ptr(p.joints), ptr(p.p2d), p.B, 49, stream())
@@ -126,22 +147,26 @@ def backward_graph(ad, arena, p, dp2d, dj3d, dR, dbeta, grad_arena, sync=None):
               ptr(dbeta), 1, stream())
     if sync is not None:
         sync.arm()
-    hmr_mod.raw_backward(arena, p.tape, B, p.masked, dR, dbeta, dcam, grad_arena, groups=p.groups)
+    hmr_mod.raw_backward(arena, p.tape, B, p.masked, dR, dbeta, dcam, grad_arena, groups=p.groups, active=p.active)
     if sync is not None:
         sync.after_backward(grad_arena)
         ad.optimizer.reduced = True
 
 
-def retrieve(ad, rows, rngs):
+def retrieve(ad, rows, rngs, active=None):
     """reference :82-96 for every video: the nearest cluster centre of video g's feature row ``rows[g]`` by cosine distance
     (one host synchronisation for all videos), then ``rngs[g].sample`` inside that cluster.  Returns the (cluster, picks) of
-    every video and the picked exemplar rows, video after video."""
+    every video and the picked exemplar rows, video after video.  ``active`` (bit mask, None: all): an idle video draws
+    nothing, gets None and placeholder rows (exemplar 0)."""
+    on = [active is None or bool((active >> g) & 1) for g in range(len(rows))]
     for g, f in enumerate(rows):
+        if not on[g]:
+            continue
         f = f.contiguous()
         _lib.call('dboa_retrieval_nearest', ptr(f), ptr(ad.centers), ad.centers.shape[0], 2048, C.c_void_p(ad._best.data_ptr() + 4 * g),
                   ptr(ad._dists), stream())
-    picked = [(c, rng.sample(ad.index[c], ad.options.sample_num)) for c, rng in zip(ad._best.tolist(), rngs)]
-    idx = torch.as_tensor([i for _, picks in picked for i in picks], dtype=torch.long, device=rows.device)
+    picked = [(c, rng.sample(ad.index[c], ad.options.sample_num)) if a else None for c, rng, a in zip(ad._best.tolist(), rngs, on)]
+    idx = torch.as_tensor([i for p in picked for i in (p[1] if p else [0] * ad.options.sample_num)], dtype=torch.long, device=rows.device)
     return picked, {k: v.index_select(0, idx) for k, v in ad.h36m_bank.items()}
 
 
@@ -162,7 +187,14 @@ def level_backward(ad, arena, buffers, image, kp, lower, grad_arena, main=None, 
     per_video = arena.shape[:-1]                                # shape of the losses recorded and returned: () or (G,)
     use_frame = o.use_frame_losses_lower if lower else o.use_frame_losses_upper
     use_temporal = o.use_temporal_losses_lower if lower else o.use_temporal_losses_upper
-    motion = bool(use_temporal and o.use_motion and (ad.global_step - o.interval) > 0)
+    act = getattr(ad, 'active', None)                           # videos taking part (bit mask; None: all)
+    # videos whose motion term is live (bit mask): all of them or none, by the frame count, unless the adaptor keeps one per video
+    every = (1 << G) - 1
+    live = getattr(ad, 'motion_active', None)
+    if live is None:
+        live = every if (ad.global_step - o.interval) > 0 else 0
+    motion = bool(use_temporal and o.use_motion and live)
+    live = None if live == every else live
     # the teacher forward is independent of the fast-weight forward: issue it on a side stream so that the two chains
     # of small, latency-bound kernels overlap on the GPU (each one alone leaves most SMs idle at batch 1)
     tpred, side = None, None
@@ -172,7 +204,7 @@ def level_backward(ad, arena, buffers, image, kp, lower, grad_arena, main=None, 
             side = _side_stream(image.device)
             side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):                           # None: the caller's stream
-            tpred = forward_graph(ad, teacher.arena, teacher._buffers, image, teacher._masks(nb, image.device))
+            tpred = forward_graph(ad, teacher.arena, teacher._buffers, image, teacher._masks(nb, image.device), act)
     if motion:
         hist_image, hist_kp = ad.get_hist()
         if main is None and G == 1:
@@ -184,9 +216,9 @@ def level_backward(ad, arena, buffers, image, kp, lower, grad_arena, main=None, 
             _lib.call('dboa_copy_async', C.c_void_p(pair.data_ptr() + half), ptr(hist_image.contiguous()), half, stream())
             main = forward_graph(ad, arena, buffers, pair)
     if main is None:
-        main = forward_graph(ad, arena, buffers, image)
+        main = forward_graph(ad, arena, buffers, image, active=act)
     batched = main.B > nb
-    hist = forward_graph(ad, arena, buffers, hist_image) if motion and not batched else None
+    hist = forward_graph(ad, arena, buffers, hist_image, active=live) if motion and not batched else None
     w = [0.0] * 8
     targets = {}
     if use_frame:
@@ -223,8 +255,12 @@ def level_backward(ad, arena, buffers, image, kp, lower, grad_arena, main=None, 
         p_hist = main.p2d[nb:] if batched else hist.p2d
         dph = dp2d[nb:] if batched else torch.empty_like(hist.p2d)
         kf, kn = getattr(ad, 'kp_range', (25, 24))
-        _lib.call('dboa_loss_motion_groups', ptr(main.p2d), ptr(p_hist), ptr(kp), ptr(hist_kp.contiguous()), float(o.motionloss_weight),
-                  ptr(mterm), ptr(dp2d), ptr(dph), nb, 1, kf, kn, G, stream())
+        margs = (ptr(main.p2d), ptr(p_hist), ptr(kp), ptr(hist_kp.contiguous()), float(o.motionloss_weight), ptr(mterm), ptr(dp2d), ptr(dph),
+                 nb, 1, kf, kn, G)
+        if live is None:
+            _lib.call('dboa_loss_motion_groups', *margs, stream())
+        else:
+            _lib.call('dboa_loss_motion_active', *margs, live, stream())
         if not batched:
             backward_graph(ad, arena, hist, dph, torch.zeros_like(hist.joints), torch.zeros_like(hist.rot), torch.zeros_like(hist.shape),
                            grad_arena)
@@ -236,10 +272,13 @@ def level_backward(ad, arena, buffers, image, kp, lower, grad_arena, main=None, 
     _mark(ad, f'{tag}: backward')
     if o.retrieval:
         rows = hmr_mod._feature_views(main.tape, main.B)[5][:nb].reshape(G, -1, 2048)[:, 0]      # each video's first sample
-        picked, ex = retrieve(ad, rows, getattr(ad, 'rngs', [random]))
-        ad.last_retrieval = picked if per_video else picked[0]
+        picked, ex = retrieve(ad, rows, getattr(ad, 'rngs', [random]), act)
+        if per_video:
+            ad.last_retrieval = [p if p is not None else q for p, q in zip(picked, ad.last_retrieval)]
+        else:
+            ad.last_retrieval = picked[0]
         if mix:
-            e = forward_graph(ad, arena, buffers, ex['img'])
+            e = forward_graph(ad, arena, buffers, ex['img'], active=act)
             n = e.B
             gt_R = torch.empty(n, 24, 3, 3, dtype=torch.float32, device=image.device)
             _lib.call('dboa_rodrigues', ptr(ex['pose'].reshape(-1, 3).contiguous()), ptr(gt_R), n * 24, 0, stream())
@@ -276,7 +315,7 @@ def fused_adapt(ad, batch):
     evaluate = getattr(ad, 'fused_eval', 'final')
     with torch.no_grad():
         _mark(ad, 'start')
-        probe = forward_graph(ad, theta, buffers, image)            # init_features (reference :132-133)
+        probe = forward_graph(ad, theta, buffers, image, active=getattr(ad, 'active', None))       # init_features (reference :132-133)
         _mark(ad, 'probe forward')
         import torch.distributed as tdist
         sync = opt.grad_sync if (opt.grad_sync is not None and tdist.is_initialized() and tdist.get_world_size() > 1) else None
@@ -290,16 +329,19 @@ def fused_adapt(ad, batch):
             ad._fast_bufs = [torch.empty_like(theta), torch.empty_like(theta)]
             ad._inner_grad = torch.empty_like(theta)
         for i in range(o.inner_step):
-            _zero(ad._inner_grad)
+            for t in _active_rows(ad, ad._inner_grad):
+                _zero(t)
             level_backward(ad, fast, buffers, image, kp, True, ad._inner_grad, main=cur if i == 0 else None)
             _mark(ad, 'lower level (loss + backward)')
             nxt = ad._fast_bufs[i % 2]
-            _lib.call('dboa_sgd_update', ptr(fast), ptr(ad._inner_grad), ptr(nxt), float(o.fastlr), theta.numel(), stream())
+            for f, g, n in zip(_active_rows(ad, fast), _active_rows(ad, ad._inner_grad), _active_rows(ad, nxt)):
+                _lib.call('dboa_sgd_update', ptr(f), ptr(g), ptr(n), float(o.fastlr), f.numel(), stream())
             fast = nxt
             _mark(ad, 'inner SGD step')
             if evaluate == 'all':
                 ad.inference(batch, _ArenaModel(model, fast))
-        _zero(grad)
+        for t in _active_rows(ad, grad):
+            _zero(t)
         ad.last_upper_loss, _ = level_backward(ad, fast, buffers, image, kp, False, grad, sync=sync)
         _mark(ad, 'upper level (forward + loss + backward)')
         opt.step(teacher=teacher, alpha=o.alpha)                    # Adam + EMA teacher, one sweep

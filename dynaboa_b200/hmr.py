@@ -151,11 +151,12 @@ def _check_groups(arena, B, groups):
         raise ValueError(f'a grouped call needs one contiguous ({groups}, {layout().floats}) arena stack')
 
 
-def raw_forward(arena, buffers, image, masks=None, tape=None, groups=1):
+def raw_forward(arena, buffers, image, masks=None, tape=None, groups=1, active=None):
     """One ``dboa_hmr_forward_groups`` call.  Returns (rotmat, shape, cam, pose6d, tape).  No autograd.
 
     ``groups`` > 1: ``arena`` is a (groups, P) stack, and video g's weights ``arena[g]`` see the samples
-    [g * B / groups, (g + 1) * B / groups) of ``image`` (and of ``masks`` and the outputs)."""
+    [g * B / groups, (g + 1) * B / groups) of ``image`` (and of ``masks`` and the outputs).  ``active``: an int whose bit g
+    means video g takes part (``dboa_hmr_forward_active``); the rows of the other videos are left unspecified.  None: all."""
     _lib.require_cuda(arena, image)
     B = image.shape[0]
     if tuple(image.shape[1:]) != (3, 224, 224):
@@ -173,20 +174,29 @@ def raw_forward(arena, buffers, image, masks=None, tape=None, groups=1):
         masks = masks.contiguous().float()
         if tuple(masks.shape) != (3, 2, B, 1024):
             raise ValueError('dropout masks must be (3,2,B,1024)')
-    _lib.call('dboa_hmr_forward_groups', ptr(arena), ptr(buffers['init_pose']), ptr(buffers['init_shape']), ptr(buffers['init_cam']),
-              ptr(image), B, ptr(masks), ptr(tape), ptr(scratch_for(B, dev)), ptr(rot), ptr(shape), ptr(cam), ptr(pose6d), stream(), groups)
+    args = (ptr(arena), ptr(buffers['init_pose']), ptr(buffers['init_shape']), ptr(buffers['init_cam']), ptr(image), B, ptr(masks),
+            ptr(tape), ptr(scratch_for(B, dev)), ptr(rot), ptr(shape), ptr(cam), ptr(pose6d), stream(), groups)
+    if active is None:
+        _lib.call('dboa_hmr_forward_groups', *args)
+    else:
+        _lib.call('dboa_hmr_forward_active', *args, int(active))
     return rot, shape, cam, pose6d, tape
 
 
-def raw_backward(arena, tape, B, masked, d_rot, d_shape, d_cam, grad_arena, groups=1):
+def raw_backward(arena, tape, B, masked, d_rot, d_shape, d_cam, grad_arena, groups=1, active=None):
     """One ``dboa_hmr_backward_groups`` call: accumulates into ``grad_arena`` (flat, arena layout).  ``groups`` > 1: ``arena``
-    and ``grad_arena`` are both (groups, P) stacks (see ``raw_forward``)."""
+    and ``grad_arena`` are both (groups, P) stacks (see ``raw_forward``).  ``active``: as in ``raw_forward``
+    (``dboa_hmr_backward_active``); the gradient arenas of the other videos are not written."""
     _check_groups(arena, B, groups)
     _check_groups(grad_arena, B, groups)
     c = lambda t: None if t is None else t.contiguous().float()
     d_rot, d_shape, d_cam = c(d_rot), c(d_shape), c(d_cam)
-    _lib.call('dboa_hmr_backward_groups', ptr(arena), ptr(tape), B, int(masked), ptr(d_rot), ptr(d_shape), ptr(d_cam), ptr(grad_arena),
-              ptr(scratch_for(B, tape.device)), stream(), groups)
+    args = (ptr(arena), ptr(tape), B, int(masked), ptr(d_rot), ptr(d_shape), ptr(d_cam), ptr(grad_arena), ptr(scratch_for(B, tape.device)),
+            stream(), groups)
+    if active is None:
+        _lib.call('dboa_hmr_backward_groups', *args)
+    else:
+        _lib.call('dboa_hmr_backward_active', *args, int(active))
 
 
 class _HMRFunction(torch.autograd.Function):

@@ -2,11 +2,13 @@
 every network forward and backward one grouped call (``dboa_hmr_forward_groups`` / ``dboa_hmr_backward_groups``).  This module
 holds only the per-video state.
 
-Each video keeps the reference's semantics: its own theta, Adam moments, teacher, fast weights, gradient, history ring,
-teacher dropout masks and retrieval picks.  The G weight arenas (and the teachers', the moments', the gradients') are one
-contiguous (G, P) stack; video g owns the rows [g * b, (g + 1) * b) of every per-sample batch.  What the videos share is the
-launch sequence and the step count of Adam (all videos advance together).  DESIGN.md section 10.
+Each video keeps the reference's semantics: its own theta, Adam moments and step count, teacher, fast weights, gradient,
+history ring, motion warm-up, teacher dropout masks and retrieval picks.  The G weight arenas (and the teachers', the moments',
+the gradients') are one contiguous (G, P) stack; video g owns the rows [g * b, (g + 1) * b) of every per-sample batch.  The
+G slots are a pool: a slot whose batch is None sits the frame out (its CTAs return at once in every grouped call), and
+``start(g)`` puts a new video into slot g.  DESIGN.md section 10.
 """
+import ctypes as C
 import random
 from types import SimpleNamespace
 
@@ -14,7 +16,7 @@ import torch
 
 from . import _lib, hmr as hmr_mod
 from ._lib import ptr, stream
-from .fused import fused_adapt
+from .fused import fused_adapt, runs
 
 
 def check_options(options, n_videos):
@@ -38,41 +40,62 @@ def check_options(options, n_videos):
 
 
 class MultiVideoAdaptor:
-    """``MultiVideoAdaptor(options, n_videos)``: every video starts from ``options.model_file`` as a fresh ``Adaptor`` does.
+    """``MultiVideoAdaptor(options, n_videos)``: a pool of G slots, each holding one video that starts from
+    ``options.model_file`` as a fresh ``Adaptor`` does.
 
-    ``adapt(batches)`` advances all videos by one frame (one batch dict per video, ``batch_size`` 1).  ``predict(images)``,
-    ``theta(g)``, ``last_upper_loss`` ((G,) device tensor).  ``mask_provider(g, B, device)`` -> (3, 2, B, 1024) keep-masks of
-    video g's teacher forward (None: drawn with torch's CUDA RNG, as ``HMR``).  ``rngs[g]``: the ``random.Random`` of video g's
-    retrieval picks; ``last_retrieval[g]``: video g's (cluster, picks)."""
+    ``adapt(batches)`` advances every slot whose entry is a batch dict (``batch_size`` 1) by one frame; a None entry leaves that
+    slot as it was.  ``start(g, seed=None)`` puts a new video into slot g.  ``predict(images)``, ``theta(g)``,
+    ``last_upper_loss`` ((G,) device tensor).  ``video_steps[g]``: frames slot g adapted since its ``start``; ``global_step``:
+    ``adapt`` calls.  ``mask_provider(g, B, device)`` -> (3, 2, B, 1024) keep-masks of video g's teacher forward (None: drawn
+    with torch's CUDA RNG, as ``HMR``).  ``rngs[g]``: the ``random.Random`` of video g's retrieval picks; ``last_retrieval[g]``:
+    video g's (cluster, picks)."""
 
     def __init__(self, options, n_videos):
         check_options(options, n_videos)
         from .adaptor import Adaptor
         self.G = G = int(n_videos)
         self.options = o = options
-        self.base = base = Adaptor(options)        # checkpoint, SMPL, prior, exemplar bank; its weights are video 0's start
+        self.base = base = Adaptor(options)        # checkpoint, SMPL, prior, exemplar bank; never adapted, so it keeps the checkpoint
         self.smpl_neutral, self.gmm_f = base.smpl_neutral, base.gmm_f
         if o.retrieval:
             self.centers, self.index, self.h36m_bank, self._dists = base.centers, base.index, base.h36m_bank, base._dists
             self._best = torch.zeros(G, dtype=torch.int32, device=base.device)
         model = base.model.module
-        self.thetas = model.arena.detach().repeat(G, 1)
+        self.thetas = torch.empty(G, model.arena.numel(), device=model.arena.device)
         self.buffers = model._buffers
-        self.teachers = base.teacher.arena.detach().repeat(G, 1) if o.use_meanteacher else None
-        self.m, self.v, self.grad = torch.zeros_like(self.thetas), torch.zeros_like(self.thetas), torch.zeros_like(self.thetas)
-        self.step_count = 0
+        self.teachers = torch.empty_like(self.thetas) if o.use_meanteacher else None
+        self.m, self.v, self.grad = torch.empty_like(self.thetas), torch.empty_like(self.thetas), torch.zeros_like(self.thetas)
         # what fused_adapt reads from a single-video adaptor's model, teacher and optimizer, over the (G, P) stacks
         self.model = SimpleNamespace(arena=self.thetas, _buffers=self.buffers, grad_arena=lambda: self.grad)
         self.teacher = SimpleNamespace(arena=self.teachers, _buffers=self.buffers, _masks=self._teacher_masks)
         self.optimizer = SimpleNamespace(step=self._adam_ema, grad_sync=None)
         self.fused_eval = 'none'
         self.global_step = 0
-        self.history = {}
         self.mask_provider = None
-        self.rngs = [random.Random(o.seed * 1000 + g) for g in range(G)]
         self.last_upper_loss = torch.zeros(G, device=self.thetas.device)
         self.last_retrieval = [None] * G
         self.teacher_dropout = bool(getattr(o, 'teacher_dropout', 1))
+        self.step_counts, self.video_steps, self.histories, self.rngs = [0] * G, [0] * G, [{} for _ in range(G)], [None] * G
+        self._on = (1 << G) - 1            # slots taking part in the current frame (bit mask)
+        self.active = None                 # what fused_adapt reads: None while every slot takes part, else _on
+        self.motion_active = 0             # slots of the current frame whose motion term is live (bit mask)
+        self._frames = self._hist = None   # persistent staging of the current frame's and the history frame's rows
+        for g in range(G):
+            self.start(g)
+
+    def start(self, g, seed=None):
+        """Put a new video into slot g: theta and teacher from the checkpoint, zero Adam moments, step and frame counts, an empty
+        history, and ``rngs[g] = random.Random(seed)`` (default ``options.seed * 1000 + g``)."""
+        if not isinstance(g, int) or not 0 <= g < self.G:
+            raise ValueError(f'slot {g!r} is not one of the {self.G} slots')
+        self.thetas[g].copy_(self.base.model.module.arena.detach())
+        if self.teachers is not None:
+            self.teachers[g].copy_(self.base.teacher.arena.detach())
+        self.m[g].zero_()
+        self.v[g].zero_()
+        self.step_counts[g] = self.video_steps[g] = 0
+        self.histories[g].clear()
+        self.rngs[g] = random.Random(self.options.seed * 1000 + g if seed is None else seed)
 
     def theta(self, g):
         """View of video g's weights (flat arena layout)."""
@@ -85,41 +108,104 @@ class MultiVideoAdaptor:
                              'across ranks')
         check_options(self.options, self.G)
 
+    def _slots(self, mask):
+        return [g for g in range(self.G) if (mask >> g) & 1]
+
     def save_hist(self, image, s2d):
-        self.history[self.global_step] = (image.clone(), s2d.clone())
-        self.history.pop(self.global_step - self.options.interval - 1, None)
+        """One copy of the frame's staged rows, kept by every active slot under its own frame count."""
+        frame = (image.clone(), s2d.clone())
+        for g in self._slots(self._on):
+            h, k = self.histories[g], self.video_steps[g]
+            h[k] = frame
+            h.pop(k - self.options.interval - 1, None)
 
     def get_hist(self):
-        return self.history[self.global_step - self.options.interval]
+        """The history rows of the slots whose motion term is live, each from its own frame ``interval`` frames back; the rows of
+        the other slots are placeholders."""
+        live = self._slots(self.motion_active)
+        frames = [self.histories[g][self.video_steps[g] - self.options.interval] for g in live]
+        if len(live) == self.G and all(f is frames[0] for f in frames):
+            return frames[0]                                     # one pool frame holds every slot's history rows
+        if self._hist is None:
+            self._hist = tuple(torch.zeros_like(t) for t in frames[0])
+        for g, frame in zip(live, frames):
+            for dst, src in zip(self._hist, frame):
+                n = src.numel() // self.G * src.element_size()
+                _lib.call('dboa_copy_async', C.c_void_p(dst.data_ptr() + g * n), C.c_void_p(src.data_ptr() + g * n), n, stream())
+        return self._hist
 
     def _teacher_masks(self, B, device):
         if not self.teacher_dropout:
             return None
         b, per = B // self.G, []
         for g in range(self.G):
+            if not (self._on >> g) & 1:
+                per.append(torch.ones(3, 2, b, 1024, device=device))       # placeholder rows: no draw for an idle slot
+                continue
             m = self.mask_provider(g, b, device) if self.mask_provider is not None else None
             per.append(m if m is not None else (torch.rand(3, 2, b, 1024, device=device) >= 0.5).float() * 2.0)
         return torch.cat(per, 2)
 
     def _adam_ema(self, teacher=None, alpha=0.0):
-        """Adam + EMA teacher over all G arenas in one sweep; the videos advance together and share the step count."""
+        """Adam + EMA teacher of the active slots, each at its own step count: one sweep per run of consecutive active slots
+        that share a step count (one sweep over the whole stack while every slot runs in step)."""
         o = self.options
-        self.step_count += 1
+        for g in self._slots(self._on):
+            self.step_counts[g] += 1
         t = None if teacher is None else teacher.arena
-        _lib.call('dboa_adam_ema_scaled', ptr(self.thetas), ptr(self.grad), ptr(self.m), ptr(self.v), ptr(t), self.thetas.numel(),
-                  float(o.lr), float(o.beta1), float(o.beta2), 1e-8, self.step_count, float(alpha), 1.0, stream())
+        for a, b in runs(self._on, self.G, key=lambda g: self.step_counts[g]):
+            _lib.call('dboa_adam_ema_scaled', ptr(self.thetas[a:b]), ptr(self.grad[a:b]), ptr(self.m[a:b]), ptr(self.v[a:b]),
+                      ptr(None if t is None else t[a:b]), self.thetas[a:b].numel(), float(o.lr), float(o.beta1), float(o.beta2), 1e-8,
+                      self.step_counts[a], float(alpha), 1.0, stream())
+
+    def _stage(self, batches):
+        """Copy the active slots' frames into the persistent (G b, ...) batch; the rows of idle slots keep what they held."""
+        dev = self.thetas.device
+        first = next(b for b in batches if b is not None)
+        if self._frames is None:
+            self._frames = {k: torch.zeros((self.G * first[k].shape[0],) + tuple(first[k].shape[1:]), dtype=torch.float32, device=dev)
+                            for k in ('image', 'smpl_j2d')}
+        for g, bt in enumerate(batches):
+            if bt is None:
+                continue
+            for k, buf in self._frames.items():
+                src = bt[k].to(dev).contiguous().float()
+                rows = buf.shape[0] // self.G
+                if tuple(src.shape) != (rows,) + tuple(buf.shape[1:]):
+                    raise ValueError(f'slot {g}: {k} of shape {tuple(src.shape)}, expected {(rows,) + tuple(buf.shape[1:])}')
+                n = src.numel() * 4
+                _lib.call('dboa_copy_async', C.c_void_p(buf.data_ptr() + g * n), ptr(src), n, stream())
+        return self._frames
 
     # ------------------------------------------------------------------ public
     def adapt(self, batches):
-        """One frame of every video (``batches[g]`` is video g's batch dict): ``fused.fused_adapt`` over all G videos -- probe
-        forward, K inner SGD steps, the upper level with teacher and motion terms, retrieval with exemplar mix-training, then
-        Adam + EMA teacher.  ``fit_losses`` and ``kp2dlosses_lower`` / ``kp2dlosses_upper`` hold this frame's (G,) losses."""
-        self._check_runtime()
+        """One frame of every slot whose entry is a batch (``batches[g]`` is slot g's batch dict, None: slot g sits this frame
+        out): ``fused.fused_adapt`` over the active slots -- probe forward, K inner SGD steps, the upper level with teacher and
+        motion terms, retrieval with exemplar mix-training, then Adam + EMA teacher.  ``fit_losses`` and ``kp2dlosses_lower`` /
+        ``kp2dlosses_upper`` hold this frame's (G,) losses, NaN for idle slots; ``last_upper_loss[g]`` of an idle slot keeps its
+        value."""
         if len(batches) != self.G:
             raise ValueError(f'expected {self.G} batches, one per video, got {len(batches)}')
-        batch = {k: torch.cat([b[k] for b in batches]).to(self.thetas.device) for k in ('image', 'smpl_j2d')}
+        on = sum(1 << g for g, b in enumerate(batches) if b is not None)
+        if on == 0:
+            raise ValueError('at least one slot needs a batch')
+        self._check_runtime()
+        o, every = self.options, (1 << self.G) - 1
+        self._on, self.active = on, (None if on == every else on)
+        self.motion_active = sum(1 << g for g in self._slots(on) if self.video_steps[g] - o.interval > 0)
+        batch = self._stage(batches)
+        prev = self.last_upper_loss
         self.fit_losses, self.kp2dlosses_lower, self.kp2dlosses_upper = {}, [], {}
         fused_adapt(self, batch)
+        if self.active is not None:
+            keep = torch.tensor([bool((on >> g) & 1) for g in range(self.G)], device=prev.device)
+            nan = lambda t: torch.where(keep, t, torch.full_like(t, float('nan')))
+            self.last_upper_loss = torch.where(keep, self.last_upper_loss, prev)
+            self.fit_losses = {k: nan(v) for k, v in self.fit_losses.items()}
+            self.kp2dlosses_lower = [nan(v) for v in self.kp2dlosses_lower]
+            self.kp2dlosses_upper = {k: nan(v) for k, v in self.kp2dlosses_upper.items()}
+        for g in self._slots(on):
+            self.video_steps[g] += 1
         self.global_step += 1
 
     def predict(self, images):

@@ -103,6 +103,20 @@ int dboa_hmr_forward_groups(const float* arena, const float* init_pose, const fl
 int dboa_hmr_backward_groups(const float* arena, const float* tape, int B, int masked, const float* d_rotmat,
                              const float* d_shape, const float* d_cam, float* grad_arena, float* scratch, dboa_stream_t stream,
                              int groups);
+/* The two calls above with only some of the videos taking part: bit g of `active` set means video g is computed.  The grid,
+ * split-K slicing and every other reduction split are those of the unmasked call, whose CTAs of idle videos return at once, so
+ * each active video's outputs, tape rows and gradient are bit-identical to the unmasked call's.  An idle video's gradient arena
+ * is not written; its rows of the outputs, tape and scratch are unspecified (nothing an active video computes reads them).
+ * The _groups calls are these with every one of the `groups` bits set.  Checked before any device access, after the _groups
+ * rules' DBOA_ERR_SHAPE: DBOA_ERR_ARG for active == 0 or a bit at position >= groups; then the _groups DBOA_ERR_UNSUPPORTED rules.
+ * A masked backward call (groups != 1) always consumes an armed bucket request. */
+int dboa_hmr_forward_active(const float* arena, const float* init_pose, const float* init_shape, const float* init_cam,
+                            const float* image, int B, const float* drop_masks, float* tape, float* scratch,
+                            float* rotmat, float* shape, float* cam, float* pose6d, dboa_stream_t stream, int groups,
+                            unsigned long long active);
+int dboa_hmr_backward_active(const float* arena, const float* tape, int B, int masked, const float* d_rotmat,
+                             const float* d_shape, const float* d_cam, float* grad_arena, float* scratch, dboa_stream_t stream,
+                             int groups, unsigned long long active);
 
 /* Gradient buckets of the NEXT dboa_hmr_backward call, for overlapping the data-parallel all-reduce with the backward
  * (SURVEY.md section 8e).  Bucket k spans the floats [dboa_hmr_bucket_offset(k), dboa_hmr_bucket_offset(k - 1)) of the gradient
@@ -259,6 +273,12 @@ int dboa_loss_motion_joints(const float* p_cur, const float* p_hist, const float
 int dboa_loss_motion_groups(const float* p_cur, const float* p_hist, const float* kp_cur, const float* kp_hist, float weight, float* term,
                             float* dp_cur, float* dp_hist, int B, int accumulate_cur, int first, int count, int groups,
                             dboa_stream_t stream);
+/* the same with a per-video enable: a video whose `active` bit is clear gets term[g] = 0 and leaves its rows of dp_cur and
+ * dp_hist untouched.  DBOA_ERR_SHAPE for groups outside 1..64 or B % groups != 0, DBOA_ERR_ARG for active == 0 or a bit at
+ * position >= groups */
+int dboa_loss_motion_active(const float* p_cur, const float* p_hist, const float* kp_cur, const float* kp_hist, float weight, float* term,
+                            float* dp_cur, float* dp_hist, int B, int accumulate_cur, int first, int count, int groups,
+                            unsigned long long active, dboa_stream_t stream);
 
 /* ---- whole-model sweeps, feature test, retrieval -------------------------------------------- */
 int dboa_sgd_update(const float* p, const float* g, float* out, float lr, long long n, dboa_stream_t stream);   /* l2l maml_update */
