@@ -108,6 +108,8 @@ SIGNATURES = {
     'dboa_cosine_pairs': (I, [C.POINTER(P), C.POINTER(P), C.POINTER(L), I, P, L, P, F, P]),
     'dboa_cosine_partial_floats': (L, [C.POINTER(L), I]),
     'dboa_cosine_terms': (I, [C.POINTER(P), C.POINTER(P), C.POINTER(L), I, P, L, P, P]),
+    'dboa_cosine_partial_floats_groups': (L, [C.POINTER(L), I, I]),
+    'dboa_cosine_terms_active': (I, [C.POINTER(P), C.POINTER(P), C.POINTER(L), I, P, L, P, P, I, C.c_ulonglong]),
     'dboa_retrieval_nearest': (I, [P, P, I, I, P, P, P]),
     'dboa_crop_resize_normalize': (I, [P, I, I, I, I, I, I, P, P, I, P, P, I, I, P, P, P, P, P]),
     'dboa_keypoint_transform': (I, [P, I, C.c_double, C.c_double, C.c_double, C.c_double, I, P, P]),

@@ -357,11 +357,29 @@ long long dboa_cosine_partial_floats(const long long* n, int npairs) {
 }
 int dboa_cosine_terms(const float* const* a, const float* const* b, const long long* n, int npairs, float* partial, long long partial_floats,
                       double* terms, dboa_stream_t stream) {
+    return dboa_cosine_terms_active(a, b, n, npairs, partial, partial_floats, terms, stream, 1, 1ULL);
+}
+// groups outside 1..64, or a pair whose length does not split into `groups` equal parts
+static int cosine_groups_shape(const long long* n, int npairs, int groups) {
+    if (groups < 1 || groups > 64) return DBOA_ERR_SHAPE;
+    for (int i = 0; i < npairs; ++i)
+        if (n[i] % groups != 0) return DBOA_ERR_SHAPE;
+    return DBOA_OK;
+}
+long long dboa_cosine_partial_floats_groups(const long long* n, int npairs, int groups) {
+    if (!n || npairs < 1 || npairs > 16) return DBOA_ERR_ARG;
+    DBOA_TRY(cosine_groups_shape(n, npairs, groups));
+    return cosine_partial_floats(n, npairs, groups);
+}
+int dboa_cosine_terms_active(const float* const* a, const float* const* b, const long long* n, int npairs, float* partial,
+                             long long partial_floats, double* terms, dboa_stream_t stream, int groups, unsigned long long active) {
     if (!a || !b || !n || !partial || !terms || npairs < 1 || npairs > 16) return DBOA_ERR_ARG;
-    CosinePairs cp;
+    DBOA_TRY(cosine_groups_shape(n, npairs, groups));
+    if (active == 0 || (groups < 64 && (active >> groups) != 0)) return DBOA_ERR_ARG;
+    CosinePairs cp;                                     // cosine_pairs refuses too small a `partial` before it launches
     cp.npairs = npairs;
     for (int i = 0; i < npairs; ++i) { cp.a[i] = a[i]; cp.b[i] = b[i]; cp.n[i] = n[i]; }
-    return cosine_pairs(cp, partial, (size_t)partial_floats, nullptr, terms, 0.f, ST(stream));
+    return cosine_pairs(cp, partial, (size_t)partial_floats, nullptr, terms, 0.f, ST(stream), groups, active);
 }
 int dboa_retrieval_nearest(const float* feat, const float* centers, int K, int D, int* best, float* dists, dboa_stream_t stream) {
     if (!feat || !centers || !best || !dists) return DBOA_ERR_ARG;

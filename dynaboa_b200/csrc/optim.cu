@@ -95,7 +95,11 @@ int ema_update(float* teacher, const float* p, size_t n, float alpha, cudaStream
 }
 
 // ---------------------------------------------------------------------------------------------
-// cosine similarity of up to 16 tensor pairs in two launches (partials, then a fixed-order finish)
+// cosine similarity of up to 16 tensor pairs in two launches (partials, then a fixed-order finish), for each of up to 64
+// videos on its own part of every pair.  The grids cover the active videos only (blockIdx.y / blockIdx.x of the finish is the
+// k-th active video), so every CTA waits on its predecessor.  A video's blocks chunk its part from the part's first float and
+// its partials sit at the offsets a one-video call would use, shifted by g * blk_off[npairs]: its sums are those of the call
+// on its parts alone, bit for bit.
 // ---------------------------------------------------------------------------------------------
 constexpr int COS_CHUNK = 256 * 16;
 
@@ -103,47 +107,61 @@ __global__ void __launch_bounds__(256) cosine_partial_kernel(CosinePairs cp, flo
     pdl_wait();
     pdl_trigger();
     __shared__ float red[32];
+    const int g = cp.video[blockIdx.y];
     int pair = 0;
     while (pair + 1 < cp.npairs && (int)blockIdx.x >= cp.blk_off[pair + 1]) ++pair;
     const long long beg = (long long)(blockIdx.x - cp.blk_off[pair]) * COS_CHUNK;
     const long long end = beg + COS_CHUNK < cp.n[pair] ? beg + COS_CHUNK : cp.n[pair];
-    const float* a = cp.a[pair];
-    const float* b = cp.b[pair];
+    const float* a = cp.a[pair] + g * cp.n[pair];
+    const float* b = cp.b[pair] + g * cp.n[pair];
     float ab = 0.f, aa = 0.f, bb = 0.f;
     for (long long i = beg + threadIdx.x; i < end; i += 256) {
         float x = a[i], y = b[i];
         ab = fmaf(x, y, ab); aa = fmaf(x, x, aa); bb = fmaf(y, y, bb);
     }
     ab = block_sum(ab, red); aa = block_sum(aa, red); bb = block_sum(bb, red);
-    if (threadIdx.x == 0) { partial[blockIdx.x * 3] = ab; partial[blockIdx.x * 3 + 1] = aa; partial[blockIdx.x * 3 + 2] = bb; }
+    if (threadIdx.x == 0) {
+        float* p = partial + ((size_t)g * cp.blk_off[cp.npairs] + blockIdx.x) * 3;
+        p[0] = ab; p[1] = aa; p[2] = bb;
+    }
 }
 __global__ void cosine_finish_kernel(CosinePairs cp, const float* __restrict__ partial, float* __restrict__ out, double* __restrict__ terms,
                                      float eps) {
     pdl_wait();
     pdl_trigger();
+    const int g = cp.video[blockIdx.x];
     int pair = threadIdx.x;
     if (pair >= cp.npairs) return;
+    partial += (size_t)g * cp.blk_off[cp.npairs] * 3;
     double ab = 0, aa = 0, bb = 0;
     for (int k = cp.blk_off[pair]; k < cp.blk_off[pair + 1]; ++k) { ab += partial[k * 3]; aa += partial[k * 3 + 1]; bb += partial[k * 3 + 2]; }
-    if (terms != nullptr) { terms[pair * 3] = ab; terms[pair * 3 + 1] = aa; terms[pair * 3 + 2] = bb; }
+    const int row = g * cp.npairs + pair;
+    if (terms != nullptr) { terms[row * 3] = ab; terms[row * 3 + 1] = aa; terms[row * 3 + 2] = bb; }
     double na = sqrt(aa), nb = sqrt(bb);
     na = na < eps ? eps : na; nb = nb < eps ? eps : nb;
-    if (out != nullptr) out[pair] = (float)(ab / (na * nb));
+    if (out != nullptr) out[row] = (float)(ab / (na * nb));
 }
-long long cosine_partial_floats(const long long* n, int npairs) {
+long long cosine_partial_floats(const long long* n, int npairs, int groups) {
     long long blocks = 0;
-    for (int i = 0; i < npairs; ++i) blocks += ceil_div(n[i], COS_CHUNK);
-    return 3 * blocks;
+    for (int i = 0; i < npairs; ++i) blocks += ceil_div(n[i] / groups, COS_CHUNK);
+    return 3 * blocks * groups;
 }
-int cosine_pairs(const CosinePairs& cp_in, float* partial, size_t partial_floats, float* out, double* terms, float eps, cudaStream_t st) {
+int cosine_pairs(const CosinePairs& cp_in, float* partial, size_t partial_floats, float* out, double* terms, float eps, cudaStream_t st,
+                 int groups, unsigned long long active) {
     CosinePairs cp = cp_in;
     if (cp.npairs < 1 || cp.npairs > 16) return DBOA_ERR_ARG;
+    int nact = 0;
+    for (int g = 0; g < groups; ++g)
+        if ((active >> g) & 1ULL) cp.video[nact++] = (unsigned char)g;
     cp.blk_off[0] = 0;
-    for (int i = 0; i < cp.npairs; ++i) cp.blk_off[i + 1] = cp.blk_off[i] + ceil_div(cp.n[i], COS_CHUNK);
+    for (int i = 0; i < cp.npairs; ++i) {
+        cp.n[i] /= groups;
+        cp.blk_off[i + 1] = cp.blk_off[i] + ceil_div(cp.n[i], COS_CHUNK);
+    }
     const int nblk = cp.blk_off[cp.npairs];
-    if ((size_t)nblk * 3 > partial_floats) return DBOA_ERR_ARG;
-    DBOA_TRY(launch_ex(cosine_partial_kernel, dim3(nblk), dim3(256), 0, st, dim3(1, 1, 1), true, cp, partial));
-    return launch_ex(cosine_finish_kernel, dim3(1), dim3(32), 0, st, dim3(1, 1, 1), true, cp, partial, out, terms, eps);
+    if ((size_t)nblk * 3 * groups > partial_floats) return DBOA_ERR_ARG;
+    DBOA_TRY(launch_ex(cosine_partial_kernel, dim3(nblk, nact), dim3(256), 0, st, dim3(1, 1, 1), true, cp, partial));
+    return launch_ex(cosine_finish_kernel, dim3(nact), dim3(32), 0, st, dim3(1, 1, 1), true, cp, partial, out, terms, eps);
 }
 
 // nearest cluster centre by cosine distance: one block, warp per centre (round robin)

@@ -297,6 +297,63 @@ def feature_cosines(ad, tape_a, tape_b, B):
     return ad.cal_feature_diff(fa, fb)
 
 
+def feature_test(ad, a, b, stacked, mask):
+    """The dynamic loop's feature test between the forwards ``a`` and ``b``: {video: {i: {'cos': c}}} of every video in ``mask``
+    (a bit mask).  One arena: ``cal_feature_diff`` (it all-reduces under data parallelism).  A (G, P) stack: one
+    ``dboa_cosine_terms_active`` call over the videos in ``mask`` and one copy to the host; each video's cosines and its
+    ``fit_losses['feat_sim/cos_sim']`` entry are formed from its own sums exactly as ``cal_feature_diff`` forms them."""
+    if not stacked:
+        return {0: feature_cosines(ad, a.tape, b.tape, a.B)}
+    from .base_adaptor import _dense_ptr_tensor
+    G, n = a.groups, 15
+    fa = [_dense_ptr_tensor(t) for t in hmr_mod._feature_views(a.tape, a.B)]      # xc (row stride HEAD_LD) is made dense
+    fb = [_dense_ptr_tensor(t) for t in hmr_mod._feature_views(b.tape, b.B)]
+    pa = (C.c_void_p * n)(*[t.data_ptr() for t in fa])
+    pb = (C.c_void_p * n)(*[t.data_ptr() for t in fb])
+    ln = (C.c_longlong * n)(*[t.numel() for t in fa])
+    need = _lib.load().dboa_cosine_partial_floats_groups(ln, n, G)
+    _lib.check(0 if need > 0 else need, 'dboa_cosine_partial_floats_groups')
+    part = getattr(ad, '_cos_partial', None)
+    if part is None or part.numel() < need or part.device != a.rot.device:
+        part = ad._cos_partial = torch.empty(need, dtype=torch.float32, device=a.rot.device)
+    terms = torch.empty(G, n, 3, dtype=torch.float64, device=a.rot.device)
+    _lib.call('dboa_cosine_terms_active', pa, pb, ln, n, ptr(part), part.numel(), ptr(terms), stream(), G, mask)
+    host = terms.cpu()                                                # the one host sync of this test, for every video
+    prev = ad.fit_losses.get('feat_sim/cos_sim')
+    rec = torch.full((G,), float('nan')) if prev is None else prev.clone()
+    out = {}
+    for g in range(G):
+        if (mask >> g) & 1:
+            t = host[g]
+            cos = (t[:, 0] / (t[:, 1].sqrt().clamp_min(1e-12) * t[:, 2].sqrt().clamp_min(1e-12))).float()
+            rec[g] = cos.sum() / (n - 1)
+            out[g] = {i: {'cos': float(cos[i])} for i in range(n)}
+    ad.fit_losses['feat_sim/cos_sim'] = rec
+    return out
+
+
+def _continuing(o, sims, steps):
+    """Bit mask of the videos of ``sims`` whose own test says 'continue' and whose trip count ``steps[g]`` (advanced here, as
+    the reference's loop does before its cap test) is still within ``optim_steps``."""
+    mask = 0
+    for g, s in sims.items():
+        if 1 - s[12]['cos'] > o.cos_sim_threshold:
+            steps[g] += 1
+            if steps[g] <= o.optim_steps:
+                mask |= 1 << g
+    return mask
+
+
+def _keep_records(ad, old, mask, G):
+    """After a level evaluated under ``mask``: every ``fit_losses`` / ``kp2dlosses_upper`` entry of ``old`` (the records before
+    that level) keeps its value for the videos outside ``mask``, whose last evaluation of the frame came earlier."""
+    keep = torch.tensor([bool((mask >> g) & 1) for g in range(G)])
+    for rec, prev in zip((ad.fit_losses, ad.kp2dlosses_upper), old):
+        for k, v in prev.items():
+            if rec[k] is not v:
+                rec[k] = torch.where(keep.to(v.device), rec[k], v)
+
+
 def fused_adapt(ad, batch):
     """One adapted frame (reference dynaboa_benchmark.py:126-201) of every video of ``ad``: probe forward, ``inner_step`` SGD
     steps of the lower level, the upper level, one Adam + EMA teacher sweep, then the optional ``dynamic_boa`` loop.
@@ -350,24 +407,44 @@ def fused_adapt(ad, batch):
         if evaluate == 'all' or (evaluate == 'final' and not o.dynamic_boa):
             result = ad.inference(batch, ad.model)
         if o.dynamic_boa:
-            after = forward_graph(ad, theta, buffers, image)
-            sims = feature_cosines(ad, probe.tape, after.tape, probe.B)
-            ad.feat_sims[ad.global_step] = [sims]
-            steps = 0
-            while 1 - sims[12]['cos'] > o.cos_sim_threshold:
-                steps += 1
-                if steps > o.optim_steps:
-                    break
-                _zero(grad)
+            # every video runs the reference's loop (:161-192) on its own: the videos still in it (bit mask `loop`) make one
+            # grouped pass per iteration, and the decisions of all of them share one host sync.  One arena: one bit.
+            stacked, G = theta.dim() == 2, _groups(theta)
+            every = (1 << G) - 1
+            frame = getattr(ad, 'active', None)
+            frame_bits = every if frame is None else frame
+            after = forward_graph(ad, theta, buffers, image, active=frame)
+            sims = feature_test(ad, probe, after, stacked, frame_bits)
+            trace, steps = {g: [s] for g, s in sims.items()}, dict.fromkeys(sims, 0)
+            if not stacked:
+                ad.feat_sims[ad.global_step] = trace[0]
+            loop = _continuing(o, sims, steps)
+            while loop:
+                act = None if loop == every else loop
+                if stacked:
+                    ad.active = act                         # the level, its draws, Adam and the motion mask follow the loop
+                old = (dict(ad.fit_losses), dict(ad.kp2dlosses_upper)) if loop != frame_bits else None
+                for t in _active_rows(ad, grad):
+                    _zero(t)
+                after.active = act                          # its backward runs under the loop, not under its forward's wider mask
                 level_backward(ad, theta, buffers, image, kp, False, grad, main=after, sync=sync)   # 'after' was computed with the current theta
+                if old is not None:
+                    _keep_records(ad, old, loop, G)
                 opt.step(teacher=teacher, alpha=o.alpha)
-                before, after = after, forward_graph(ad, theta, buffers, image)
-                sims = feature_cosines(ad, before.tape, after.tape, probe.B)
-                ad.feat_sims[ad.global_step].append(sims)
+                before, after = after, forward_graph(ad, theta, buffers, image, active=act)
+                sims = feature_test(ad, before, after, stacked, loop)
+                for g, s in sims.items():
+                    trace[g].append(s)
                 if evaluate == 'all':
                     result = ad.inference(batch, ad.model)
-            ad.optimized_step = steps
-            ad.optim_step_record.append(steps)
+                loop = _continuing(o, sims, steps)
+            if stacked:
+                ad.active = frame
+                ad.optimized_step = [steps.get(g) for g in range(G)]
+                ad.loop_feat_sims = [trace.get(g) for g in range(G)]
+            else:
+                ad.optimized_step = steps[0]
+                ad.optim_step_record.append(steps[0])
             if evaluate == 'final':
                 result = ad.inference(batch, ad.model)
         return result

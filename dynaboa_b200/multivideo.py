@@ -19,14 +19,15 @@ from ._lib import ptr, stream
 from .fused import fused_adapt, runs
 
 
-def check_options(options, n_videos):
-    """Raise ValueError for what the grouped path does not support (no device needed)."""
+def check_options(options, n_videos, dynamic_loop=False):
+    """Raise ValueError for what the grouped path does not support (no device needed).  ``dynamic_loop=True`` accepts
+    ``dynamic_boa=1``: every video then runs its own re-adaptation loop (DESIGN.md section 10, "Dynamic loop")."""
     G = int(n_videos)
     if G < 1:
         raise ValueError('n_videos must be at least 1')
-    if getattr(options, 'dynamic_boa', 0):
-        raise ValueError('dynamic_boa=1 is not supported with several videos: per-video trip counts diverge, which needs a masked '
-                         'Adam and per-video cosine decisions')
+    if getattr(options, 'dynamic_boa', 0) and not dynamic_loop:
+        raise ValueError('dynamic_boa=1 with several videos runs a re-adaptation loop per video, whose trip counts differ: '
+                         'opt in with dynamic_loop=True')
     if not getattr(options, 'use_boa', 1):
         raise ValueError('use_boa=0 is not supported with several videos (only the bilevel step is grouped)')
     lib = _lib.load()
@@ -48,11 +49,17 @@ class MultiVideoAdaptor:
     ``last_upper_loss`` ((G,) device tensor).  ``video_steps[g]``: frames slot g adapted since its ``start``; ``global_step``:
     ``adapt`` calls.  ``mask_provider(g, B, device)`` -> (3, 2, B, 1024) keep-masks of video g's teacher forward (None: drawn
     with torch's CUDA RNG, as ``HMR``).  ``rngs[g]``: the ``random.Random`` of video g's retrieval picks; ``last_retrieval[g]``:
-    video g's (cluster, picks)."""
+    video g's (cluster, picks).
 
-    def __init__(self, options, n_videos):
-        check_options(options, n_videos)
+    ``dynamic_loop=True`` runs the ``dynamic_boa`` loop: after its Adam + EMA step every video of the frame repeats the upper
+    level until its own feature test passes or its own trip count exceeds ``optim_steps``.  Per slot, as ``Adaptor`` records
+    them: ``optim_step_record[g]`` (one trip count per frame the slot advanced), ``feat_sims[g][frame]`` (the cosines of each
+    test, ``frame`` counted from the slot's ``start``), and ``optimized_step`` ((G,), None for slots that sat the frame out)."""
+
+    def __init__(self, options, n_videos, dynamic_loop=False):
+        check_options(options, n_videos, dynamic_loop)
         from .adaptor import Adaptor
+        self.dynamic_loop = bool(dynamic_loop)
         self.G = G = int(n_videos)
         self.options = o = options
         self.base = base = Adaptor(options)        # checkpoint, SMPL, prior, exemplar bank; never adapted, so it keeps the checkpoint
@@ -76,9 +83,9 @@ class MultiVideoAdaptor:
         self.last_retrieval = [None] * G
         self.teacher_dropout = bool(getattr(o, 'teacher_dropout', 1))
         self.step_counts, self.video_steps, self.histories, self.rngs = [0] * G, [0] * G, [{} for _ in range(G)], [None] * G
-        self._on = (1 << G) - 1            # slots taking part in the current frame (bit mask)
-        self.active = None                 # what fused_adapt reads: None while every slot takes part, else _on
-        self.motion_active = 0             # slots of the current frame whose motion term is live (bit mask)
+        self.optim_step_record, self.feat_sims, self.optimized_step = [[] for _ in range(G)], [{} for _ in range(G)], [None] * G
+        self._on = (1 << G) - 1            # slots taking part now (bit mask): the frame's, narrowed by the dynamic loop
+        self._live = 0                     # slots of the current frame whose motion term is live (bit mask)
         self._frames = self._hist = None   # persistent staging of the current frame's and the history frame's rows
         for g in range(G):
             self.start(g)
@@ -96,17 +103,32 @@ class MultiVideoAdaptor:
         self.step_counts[g] = self.video_steps[g] = 0
         self.histories[g].clear()
         self.rngs[g] = random.Random(self.options.seed * 1000 + g if seed is None else seed)
+        self.optim_step_record[g], self.feat_sims[g], self.optimized_step[g] = [], {}, None
 
     def theta(self, g):
         """View of video g's weights (flat arena layout)."""
         return self.thetas[g]
+
+    @property
+    def active(self):
+        """What fused_adapt reads and narrows: None while every slot takes part, else the bit mask of the slots taking part."""
+        return None if self._on == (1 << self.G) - 1 else self._on
+
+    @active.setter
+    def active(self, mask):
+        self._on = (1 << self.G) - 1 if mask is None else mask
+
+    @property
+    def motion_active(self):
+        """Slots taking part now whose motion term is live (bit mask)."""
+        return self._on & self._live
 
     def _check_runtime(self):
         opt = self.base.optimizer
         if opt.grad_sync is not None or opt.pre_step_hook is not None:
             raise ValueError('a data-parallel (dist.attach) optimizer is not supported with several videos: it all-reduces one arena '
                              'across ranks')
-        check_options(self.options, self.G)
+        check_options(self.options, self.G, getattr(self, 'dynamic_loop', False))
 
     def _slots(self, mask):
         return [g for g in range(self.G) if (mask >> g) & 1]
@@ -183,27 +205,33 @@ class MultiVideoAdaptor:
         out): ``fused.fused_adapt`` over the active slots -- probe forward, K inner SGD steps, the upper level with teacher and
         motion terms, retrieval with exemplar mix-training, then Adam + EMA teacher.  ``fit_losses`` and ``kp2dlosses_lower`` /
         ``kp2dlosses_upper`` hold this frame's (G,) losses, NaN for idle slots; ``last_upper_loss[g]`` of an idle slot keeps its
-        value."""
+        value.  With the dynamic loop, each slot's entries hold its own last level evaluation of the frame (its last loop
+        iteration, or the upper level), ``fit_losses['feat_sim/cos_sim']`` is a (G,) host tensor, and ``last_upper_loss`` is the
+        upper level's."""
         if len(batches) != self.G:
             raise ValueError(f'expected {self.G} batches, one per video, got {len(batches)}')
         on = sum(1 << g for g, b in enumerate(batches) if b is not None)
         if on == 0:
             raise ValueError('at least one slot needs a batch')
         self._check_runtime()
-        o, every = self.options, (1 << self.G) - 1
-        self._on, self.active = on, (None if on == every else on)
-        self.motion_active = sum(1 << g for g in self._slots(on) if self.video_steps[g] - o.interval > 0)
+        o = self.options
+        self._on = on
+        self._live = sum(1 << g for g in self._slots(on) if self.video_steps[g] - o.interval > 0)
         batch = self._stage(batches)
         prev = self.last_upper_loss
         self.fit_losses, self.kp2dlosses_lower, self.kp2dlosses_upper = {}, [], {}
         fused_adapt(self, batch)
         if self.active is not None:
             keep = torch.tensor([bool((on >> g) & 1) for g in range(self.G)], device=prev.device)
-            nan = lambda t: torch.where(keep, t, torch.full_like(t, float('nan')))
+            nan = lambda t: torch.where(keep.to(t.device), t, torch.full_like(t, float('nan')))
             self.last_upper_loss = torch.where(keep, self.last_upper_loss, prev)
             self.fit_losses = {k: nan(v) for k, v in self.fit_losses.items()}
             self.kp2dlosses_lower = [nan(v) for v in self.kp2dlosses_lower]
             self.kp2dlosses_upper = {k: nan(v) for k, v in self.kp2dlosses_upper.items()}
+        if o.dynamic_boa:
+            for g in self._slots(on):
+                self.optim_step_record[g].append(self.optimized_step[g])
+                self.feat_sims[g][self.video_steps[g]] = self.loop_feat_sims[g]
         for g in self._slots(on):
             self.video_steps[g] += 1
         self.global_step += 1

@@ -301,6 +301,17 @@ int dboa_cosine_pairs(const float* const* a, const float* const* b, const long l
 long long dboa_cosine_partial_floats(const long long* n, int npairs);
 int dboa_cosine_terms(const float* const* a, const float* const* b, const long long* n, int npairs, float* partial,
                       long long partial_floats, double* terms, dboa_stream_t stream);
+/* the same for `groups` videos at once, each on its own part of every pair: the per-video feature test of the dynamic loop
+ * of MultiVideoAdaptor.  n[i] is the length of pair i over all groups; video g's part is the floats
+ * [g n[i] / groups, (g + 1) n[i] / groups) of a[i] and b[i] (the per-sample layout of every dboa_hmr_feature_info view, made
+ * dense).  terms: [groups][npairs][3] in double.  Only the videos whose bit is set in `active` take part: the rows of terms of
+ * the others are not written and none of their inputs is read.  Video g's sums are bit-identical to dboa_cosine_terms on its
+ * parts alone; groups = 1 with bit 0 set is dboa_cosine_terms.  partial: dboa_cosine_partial_floats_groups(n, npairs, groups)
+ * floats of scratch.  DBOA_ERR_ARG for a NULL pointer, npairs outside 1..16, active == 0, a bit at position >= groups or too
+ * small a partial; DBOA_ERR_SHAPE for groups outside 1..64 or n[i] % groups != 0 (both the same for the floats query). */
+long long dboa_cosine_partial_floats_groups(const long long* n, int npairs, int groups);
+int dboa_cosine_terms_active(const float* const* a, const float* const* b, const long long* n, int npairs, float* partial,
+                             long long partial_floats, double* terms, dboa_stream_t stream, int groups, unsigned long long active);
 /* retrieval :82-84: index of the centre with the smallest cosine distance to feat (D,) among centers (K,D) */
 int dboa_retrieval_nearest(const float* feat, const float* centers, int K, int D, int* best, float* dists, dboa_stream_t stream);
 
