@@ -77,6 +77,52 @@ def test_smpl_golden_and_properties(golden):
     assert torch.equal(out.joints[:, 8], out.joints[:, 39 - 25 + 25]) or True       # (joint map sanity is checked in constants)
 
 
+def test_loss_head_ref_agrees_with_adaptor_ref():
+    """oracle/loss_head_ref.py (the per-video restatement the GPU loss-head tests evaluate in fp64) gives the adaptor
+    oracle's frame, teacher, labelled and motion losses for one video in fp32, and each video's own values when grouped."""
+    import torch.nn.functional as F
+    from dynaboa_b200 import config
+    from oracle import loss_head_ref as L
+    g = torch.Generator().manual_seed(5)
+    B = 3
+    p2d, j3d, beta = torch.randn(B, 49, 2, generator=g) * 0.3, torch.randn(B, 49, 3, generator=g) * 0.3, torch.randn(B, 10, generator=g)
+    R = G.batch_rodrigues(torch.randn(B * 24, 3, generator=g) * 0.6).view(B, 24, 3, 3)
+    kp = torch.cat([torch.randn(B, 49, 2, generator=g) * 0.3, (torch.rand(B, 49, 1, generator=g) > 0.2).float()], -1)
+    kh = torch.cat([torch.randn(B, 49, 2, generator=g) * 0.3, (torch.rand(B, 49, 1, generator=g) > 0.2).float()], -1)
+    t_p2d, t_j3d, t_beta = torch.randn(B, 49, 2, generator=g) * 0.3, torch.randn(B, 49, 3, generator=g) * 0.3, torch.randn(B, 10, generator=g)
+    t_R = G.batch_rodrigues(torch.randn(B * 24, 3, generator=g) * 0.4).view(B, 24, 3, 3)
+    gt_s3d = torch.cat([torch.randn(B, 24, 3, generator=g) * 0.3, torch.ones(B, 24, 1)], -1)
+    consts = prior_ref.gmm_constants(dict(np.load(config.GMM_PRIOR)))
+    ora = adaptor_ref.OracleAdaptor.__new__(adaptor_ref.OracleAdaptor)
+    ora.o, ora.gmm, ora.fit_losses = adaptor_ref.default_options(), consts, {}
+    prior = L.pose_prior(R, (consts['means'], consts['precisions'], -torch.log(consts['nll_weights']).reshape(-1)))
+    o = ora.o
+    w = [o.s2dloss_weight, o.shape_prior_weight, o.pose_prior_weight, 5, 5, 0.001, 1, 5]
+    t = L.head_terms(1, p2d, j3d, R, beta, w, kp=kp, prior=prior, t_p2d=t_p2d, t_j3d=t_j3d, t_beta=t_beta, t_R=t_R, gt_s3d=gt_s3d)[0]
+    loss, s2d = ora.frame_losses(p2d, kp, beta, R, 'll')
+    conf = kp[:, 25:, -1:]
+    expect = [s2d, ora.shape_prior(beta), ora.pose_prior(R), F.mse_loss(p2d, t_p2d), F.mse_loss(j3d, t_j3d), F.mse_loss(beta, t_beta),
+              F.mse_loss(R, t_R), adaptor_ref.OracleAdaptor.s3d_loss(j3d[:, 25:], gt_s3d[:, :, :3], conf)]
+    for i, e in enumerate(expect):
+        assert abs(float(t[i]) - float(e)) <= 1e-6 * abs(float(e)), i
+    assert abs(float(t[:3] @ torch.tensor(w[:3])) - float(loss)) <= 1e-6 * float(loss)
+    motion = ((((p2d[:, 25:] - t_p2d[:, 25:]) - (kp[:, 25:, :2] - kh[:, 25:, :2])) ** 2) * ((kp[:, 25:, -1:] + kh[:, 25:, -1:]) == 2)).mean()
+    assert abs(float(L.motion_terms(1, p2d, t_p2d, kp, kh)[0]) - float(motion)) <= 1e-6 * float(motion)
+    # grouped: video g's terms are those of its rows alone
+    tg = L.head_terms(B, p2d, j3d, R, beta, w, kp=kp, prior=prior, t_p2d=t_p2d, t_j3d=t_j3d, t_beta=t_beta, t_R=t_R, gt_s3d=gt_s3d,
+                      kp_range=(0, 25))
+    mg = L.motion_terms(B, p2d, t_p2d, kp, kh, 0, 25)
+    for v in range(B):
+        s = slice(v, v + 1)
+        one = L.head_terms(1, p2d[s], j3d[s], R[s], beta[s], w, kp=kp[s], prior=prior[s], t_p2d=t_p2d[s], t_j3d=t_j3d[s], t_beta=t_beta[s],
+                           t_R=t_R[s], gt_s3d=gt_s3d[s], kp_range=(0, 25))[0]
+        assert torch.equal(tg[v], one) and torch.equal(mg[v], L.motion_terms(1, p2d[s], t_p2d[s], kp[s], kh[s], 0, 25)[0]), v
+    # the four branches of the axis-angle conversion, decided as rotmath.cuh decides them
+    Rb = torch.stack([torch.diag(torch.tensor(d)) for d in ((1., -1., -1.), (-1., 1., -1.), (-1., -1., 1.), (1., 1., 1.))])
+    assert L.r2aa_branch(Rb).tolist() == [0, 1, 2, 3]
+    assert L.R2AA_EPS < 1e-6 and np.float32(L.R2AA_EPS) == np.float32(1e-6)
+
+
 def test_l2l_functional_and_module_forms_agree():
     torch.manual_seed(0)
     net = torch.nn.Sequential(torch.nn.Linear(6, 5), torch.nn.Tanh(), torch.nn.Linear(5, 2))
