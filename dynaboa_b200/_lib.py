@@ -115,6 +115,7 @@ SIGNATURES = {
     'dboa_keypoint_transform': (I, [P, I, C.c_double, C.c_double, C.c_double, C.c_double, I, P, P]),
     'dboa_eval_scratch_floats': (L, [I, I]),
     'dboa_eval_metrics': (I, [P, P, P, P, I, I, P, I, P, P, I, P]),
+    'dboa_eval_metrics_active': (I, [P, P, P, P, I, I, P, I, P, P, I, I, C.c_ulonglong, P]),
     'dboa_render_scratch_bytes': (L, [I, I, I, I, I]),
     'dboa_render_overlay': (I, [P, P, P, P, I, I, C.POINTER(F), C.POINTER(F), C.POINTER(F), P, I, I, I, P, L, P, P, P]),
 }

@@ -19,6 +19,35 @@ from . import _lib, constants
 from .base_adaptor import BaseAdaptor
 
 
+RESULT_FILES = ('lowerlevel_kp2dloss.pt', 'upperlevel_kp2dloss.pt', 'res.pt', 'lower_res.pt', 'steps_statistic_res.pt', 'feat_sims.pt',
+                'optim_step_record.pt', 'res.txt')
+
+
+def write_records(exppath, step, rec):
+    """The eight result files of the reference driver, same names, same joblib pickles, same keys
+    (dynaboa_benchmark.py:111-123), into the directory ``exppath``.  ``step``: the last frame's index, as ``res.txt`` reports
+    it.  ``rec``: mpjpe, pampjpe, pve (one entry per frame), mpjpe_all_lower, pampjpe_all_lower (one list per inner step),
+    mpjpe_statistics, pampjpe_statistics, feat_sims, optim_step_record, kp2dlosses_lower (a list) and kp2dlosses_upper (a dict
+    by frame)."""
+    import joblib
+    p = lambda name: osp.join(exppath, name)
+    mpjpe_all, pampjpe_all, pve_all = rec['mpjpe'], rec['pampjpe'], rec['pve']
+    lower_m, lower_p = rec['mpjpe_all_lower'], rec['pampjpe_all_lower']
+    joblib.dump({'kp2dloss': [float(x) for x in rec['kp2dlosses_lower']]}, p('lowerlevel_kp2dloss.pt'))
+    joblib.dump({'kp2dloss': {k: float(v) for k, v in rec['kp2dlosses_upper'].items()}}, p('upperlevel_kp2dloss.pt'))
+    joblib.dump({'mpjpe': mpjpe_all, 'pampjpe': pampjpe_all, 'pve': pve_all}, p('res.pt'))
+    joblib.dump({'mpjpe': lower_m, 'pampjpe': lower_p}, p('lower_res.pt'))
+    joblib.dump({'mpjpe': rec['mpjpe_statistics'], 'pampjpe': rec['pampjpe_statistics']}, p('steps_statistic_res.pt'))
+    joblib.dump({'feat': rec['feat_sims']}, p('feat_sims.pt'))
+    joblib.dump({'step': rec['optim_step_record']}, p('optim_step_record.pt'))
+    with open(p('res.txt'), 'w') as f:
+        f.write(f'Step:{step}: MPJPE:{np.mean(mpjpe_all)}, PAMPJPE:{np.mean(pampjpe_all)}, PVE:{np.mean(pve_all)}\n')
+        for i in range(len(lower_m)):
+            lo_m = np.mean(lower_m[i]) if len(lower_m[i]) else float('nan')
+            lo_p = np.mean(lower_p[i]) if len(lower_p[i]) else float('nan')
+            f.write(f'Lower-level  Step:{i} MPJPE:{lo_m}, PAMPJPE:{lo_p}\n')
+
+
 class Adaptor(BaseAdaptor):
     def __init__(self, options):
         super().__init__(options)
@@ -52,23 +81,11 @@ class Adaptor(BaseAdaptor):
         return summary
 
     def save_records(self, mpjpe_all, pampjpe_all, pve_all):
-        """The eight result files of the reference driver, same names, same joblib pickles, same keys
-        (dynaboa_benchmark.py:111-123)."""
-        import joblib
-        p = lambda name: osp.join(self.exppath, name)
-        joblib.dump({'kp2dloss': [float(x) for x in self.kp2dlosses_lower]}, p('lowerlevel_kp2dloss.pt'))
-        joblib.dump({'kp2dloss': {k: float(v) for k, v in self.kp2dlosses_upper.items()}}, p('upperlevel_kp2dloss.pt'))
-        joblib.dump({'mpjpe': mpjpe_all, 'pampjpe': pampjpe_all, 'pve': pve_all}, p('res.pt'))
-        joblib.dump({'mpjpe': self.mpjpe_all_lower, 'pampjpe': self.pampjpe_all_lower}, p('lower_res.pt'))
-        joblib.dump({'mpjpe': self.mpjpe_statistics, 'pampjpe': self.pampjpe_statistics}, p('steps_statistic_res.pt'))
-        joblib.dump({'feat': self.feat_sims}, p('feat_sims.pt'))
-        joblib.dump({'step': self.optim_step_record}, p('optim_step_record.pt'))
-        with open(p('res.txt'), 'w') as f:
-            f.write(f'Step:{self.global_step}: MPJPE:{np.mean(mpjpe_all)}, PAMPJPE:{np.mean(pampjpe_all)}, PVE:{np.mean(pve_all)}\n')
-            for i in range(self.options.inner_step):
-                lo_m = np.mean(self.mpjpe_all_lower[i]) if len(self.mpjpe_all_lower[i]) else float('nan')
-                lo_p = np.mean(self.pampjpe_all_lower[i]) if len(self.pampjpe_all_lower[i]) else float('nan')
-                f.write(f'Lower-level  Step:{i} MPJPE:{lo_m}, PAMPJPE:{lo_p}\n')
+        """The eight result files of the reference driver (``write_records``)."""
+        write_records(self.exppath, self.global_step, dict(
+            mpjpe=mpjpe_all, pampjpe=pampjpe_all, pve=pve_all, mpjpe_all_lower=self.mpjpe_all_lower, pampjpe_all_lower=self.pampjpe_all_lower,
+            mpjpe_statistics=self.mpjpe_statistics, pampjpe_statistics=self.pampjpe_statistics, feat_sims=self.feat_sims,
+            optim_step_record=self.optim_step_record, kp2dlosses_lower=self.kp2dlosses_lower, kp2dlosses_upper=self.kp2dlosses_upper))
 
     def _outer_step(self, loss):
         self.optimizer.zero_grad()
@@ -177,8 +194,10 @@ class Adaptor(BaseAdaptor):
             return mpjpe * 1000, pampjpe * 1000, pve * 1000, out[3]
         return mpjpe * 1000, pampjpe * 1000, pve * 1000
 
-    def eval_metrics(self, pred_vertices, gt_vertices, gt_vertices_neutral):
-        """(B,3) device tensor: MPJPE, PA-MPJPE, PVE (metres) of each sample -- ``dboa_eval_metrics``."""
+    def eval_metrics(self, pred_vertices, gt_vertices, gt_vertices_neutral, groups=1, active=None):
+        """(B,3) device tensor: MPJPE, PA-MPJPE, PVE (metres) of each sample -- ``dboa_eval_metrics``.  ``groups`` videos of
+        B / groups rows each, of which only those whose bit is set in ``active`` (an int; None: all) are evaluated
+        (``dboa_eval_metrics_active``): the rows of the others are left unwritten."""
         B, dev = pred_vertices.shape[0], pred_vertices.device
         if getattr(self, '_eval_consts', None) is None or self._eval_consts[0].device != dev:
             self._eval_consts = (self.J_regressor.to(dev).contiguous().float(),
@@ -188,8 +207,12 @@ class Adaptor(BaseAdaptor):
         scratch = torch.empty(_lib.load().dboa_eval_scratch_floats(B, J.shape[0]), dtype=torch.float32, device=dev)
         out = torch.empty(B, 3, dtype=torch.float32, device=dev)
         keep = [t.contiguous().float() for t in (pred_vertices, gt_vertices, gt_vertices_neutral)]
-        _lib.call('dboa_eval_metrics', _lib.ptr(keep[0]), _lib.ptr(keep[1]), _lib.ptr(keep[2]), _lib.ptr(J), int(J.shape[0]),
-                  int(pred_vertices.shape[1]), _lib.ptr(jmap), int(jmap.numel()), _lib.ptr(scratch), _lib.ptr(out), B, _lib.stream())
+        args = (_lib.ptr(keep[0]), _lib.ptr(keep[1]), _lib.ptr(keep[2]), _lib.ptr(J), int(J.shape[0]), int(pred_vertices.shape[1]), _lib.ptr(jmap),
+                int(jmap.numel()), _lib.ptr(scratch), _lib.ptr(out), B)
+        if groups == 1 and active is None:
+            _lib.call('dboa_eval_metrics', *args, _lib.stream())
+        else:
+            _lib.call('dboa_eval_metrics_active', *args, int(groups), (1 << int(groups)) - 1 if active is None else int(active), _lib.stream())
         return out
 
     def adapt(self, batch):

@@ -400,8 +400,15 @@ int dboa_keypoint_transform(const float* kp, int n, double t00, double t02, doub
 long long dboa_eval_scratch_floats(int B, int NJ) { return (long long)eval_scratch_floats(B, NJ); }
 int dboa_eval_metrics(const float* pred_verts, const float* gt_verts_joints, const float* gt_verts_pve, const float* J_regressor, int NJ,
                       int NV, const int* joint_map, int n_map, float* scratch, float* out, int B, dboa_stream_t stream) {
+    return dboa_eval_metrics_active(pred_verts, gt_verts_joints, gt_verts_pve, J_regressor, NJ, NV, joint_map, n_map, scratch, out, B, 1, 1ULL,
+                                    stream);
+}
+int dboa_eval_metrics_active(const float* pred_verts, const float* gt_verts_joints, const float* gt_verts_pve, const float* J_regressor, int NJ,
+                             int NV, const int* joint_map, int n_map, float* scratch, float* out, int B, int groups, unsigned long long active,
+                             dboa_stream_t stream) {
     if (!pred_verts || !gt_verts_joints || !gt_verts_pve || !J_regressor || !joint_map || !scratch || !out) return DBOA_ERR_ARG;
-    return eval_metrics(pred_verts, gt_verts_joints, gt_verts_pve, J_regressor, NJ, NV, joint_map, n_map, scratch, out, B, ST(stream));
+    return eval_metrics(pred_verts, gt_verts_joints, gt_verts_pve, J_regressor, NJ, NV, joint_map, n_map, scratch, out, B, groups, active,
+                        ST(stream));
 }
 
 long long dboa_render_scratch_bytes(int W, int H, int NV, int NF, int samples) { return render_scratch_bytes(W, H, NV, NF, samples); }

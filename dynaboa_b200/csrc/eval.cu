@@ -24,11 +24,13 @@ constexpr int EV_MAXJ = 32;
 
 __global__ void __launch_bounds__(EV_NT) eval_joints_kernel(const float* __restrict__ pred, const float* __restrict__ gt_j,
                                                             const float* __restrict__ gt_v, const float* __restrict__ Jreg, int NV,
-                                                            float* __restrict__ scratch /* [B][2][NJ][3] joints, then [B][NJ] pve partials */) {
+                                                            float* __restrict__ scratch /* [B][2][NJ][3] joints, then [B][NJ] pve partials */,
+                                                            int per_video, unsigned long long active) {
     __shared__ float red[32];
+    const int j = blockIdx.x, b = blockIdx.y, z = blockIdx.z, NJ = gridDim.x, B = gridDim.y;
+    if (!((active >> (b / per_video)) & 1ULL)) return;                // idle video: uniform over the CTA, before the wait
     pdl_wait();
     pdl_trigger();
-    const int j = blockIdx.x, b = blockIdx.y, z = blockIdx.z, NJ = gridDim.x, B = gridDim.y;
     if (z < 2) {
         const float* v = (z == 0 ? pred : gt_j) + (size_t)b * NV * 3;
         const float* w = Jreg + (size_t)j * NV;
@@ -84,11 +86,11 @@ __device__ void svd3_jacobi(double a[3][3], double v[3][3]) {
 }
 
 __global__ void eval_metrics_kernel(const float* __restrict__ scratch, const int* __restrict__ joint_map, int n_map, int NJ, int NV, int B,
-                                    float* __restrict__ out /* [B][3]: mpjpe, pa-mpjpe, pve */) {
+                                    float* __restrict__ out /* [B][3]: mpjpe, pa-mpjpe, pve */, int per_video, unsigned long long active) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B || !((active >> (b / per_video)) & 1ULL)) return;       // idle rows exit before the wait
     pdl_wait();
     pdl_trigger();
-    const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= B) return;
     const float* jp = scratch + ((size_t)b * 2 + 0) * NJ * 3;
     const float* jg = scratch + ((size_t)b * 2 + 1) * NJ * 3;
     double S1[EV_MAXJ][3], S2[EV_MAXJ][3];
@@ -171,13 +173,18 @@ __global__ void eval_metrics_kernel(const float* __restrict__ scratch, const int
 
 size_t eval_scratch_floats(int B, int NJ) { return (size_t)B * 2 * NJ * 3 + (size_t)B * NJ; }
 
+// `groups` videos of B / groups rows each; only the rows of the videos whose bit is set in `active` are read, computed and
+// written.  A row's arithmetic does not depend on the other rows, so an active row is bit-identical to a call on its rows alone.
 int eval_metrics(const float* pred_verts, const float* gt_verts_joints, const float* gt_verts_pve, const float* Jreg, int NJ, int NV,
-                 const int* joint_map, int n_map, float* scratch, float* out, int B, cudaStream_t st) {
+                 const int* joint_map, int n_map, float* scratch, float* out, int B, int groups, unsigned long long active, cudaStream_t st) {
     if (NJ < 1 || NJ > EV_MAXJ || n_map < 1 || n_map > EV_MAXJ || B < 1) return DBOA_ERR_SHAPE;
+    if (groups < 1 || groups > 64 || B % groups != 0) return DBOA_ERR_SHAPE;
+    if (active == 0 || (groups < 64 && (active >> groups) != 0)) return DBOA_ERR_ARG;
+    const int per_video = B / groups;
     DBOA_TRY(launch_ex(eval_joints_kernel, dim3(NJ, B, 3), dim3(EV_NT), 0, st, dim3(1, 1, 1), true, pred_verts, gt_verts_joints, gt_verts_pve,
-                       Jreg, NV, scratch));
+                       Jreg, NV, scratch, per_video, active));
     return launch_ex(eval_metrics_kernel, dim3(ceil_div(B, 64)), dim3(64), 0, st, dim3(1, 1, 1), true, (const float*)scratch, joint_map, n_map,
-                     NJ, NV, B, out);
+                     NJ, NV, B, out, per_video, active);
 }
 
 }  // namespace dboa

@@ -135,7 +135,7 @@ int keypoint_transform(const float* kp, int n, double t00, double t02, double t1
 // ---- eval.cu (evaluation metrics on the device)
 size_t eval_scratch_floats(int B, int NJ);
 int eval_metrics(const float* pred_verts, const float* gt_verts_joints, const float* gt_verts_pve, const float* Jreg, int NJ, int NV,
-                 const int* joint_map, int n_map, float* scratch, float* out, int B, cudaStream_t st);
+                 const int* joint_map, int n_map, float* scratch, float* out, int B, int groups, unsigned long long active, cudaStream_t st);
 
 // render.cu: mesh overlay (include/dynaboa_b200.h, "mesh overlay")
 long long render_scratch_bytes(int W, int H, int NV, int NF, int samples);

@@ -6,17 +6,24 @@ Each video keeps the reference's semantics: its own theta, Adam moments and step
 history ring, motion warm-up, teacher dropout masks and retrieval picks.  The G weight arenas (and the teachers', the moments',
 the gradients') are one contiguous (G, P) stack; video g owns the rows [g * b, (g + 1) * b) of every per-sample batch.  The
 G slots are a pool: a slot whose batch is None sits the frame out (its CTAs return at once in every grouped call), and
-``start(g)`` puts a new video into slot g.  DESIGN.md section 10.
+``start(g)`` puts a new video into slot g; ``run(videos)`` feeds a queue of videos through the slots.  With ``fused_eval``
+'final' or 'all' every video gets the records and result files of the single-video driver.  DESIGN.md section 10.
 """
 import ctypes as C
+import os
 import random
 from types import SimpleNamespace
 
+import numpy as np
 import torch
 
 from . import _lib, hmr as hmr_mod
 from ._lib import ptr, stream
 from .fused import fused_adapt, runs
+
+EVAL_MODES = ('none', 'final', 'all')
+GT_KEYS = ('pose', 'betas', 'gender')
+PENDING_FRAMES = 256        # device records kept before adapt forms them on the host (one synchronisation)
 
 
 def check_options(options, n_videos, dynamic_loop=False):
@@ -54,7 +61,14 @@ class MultiVideoAdaptor:
     ``dynamic_loop=True`` runs the ``dynamic_boa`` loop: after its Adam + EMA step every video of the frame repeats the upper
     level until its own feature test passes or its own trip count exceeds ``optim_steps``.  Per slot, as ``Adaptor`` records
     them: ``optim_step_record[g]`` (one trip count per frame the slot advanced), ``feat_sims[g][frame]`` (the cosines of each
-    test, ``frame`` counted from the slot's ``start``), and ``optimized_step`` ((G,), None for slots that sat the frame out)."""
+    test, ``frame`` counted from the slot's ``start``), and ``optimized_step`` ((G,), None for slots that sat the frame out).
+
+    ``fused_eval`` ('none', 'final' or 'all', as ``Adaptor``'s): evaluate every advancing video against its ground truth
+    (batches then need pose, betas and gender).  Each evaluation stays on the device; ``records(g)`` forms slot g's host
+    records (``mpjpe_all[g]``, ``pampjpe_all[g]``, ``pve_all[g]``, with 'all' also ``mpjpe_all_lower[g]`` /
+    ``pampjpe_all_lower[g]`` and ``mpjpe_statistics[g]`` / ``pampjpe_statistics[g]``, and the run's 2D keypoint losses), and
+    ``start(g)`` forms them before it resets the slot.  ``run(videos, exppath=None, names=None)`` adapts a list of videos
+    through the slots and returns one summary per video."""
 
     def __init__(self, options, n_videos, dynamic_loop=False):
         check_options(options, n_videos, dynamic_loop)
@@ -87,14 +101,23 @@ class MultiVideoAdaptor:
         self._on = (1 << G) - 1            # slots taking part now (bit mask): the frame's, narrowed by the dynamic loop
         self._live = 0                     # slots of the current frame whose motion term is live (bit mask)
         self._frames = self._hist = None   # persistent staging of the current frame's and the history frame's rows
+        self._pending = []                 # device records of the frames adapted since the records were last formed
+        self._gt = None                    # the current frame's ground-truth meshes (gender-selected, neutral)
+        self.slot_video = [None] * G       # run(): index of the video slot g holds
+        self.mpjpe_all, self.pampjpe_all, self.pve_all = [[] for _ in range(G)], [[] for _ in range(G)], [[] for _ in range(G)]
+        self.mpjpe_all_lower, self.pampjpe_all_lower = [None] * G, [None] * G
+        self.mpjpe_statistics, self.pampjpe_statistics = [{} for _ in range(G)], [{} for _ in range(G)]
+        self.kp2dloss_lower_all, self.kp2dloss_upper_all = [[] for _ in range(G)], [{} for _ in range(G)]
         for g in range(G):
             self.start(g)
 
     def start(self, g, seed=None):
         """Put a new video into slot g: theta and teacher from the checkpoint, zero Adam moments, step and frame counts, an empty
-        history, and ``rngs[g] = random.Random(seed)`` (default ``options.seed * 1000 + g``)."""
+        history, empty records, and ``rngs[g] = random.Random(seed)`` (default ``options.seed * 1000 + g``).  The records of
+        the frames adapted so far are formed on the host first (one synchronisation, if any are pending)."""
         if not isinstance(g, int) or not 0 <= g < self.G:
             raise ValueError(f'slot {g!r} is not one of the {self.G} slots')
+        self._form_records()
         self.thetas[g].copy_(self.base.model.module.arena.detach())
         if self.teachers is not None:
             self.teachers[g].copy_(self.base.teacher.arena.detach())
@@ -104,6 +127,11 @@ class MultiVideoAdaptor:
         self.histories[g].clear()
         self.rngs[g] = random.Random(self.options.seed * 1000 + g if seed is None else seed)
         self.optim_step_record[g], self.feat_sims[g], self.optimized_step[g] = [], {}, None
+        n = self.options.inner_step
+        self.mpjpe_all[g], self.pampjpe_all[g], self.pve_all[g] = [], [], []
+        self.mpjpe_all_lower[g], self.pampjpe_all_lower[g] = [[] for _ in range(n)], [[] for _ in range(n)]
+        self.mpjpe_statistics[g], self.pampjpe_statistics[g] = {}, {}
+        self.kp2dloss_lower_all[g], self.kp2dloss_upper_all[g] = [], {}
 
     def theta(self, g):
         """View of video g's weights (flat arena layout)."""
@@ -184,13 +212,17 @@ class MultiVideoAdaptor:
         """Copy the active slots' frames into the persistent (G b, ...) batch; the rows of idle slots keep what they held."""
         dev = self.thetas.device
         first = next(b for b in batches if b is not None)
+        keys = ('image', 'smpl_j2d') + (GT_KEYS if self.fused_eval != 'none' else ())
         if self._frames is None:
-            self._frames = {k: torch.zeros((self.G * first[k].shape[0],) + tuple(first[k].shape[1:]), dtype=torch.float32, device=dev)
-                            for k in ('image', 'smpl_j2d')}
+            self._frames = {}
+        for k in keys:
+            if k not in self._frames:
+                self._frames[k] = torch.zeros((self.G * first[k].shape[0],) + tuple(first[k].shape[1:]), dtype=torch.float32, device=dev)
         for g, bt in enumerate(batches):
             if bt is None:
                 continue
-            for k, buf in self._frames.items():
+            for k in keys:
+                buf = self._frames[k]
                 src = bt[k].to(dev).contiguous().float()
                 rows = buf.shape[0] // self.G
                 if tuple(src.shape) != (rows,) + tuple(buf.shape[1:]):
@@ -213,6 +245,13 @@ class MultiVideoAdaptor:
         on = sum(1 << g for g, b in enumerate(batches) if b is not None)
         if on == 0:
             raise ValueError('at least one slot needs a batch')
+        if self.fused_eval not in EVAL_MODES:
+            raise ValueError(f'fused_eval must be one of {EVAL_MODES}, got {self.fused_eval!r}')
+        if self.fused_eval != 'none':
+            for g in self._slots(on):
+                missing = [k for k in GT_KEYS if k not in batches[g]]
+                if missing:
+                    raise ValueError(f'slot {g}: fused_eval={self.fused_eval!r} needs the ground truth {", ".join(missing)} in the batch')
         self._check_runtime()
         o = self.options
         self._on = on
@@ -220,7 +259,9 @@ class MultiVideoAdaptor:
         batch = self._stage(batches)
         prev = self.last_upper_loss
         self.fit_losses, self.kp2dlosses_lower, self.kp2dlosses_upper = {}, [], {}
+        self._evals, self._gt, self._lower_evals = [], None, 0
         fused_adapt(self, batch)
+        self._gt = None
         if self.active is not None:
             keep = torch.tensor([bool((on >> g) & 1) for g in range(self.G)], device=prev.device)
             nan = lambda t: torch.where(keep.to(t.device), t, torch.full_like(t, float('nan')))
@@ -232,9 +273,134 @@ class MultiVideoAdaptor:
             for g in self._slots(on):
                 self.optim_step_record[g].append(self.optimized_step[g])
                 self.feat_sims[g][self.video_steps[g]] = self.loop_feat_sims[g]
+        self._pending.append((on, {g: self.video_steps[g] for g in self._slots(on)}, self.fused_eval == 'all', self._evals,
+                              list(self.kp2dlosses_lower), self.kp2dlosses_upper.get(self.global_step)))
+        if len(self._pending) >= PENDING_FRAMES:
+            self._form_records()
         for g in self._slots(on):
             self.video_steps[g] += 1
         self.global_step += 1
+
+    def inference(self, batch, model, need_feature=False):
+        """One evaluation of the stack ``model.arena`` (theta, or the fast weights of the next inner step) on the staged frame,
+        for the slots taking part now: one grouped forward, the neutral SMPL decode and ``dboa_eval_metrics_active``.  The
+        ground-truth meshes are computed at the frame's first evaluation and reused.  The (G b, 3) result stays on the device
+        until the records are formed; returns None."""
+        lower = model.arena is not self.thetas
+        with torch.no_grad():
+            rot, shape, _, _, _ = hmr_mod.raw_forward(model.arena, self.buffers, batch['image'], groups=self.G, active=self.active)
+            pred = self.base.decode_smpl_params(rot, shape)['vts']
+            if self._gt is None:                             # as Adaptor.inference, for every staged row
+                pose, betas, gender, b = batch['pose'], batch['betas'], batch['gender'], self.base
+                gt = b.smpl_male(global_orient=pose[:, :3], body_pose=pose[:, 3:], betas=betas).vertices
+                gt_f = b.smpl_female(global_orient=pose[:, :3], body_pose=pose[:, 3:], betas=betas).vertices
+                gt = torch.where((gender == 1).view(-1, 1, 1), gt_f, gt)
+                gt_n = self.smpl_neutral(betas=betas, body_pose=pose[:, 3:], global_orient=pose[:, :3], pose2rot=True).vertices
+                self._gt = (gt, gt_n)
+            out = self.base.eval_metrics(pred, *self._gt, groups=self.G, active=self._on)
+        self._evals.append((out, self._on, self._lower_evals if lower else None))
+        if lower:
+            self._lower_evals += 1
+
+    def _form_records(self):
+        """File the device records of every frame adapted since the last call into the slots' host records: one copy to the
+        host (and so one synchronisation) for all of them."""
+        if not self._pending:
+            return
+        G, b = self.G, self._frames['image'].shape[0] // self.G
+        flat = [t.reshape(-1) for _, _, _, evals, low, up in self._pending for t in [e[0] for e in evals] + low + ([up] if up is not None else [])]
+        host = torch.cat(flat).cpu().numpy() if flat else None
+        off = 0
+
+        def take(n):
+            nonlocal off
+            off += n
+            return host[off - n:off]
+        for on, frames, steps, evals, low, up in self._pending:
+            evals = [(take(out.numel()).reshape(-1, 3), mask, step) for out, mask, step in evals]
+            low = [take(G) for _ in low]
+            up = take(G) if up is not None else None
+            for g, t in frames.items():
+                # Adaptor.inference's values: metrics[:, 0] * 1000, metrics[:, 1] * 1000, float(metrics[:, 2].mean()) * 1000
+                mine = [(np.ascontiguousarray(m[g * b:(g + 1) * b]), step) for m, mask, step in evals if (mask >> g) & 1]
+                thetas = [(m[:, 0] * 1000, m[:, 1] * 1000, float(m[:, 2].mean()) * 1000) for m, step in mine if step is None]
+                for m, step in mine:
+                    if step is not None:
+                        self.mpjpe_all_lower[g][step].append(m[:, 0] * 1000)
+                        self.pampjpe_all_lower[g][step].append(m[:, 1] * 1000)
+                if thetas:
+                    self.mpjpe_all[g].append(thetas[-1][0])
+                    self.pampjpe_all[g].append(thetas[-1][1])
+                    self.pve_all[g].append(thetas[-1][2])
+                if steps:                                    # 'all': every theta evaluation of the frame
+                    self.mpjpe_statistics[g][t] = [x[0] for x in thetas]
+                    self.pampjpe_statistics[g][t] = [x[1] for x in thetas]
+                self.kp2dloss_lower_all[g] += [float(v[g]) for v in low]
+                if up is not None:
+                    self.kp2dloss_upper_all[g][t] = float(up[g])
+        self._pending = []
+
+    def records(self, g):
+        """Slot g's records since its ``start`` as host values, under the names ``adaptor.write_records`` takes (the values of
+        ``Adaptor.excute``'s records for that video), and ``frames``."""
+        self._form_records()
+        n = self.video_steps[g]
+        return dict(frames=n, mpjpe=list(self.mpjpe_all[g]), pampjpe=list(self.pampjpe_all[g]), pve=list(self.pve_all[g]),
+                    mpjpe_all_lower=[list(x) for x in self.mpjpe_all_lower[g]], pampjpe_all_lower=[list(x) for x in self.pampjpe_all_lower[g]],
+                    mpjpe_statistics=[self.mpjpe_statistics[g].get(t, []) for t in range(n)],
+                    pampjpe_statistics=[self.pampjpe_statistics[g].get(t, []) for t in range(n)],
+                    feat_sims=dict(self.feat_sims[g]), optim_step_record=list(self.optim_step_record[g]),
+                    kp2dlosses_lower=list(self.kp2dloss_lower_all[g]), kp2dlosses_upper=dict(self.kp2dloss_upper_all[g]))
+
+    def run(self, videos, exppath=None, names=None):
+        """Adapt every video of ``videos`` (a list of iterables of batch dicts with batch size 1: a ``DataLoader`` over a
+        sequence, a ``SyntheticStream``) through the G slots.  Slots are filled in order and refilled from the queue as soon as
+        their video ends; video i starts with ``start(g, seed=options.seed * 1000 + i)``, so its seed follows the video, and
+        ``slot_video[g]`` is the index of the video slot g holds (for a ``mask_provider``).  Returns one summary per video, in
+        order: name, frames, and the mean MPJPE, PA-MPJPE and PVE of its frames (``res.txt``'s; NaN without evaluation).  With
+        ``exppath``, each video's eight result files go to ``exppath/<name>/`` when it finishes (``names``: default the
+        video's index)."""
+        from .adaptor import write_records
+        videos = list(videos)
+        names = [str(i) for i in range(len(videos))] if names is None else [str(x) for x in names]
+        if len(names) != len(videos):
+            raise ValueError(f'{len(names)} names for {len(videos)} videos')
+        queue, its, nxt, out = list(range(len(videos))), [None] * self.G, [None] * self.G, [None] * len(videos)
+        mean = lambda v: float(np.mean(v)) if len(v) else float('nan')
+
+        def fill(g):
+            self.slot_video[g] = None
+            while queue:
+                i = queue.pop(0)
+                its[g] = iter(videos[i])
+                nxt[g] = next(its[g], None)
+                if nxt[g] is None:                           # an empty video
+                    out[i] = dict(name=names[i], frames=0, mpjpe=float('nan'), pampjpe=float('nan'), pve=float('nan'))
+                    continue
+                self.start(g, seed=self.options.seed * 1000 + i)
+                self.slot_video[g] = i
+                return
+
+        def finish(g):
+            i, rec = self.slot_video[g], self.records(g)
+            out[i] = dict(name=names[i], frames=rec['frames'], mpjpe=mean(rec['mpjpe']), pampjpe=mean(rec['pampjpe']), pve=mean(rec['pve']))
+            if exppath is not None:
+                d = os.path.join(exppath, names[i])
+                os.makedirs(d, exist_ok=True)
+                write_records(d, rec['frames'] - 1, rec)
+
+        for g in range(self.G):
+            fill(g)
+        while any(i is not None for i in self.slot_video):
+            self.adapt([nxt[g] if self.slot_video[g] is not None else None for g in range(self.G)])
+            for g in range(self.G):
+                if self.slot_video[g] is None:
+                    continue
+                nxt[g] = next(its[g], None)
+                if nxt[g] is None:
+                    finish(g)
+                    fill(g)
+        return out
 
     def predict(self, images):
         """Every video's prediction for its rows of ``images`` with its current weights: a list of G dicts with rotmat, betas,

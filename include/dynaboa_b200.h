@@ -338,6 +338,14 @@ int dboa_keypoint_transform(const float* kp, int n, double t00, double t02, doub
 long long dboa_eval_scratch_floats(int B, int NJ);
 int dboa_eval_metrics(const float* pred_verts, const float* gt_verts_joints, const float* gt_verts_pve, const float* J_regressor, int NJ,
                       int NV, const int* joint_map, int n_map, float* scratch, float* out, int B, dboa_stream_t stream);
+/* the same for `groups` videos of b = B / groups rows each (video g owns the rows [g b, (g + 1) b)), of which only the videos
+ * whose bit is set in `active` take part: the rows of the others are not read and their rows of out are not written.  An
+ * active row is bit-identical to dboa_eval_metrics on that video's rows alone; groups = 1 with bit 0 set is dboa_eval_metrics.
+ * Before any device access: DBOA_ERR_ARG for a NULL pointer, DBOA_ERR_SHAPE for NJ or n_map outside 1..32, B < 1, groups
+ * outside 1..64 or B % groups != 0, then DBOA_ERR_ARG for active == 0 or a bit at position >= groups. */
+int dboa_eval_metrics_active(const float* pred_verts, const float* gt_verts_joints, const float* gt_verts_pve, const float* J_regressor,
+                             int NJ, int NV, const int* joint_map, int n_map, float* scratch, float* out, int B, int groups,
+                             unsigned long long active, dboa_stream_t stream);
 
 /* ---- mesh overlay (render_demo.py:58-153) -----------------------------------------------------
  * replaces: Renderer.render (pyrender + trimesh, OpenGL off-screen) as called by base_adaptor.py:429-443 and

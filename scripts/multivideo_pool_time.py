@@ -3,8 +3,8 @@ measurement:
 
 (a) occupancy: G = 8 slots with n = 1..8 of them active (the others None), ms per step from CUDA events over `frames` steps after
     `warmup` untimed ones, next to single-video ``Adaptor.adapt``;
-(b) pool: `videos` ``SyntheticStream``s with seeded lengths in [4, 40] through G = 8 slots, each slot refilled with ``start`` as
-    soon as its video ends, against the same videos through ``Adaptor.adapt`` one after another.  Adapted frames per second of
+(b) pool: `videos` ``SyntheticStream``s with seeded lengths in [4, 40] through G = 8 slots by ``MultiVideoAdaptor.run``, each
+    slot refilled as soon as its video ends, against the same videos through ``Adaptor.adapt`` one after another.  Adapted frames per second of
     wall time, ending in a device synchronise; the first `warmup` frames of each arm run once before the timed pass.
 
     python scripts/multivideo_pool_time.py [--frames 12] [--warmup 3] [--videos 24] [--seed 0] [--out FILE]"""
@@ -98,25 +98,9 @@ def main():
     vframes = [[fetch(s, t) for t in range(L)] for s, L in zip(vstreams, lengths)]
 
     def pool(mv):
-        queue, slot, done, steps = list(range(args.videos)), [None] * G, 0, 0
-        for g in range(G):
-            if queue:
-                mv.start(g)
-                slot[g] = [queue.pop(0), 0]
-        while any(s is not None for s in slot):
-            mv.adapt([vframes[s[0]][s[1]] if s is not None else None for s in slot])
-            steps += 1
-            for g, s in enumerate(slot):
-                if s is None:
-                    continue
-                s[1] += 1
-                done += 1
-                if s[1] == lengths[s[0]]:
-                    slot[g] = None
-                    if queue:
-                        mv.start(g)
-                        slot[g] = [queue.pop(0), 0]
-        return done, steps
+        steps = mv.global_step
+        done = sum(r['frames'] for r in mv.run(vframes))       # fused_eval 'none': adaptation only
+        return done, mv.global_step - steps
 
     def sequential(ad):
         snap = (ad.model.module.arena.clone(), ad.teacher.arena.clone())
