@@ -39,6 +39,10 @@ class DgradFusedStruct(C.Structure):
                    ('accumulate', I)])
 
 
+class CropDescStruct(C.Structure):
+    _fields_ = [(n, P) for n in ('img', 'wx', 'sx', 'wy', 'sy')] + [(n, I) for n in ('is_u8', 'H', 'W', 'ul_x', 'ul_y', 'Hc', 'Tx', 'Ty')]
+
+
 # name -> (restype, argtypes); mirrors include/dynaboa_b200.h one to one
 SIGNATURES = {
     'dboa_version': (C.c_char_p, []),
@@ -113,6 +117,8 @@ SIGNATURES = {
     'dboa_retrieval_nearest': (I, [P, P, I, I, P, P, P]),
     'dboa_crop_resize_normalize': (I, [P, I, I, I, I, I, I, P, P, I, P, P, I, I, P, P, P, P, P]),
     'dboa_keypoint_transform': (I, [P, I, C.c_double, C.c_double, C.c_double, C.c_double, I, P, P]),
+    'dboa_crop_resize_normalize_groups': (I, [C.POINTER(CropDescStruct), I, C.c_ulonglong, I, P, P, P, L, P, P]),
+    'dboa_keypoint_transform_groups': (I, [P, I, C.POINTER(C.c_double), I, P, I, C.c_ulonglong, P]),
     'dboa_eval_scratch_floats': (L, [I, I]),
     'dboa_eval_metrics': (I, [P, P, P, P, I, I, P, I, P, P, I, P]),
     'dboa_eval_metrics_active': (I, [P, P, P, P, I, I, P, I, P, P, I, I, C.c_ulonglong, P]),

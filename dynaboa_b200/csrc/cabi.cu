@@ -396,6 +396,16 @@ int dboa_keypoint_transform(const float* kp, int n, double t00, double t02, doub
     if (!kp || !out || n < 0) return DBOA_ERR_ARG;
     return keypoint_transform(kp, n, t00, t02, t11, t12, res, out, ST(stream));
 }
+int dboa_crop_resize_normalize_groups(const dboa_crop_desc* frames, int groups, unsigned long long active, int res, const float* mean3,
+                                      const float* std3, float* tmp, long long tmp_floats, float* out, dboa_stream_t stream) {
+    if (!frames || !mean3 || !std3 || !tmp || !out) return DBOA_ERR_ARG;
+    return crop_resize_normalize_groups(frames, groups, active, res, mean3, std3, tmp, tmp_floats, out, ST(stream));
+}
+int dboa_keypoint_transform_groups(const float* kp, int n, const double* t4, int res, float* out, int groups, unsigned long long active,
+                                   dboa_stream_t stream) {
+    if (!kp || !t4 || !out) return DBOA_ERR_ARG;
+    return keypoint_transform_groups(kp, n, t4, res, out, groups, active, ST(stream));
+}
 
 long long dboa_eval_scratch_floats(int B, int NJ) { return (long long)eval_scratch_floats(B, NJ); }
 int dboa_eval_metrics(const float* pred_verts, const float* gt_verts_joints, const float* gt_verts_pve, const float* J_regressor, int NJ,

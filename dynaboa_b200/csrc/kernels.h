@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
+#include "../../include/dynaboa_b200.h"
 
 namespace dboa {
 
@@ -131,6 +132,12 @@ int crop_resize_normalize(const void* img, int is_u8, int H, int W, int ul_x, in
                           const float* wy, const int* sy, int Ty, int res, const float mean[3], const float stdv[3], float* tmp, float* out,
                           cudaStream_t st);
 int keypoint_transform(const float* kp, int n, double t00, double t02, double t11, double t12, int res, float* out, cudaStream_t st);
+// the two above for several streams, one launch per pass (include/dynaboa_b200.h, "grouped input side"); every check but the
+// NULL pointers of the C entries
+int crop_resize_normalize_groups(const dboa_crop_desc* frames, int groups, unsigned long long active, int res, const float mean[3],
+                                 const float stdv[3], float* tmp, long long tmp_floats, float* out, cudaStream_t st);
+int keypoint_transform_groups(const float* kp, int n, const double* t4, int res, float* out, int groups, unsigned long long active,
+                              cudaStream_t st);
 
 // ---- eval.cu (evaluation metrics on the device)
 size_t eval_scratch_floats(int B, int NJ);

@@ -68,15 +68,20 @@ class MultiVideoAdaptor:
     records (``mpjpe_all[g]``, ``pampjpe_all[g]``, ``pve_all[g]``, with 'all' also ``mpjpe_all_lower[g]`` /
     ``pampjpe_all_lower[g]`` and ``mpjpe_statistics[g]`` / ``pampjpe_statistics[g]``, and the run's 2D keypoint losses), and
     ``start(g)`` forms them before it resets the slot.  ``run(videos, exppath=None, names=None)`` adapts a list of videos
-    through the slots and returns one summary per video."""
+    through the slots and returns one summary per video.
+
+    ``motion_lead`` (class attribute, 0 here): slot g's motion term is live while ``video_steps[g] + motion_lead - interval > 0``
+    and reads its frame ``video_steps[g] + motion_lead - interval``; ``feat_sims[g]`` and the upper-level 2D losses are keyed by
+    ``video_steps[g] + motion_lead``.  The webcam client advances its step before the levels (1: webcam.MultiWebcamAdaptor)."""
+
+    motion_lead = 0
 
     def __init__(self, options, n_videos, dynamic_loop=False):
         check_options(options, n_videos, dynamic_loop)
-        from .adaptor import Adaptor
         self.dynamic_loop = bool(dynamic_loop)
         self.G = G = int(n_videos)
         self.options = o = options
-        self.base = base = Adaptor(options)        # checkpoint, SMPL, prior, exemplar bank; never adapted, so it keeps the checkpoint
+        self.base = base = self._make_base(options)    # checkpoint, SMPL, prior, exemplar bank; never adapted, so it keeps the checkpoint
         self.smpl_neutral, self.gmm_f = base.smpl_neutral, base.gmm_f
         if o.retrieval:
             self.centers, self.index, self.h36m_bank, self._dists = base.centers, base.index, base.h36m_bank, base._dists
@@ -110,6 +115,11 @@ class MultiVideoAdaptor:
         self.kp2dloss_lower_all, self.kp2dloss_upper_all = [[] for _ in range(G)], [{} for _ in range(G)]
         for g in range(G):
             self.start(g)
+
+    def _make_base(self, options):
+        """The single-video adaptor whose checkpoint, SMPL models, prior and exemplar bank the pool shares."""
+        from .adaptor import Adaptor
+        return Adaptor(options)
 
     def start(self, g, seed=None):
         """Put a new video into slot g: theta and teacher from the checkpoint, zero Adam moments, step and frame counts, an empty
@@ -170,10 +180,10 @@ class MultiVideoAdaptor:
             h.pop(k - self.options.interval - 1, None)
 
     def get_hist(self):
-        """The history rows of the slots whose motion term is live, each from its own frame ``interval`` frames back; the rows of
-        the other slots are placeholders."""
+        """The history rows of the slots whose motion term is live, each from its own frame ``interval - motion_lead`` frames
+        back; the rows of the other slots are placeholders."""
         live = self._slots(self.motion_active)
-        frames = [self.histories[g][self.video_steps[g] - self.options.interval] for g in live]
+        frames = [self.histories[g][self.video_steps[g] + self.motion_lead - self.options.interval] for g in live]
         if len(live) == self.G and all(f is frames[0] for f in frames):
             return frames[0]                                     # one pool frame holds every slot's history rows
         if self._hist is None:
@@ -253,10 +263,14 @@ class MultiVideoAdaptor:
                 if missing:
                     raise ValueError(f'slot {g}: fused_eval={self.fused_eval!r} needs the ground truth {", ".join(missing)} in the batch')
         self._check_runtime()
+        self._adapt_staged(on, self._stage(batches))
+
+    def _adapt_staged(self, on, batch):
+        """The frame of ``adapt`` on rows already staged in ``batch`` (the persistent staging), for the slots in ``on`` (bit
+        mask): a subclass that writes the staged rows itself runs the same step through here."""
         o = self.options
         self._on = on
-        self._live = sum(1 << g for g in self._slots(on) if self.video_steps[g] - o.interval > 0)
-        batch = self._stage(batches)
+        self._live = sum(1 << g for g in self._slots(on) if self.video_steps[g] + self.motion_lead - o.interval > 0)
         prev = self.last_upper_loss
         self.fit_losses, self.kp2dlosses_lower, self.kp2dlosses_upper = {}, [], {}
         self._evals, self._gt, self._lower_evals = [], None, 0
@@ -272,7 +286,7 @@ class MultiVideoAdaptor:
         if o.dynamic_boa:
             for g in self._slots(on):
                 self.optim_step_record[g].append(self.optimized_step[g])
-                self.feat_sims[g][self.video_steps[g]] = self.loop_feat_sims[g]
+                self.feat_sims[g][self.video_steps[g] + self.motion_lead] = self.loop_feat_sims[g]
         self._pending.append((on, {g: self.video_steps[g] for g in self._slots(on)}, self.fused_eval == 'all', self._evals,
                               list(self.kp2dlosses_lower), self.kp2dlosses_upper.get(self.global_step)))
         if len(self._pending) >= PENDING_FRAMES:
@@ -337,7 +351,7 @@ class MultiVideoAdaptor:
                     self.pampjpe_statistics[g][t] = [x[1] for x in thetas]
                 self.kp2dloss_lower_all[g] += [float(v[g]) for v in low]
                 if up is not None:
-                    self.kp2dloss_upper_all[g][t] = float(up[g])
+                    self.kp2dloss_upper_all[g][t + self.motion_lead] = float(up[g])
         self._pending = []
 
     def records(self, g):
@@ -402,13 +416,15 @@ class MultiVideoAdaptor:
                     fill(g)
         return out
 
-    def predict(self, images):
+    def predict(self, images, active=None):
         """Every video's prediction for its rows of ``images`` with its current weights: a list of G dicts with rotmat, betas,
-        cam, joints (49) and vertices."""
+        cam, joints (49) and vertices.  ``active`` (bit mask; None: every slot): one grouped forward of only those slots
+        (``dboa_hmr_forward_active``), then the SMPL decode; the entries of the other slots are None."""
         with torch.no_grad():
             image = images.to(self.thetas.device).contiguous().float()
-            rot, shape, cam, _, _ = hmr_mod.raw_forward(self.thetas, self.buffers, image, groups=self.G)
+            rot, shape, cam, _, _ = hmr_mod.raw_forward(self.thetas, self.buffers, image, groups=self.G, active=active)
             out = self.base.decode_smpl_params(rot, shape)
         b = image.shape[0] // self.G
         s = [slice(g * b, (g + 1) * b) for g in range(self.G)]
-        return [dict(rotmat=rot[q], betas=shape[q], cam=cam[q], joints=out['s3d'][q], vertices=out['vts'][q]) for q in s]
+        return [dict(rotmat=rot[q], betas=shape[q], cam=cam[q], joints=out['s3d'][q], vertices=out['vts'][q])
+                if active is None or (active >> g) & 1 else None for g, q in enumerate(s)]

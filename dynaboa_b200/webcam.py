@@ -16,15 +16,20 @@ What differs from the benchmark client, and where it lands here:
 
 ``online_adaptation(frame, detections)`` returns the reference's result dictionary (``vts``, ``cam``, ``bbox`` and, with
 ``test_basemodel``, ``vts_base`` / ``cam_base``).
+
+``MultiWebcamAdaptor`` serves several live streams from one GPU: a ``multivideo.MultiVideoAdaptor`` pool with the webcam
+client's semantics per stream, whose input side crops every stream's frame in one grouped call (DESIGN.md section 10,
+"Webcam streams").
 """
 from types import SimpleNamespace
 
 import numpy as np
 import torch
 
-from . import config, dataprocess
+from . import config, dataprocess, hmr as hmr_mod
 from .adaptor import Adaptor
 from .hmr import hmr
+from .multivideo import MultiVideoAdaptor
 
 
 def webcam_options(o):
@@ -104,3 +109,151 @@ class WebcamAdaptor(Adaptor):
                 rot_b, shape_b, cam_b = self.basemodel(image)
                 res.update(vts_base=self.decode_smpl_params(rot_b, shape_b)['vts'], cam_base=cam_b)
         return res
+
+
+def _box(det, scaleFactor=1.2):
+    """``WebcamAdaptor.dataprocess``'s host side for one stream: (center, scale, bbox (1, 3), keypoints with the 0.3 confidence
+    threshold applied in double)."""
+    kp = np.array(det, dtype=np.float64, copy=True)
+    x0, y0, x1, y1 = kp[:, 0].min(), kp[:, 1].min(), kp[:, 0].max(), kp[:, 1].max()
+    center = [(x1 + x0) / 2, (y1 + y0) / 2]
+    scale = scaleFactor * max(x1 - x0, y1 - y0) / 200
+    kp[:, 2] = kp[:, 2] > 0.3
+    return center, scale, np.stack([center[0], center[1], scale * 200])[None, :], kp
+
+
+def _frame_ok(f):
+    dt = f.dtype if torch.is_tensor(f) else np.dtype(f.dtype)
+    ok = (torch.uint8, torch.float32) if torch.is_tensor(f) else (np.dtype(np.uint8), np.dtype(np.float32))
+    return f.ndim == 3 and f.shape[2] == 3 and dt in ok
+
+
+class MultiWebcamAdaptor(MultiVideoAdaptor):
+    """``MultiWebcamAdaptor(options, n_streams, dynamic_loop=False)``: G live streams (cameras, or people's recorded clips)
+    adapted in lockstep, each with the semantics of its own ``WebcamAdaptor``: the 25 OpenPose joints in the 2D and motion
+    terms (``kp_range``), the teacher in eval mode, no retrieval, and the motion term ``interval - 1`` frames back, live one
+    frame earlier (``motion_lead = 1``).  ``options`` is the webcam script's namespace (completed by ``webcam_options``);
+    ``dynamic_loop=True`` accepts ``dynamic_boa=1`` and runs the re-adaptation loop per stream.
+
+    ``online_adaptation(frames, detections)`` advances every stream that has a frame and detections by one tick: the boxes on
+    the host, one grouped crop and one grouped keypoint call into the pool's staging rows, the bilevel step, one masked output
+    forward.  ``adapt_processed`` does the same on already cropped rows.  ``reload(g)`` is the demo's key ``r`` for stream g;
+    ``start(g)`` puts a new camera into slot g.  Per slot, ``video_steps[g]`` counts the stream's frames."""
+    kp_range = (0, 25)
+    motion_lead = 1
+
+    def __init__(self, options, n_streams, dynamic_loop=False):
+        super().__init__(webcam_options(options), n_streams, dynamic_loop)
+        self.fused_eval = 'none'
+
+    def _make_base(self, options):
+        return WebcamAdaptor(SimpleNamespace(**dict(vars(options), test_basemodel=0)))     # base outputs: its own checkpoint arena
+
+    def _rows(self):
+        """The pool's persistent staging rows, (G, 3, 224, 224) images and the (G, 49, 3) keypoint block."""
+        if self._frames is None:
+            dev = self.thetas.device
+            self._frames = {'image': torch.zeros(self.G, 3, 224, 224, device=dev), 'smpl_j2d': torch.zeros(self.G, 49, 3, device=dev)}
+        return self._frames
+
+    def reload(self, g):
+        """Key ``r`` of the demo for stream g (reference dynaboa_webcam.py:184-194): theta and teacher back to the checkpoint and
+        a fresh Adam (zero moments, step count 0).  The stream's history and frame count are kept, so its motion term stays as
+        it was; the other streams are left alone."""
+        if not isinstance(g, int) or not 0 <= g < self.G:
+            raise ValueError(f'slot {g!r} is not one of the {self.G} slots')
+        self.thetas[g].copy_(self.base.model.module.arena.detach())
+        if self.teachers is not None:
+            self.teachers[g].copy_(self.base.teacher.arena.detach())
+        self.m[g].zero_()
+        self.v[g].zero_()
+        self.step_counts[g] = 0
+
+    def online_adaptation(self, frames, detections):
+        """One tick of every stream (reference :221-337 per stream).  ``frames[g]``: an (H, W, 3) RGB uint8 / float32 frame (numpy
+        or CUDA tensor), ``detections[g]``: its (1, 25, 3) or (25, 3) OpenPose detections in frame pixels; a None frame or None
+        detections (no person found) leaves stream g as it was.  Returns per stream the reference's result dictionary, or None
+        for a stream that sat the tick out (all None when no stream has a frame)."""
+        on, bboxes = self.input_side(frames, detections)
+        return self._tick(on, bboxes) if on else [None] * self.G
+
+    def input_side(self, frames, detections):
+        """The input side of ``online_adaptation`` alone: the boxes on the host (``WebcamAdaptor.dataprocess``'s arithmetic),
+        then one grouped crop and one grouped keypoint call into the staging rows of the streams that have a frame and
+        detections.  Returns (their bit mask, per stream the (1, 3) bbox or None)."""
+        G = self.G
+        if len(frames) != G or len(detections) != G:
+            raise ValueError(f'expected {G} frames and {G} detections, one per stream, got {len(frames)} and {len(detections)}')
+        on, centers, scales, bboxes, kps = 0, [None] * G, [None] * G, [None] * G, np.zeros((G, 25, 3))
+        for g, (f, d) in enumerate(zip(frames, detections)):
+            if f is None or d is None:
+                continue
+            det = np.asarray(d.cpu() if torch.is_tensor(d) else d)
+            if det.shape == (1, 25, 3):
+                det = det[0]
+            if det.shape != (25, 3):
+                raise ValueError(f'stream {g}: detections of shape {det.shape}, expected (1, 25, 3) or (25, 3)')
+            if not _frame_ok(f):
+                raise ValueError(f'stream {g}: expected an (H, W, 3) uint8 / float32 frame, got {tuple(f.shape)} {f.dtype}')
+            centers[g], scales[g], bboxes[g], kps[g] = _box(det)
+            on |= 1 << g
+        if on == 0:
+            return 0, bboxes
+        self._check_runtime()
+        dev, rows = self.thetas.device, self._rows()
+        imgs = [None if not (on >> g) & 1 else (f if torch.is_tensor(f) else torch.from_numpy(np.ascontiguousarray(f))).to(dev, non_blocking=True)
+                for g, f in enumerate(frames)]
+        dataprocess.crop_groups(imgs, centers, scales, rows['image'], on)
+        dataprocess.j2d_processing_groups(torch.from_numpy(kps).float().to(dev), centers, scales, rows['smpl_j2d'], on)
+        return on, bboxes
+
+    def adapt_processed(self, images, kps, bboxes=None, active=None):
+        """The same on already cropped frames: ``images`` (G, 3, 224, 224) and ``kps`` (G, 49, 3) (rows 0..24 = OpenPose joints in
+        [-1, 1]) with ``active`` (bit mask; None: every stream), or lists of G (1, 3, 224, 224) / (1, 49, 3) entries with None
+        for a stream that sits the tick out.  ``bboxes[g]`` goes to stream g's result."""
+        G = self.G
+        if isinstance(images, (list, tuple)) != isinstance(kps, (list, tuple)):
+            raise ValueError('images and kps must both be lists or both be tensors')
+        if isinstance(images, (list, tuple)):
+            if len(images) != G or len(kps) != G:
+                raise ValueError(f'expected {G} images and {G} keypoint blocks, one per stream, got {len(images)} and {len(kps)}')
+            pairs = [None if i is None or k is None else (i, k) for i, k in zip(images, kps)]
+        else:
+            if tuple(images.shape) != (G, 3, 224, 224) or tuple(kps.shape) != (G, 49, 3):
+                raise ValueError(f'expected ({G}, 3, 224, 224) images and a ({G}, 49, 3) keypoint block, got {tuple(images.shape)} '
+                                 f'and {tuple(kps.shape)}')
+            active = (1 << G) - 1 if active is None else int(active)
+            pairs = [(images[g:g + 1], kps[g:g + 1]) if (active >> g) & 1 else None for g in range(G)]
+        for g, p in enumerate(pairs):
+            if p is not None and (tuple(p[0].shape) != (1, 3, 224, 224) or tuple(p[1].shape) != (1, 49, 3)):
+                raise ValueError(f'stream {g}: image {tuple(p[0].shape)} and keypoints {tuple(p[1].shape)}, expected (1, 3, 224, 224) '
+                                 'and (1, 49, 3)')
+        on = sum(1 << g for g, p in enumerate(pairs) if p is not None)
+        if on == 0:
+            return [None] * G
+        self._check_runtime()
+        self._rows()
+        self._stage([None if p is None else {'image': p[0], 'smpl_j2d': p[1]} for p in pairs])
+        return self._tick(on, [None] * G if bboxes is None else bboxes)
+
+    def _tick(self, on, bboxes):
+        """The pool step on the staged rows, then one masked forward of the adapted weights (and, with ``test_basemodel``, one
+        forward of the checkpoint arena the base adaptor holds) and the result dictionaries."""
+        rows = self._frames
+        self._adapt_staged(on, rows)
+        preds = self.predict(rows['image'], on)
+        base = None
+        if self.options.test_basemodel:
+            with torch.no_grad():
+                rot, shape, cam, _, _ = hmr_mod.raw_forward(self.base.model.module.arena, self.buffers, rows['image'])
+                base = (self.base.decode_smpl_params(rot, shape)['vts'], cam)
+        out = []
+        for g, p in enumerate(preds):
+            if p is None:
+                out.append(None)
+                continue
+            res = {'vts': p['vertices'], 'cam': p['cam'], 'bbox': bboxes[g]}
+            if base is not None:
+                res.update(vts_base=base[0][g:g + 1], cam_base=base[1][g:g + 1])
+            out.append(res)
+        return out

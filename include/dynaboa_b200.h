@@ -328,6 +328,34 @@ int dboa_crop_resize_normalize(const void* img, int is_u8, int H, int W, int ul_
  * then 2 p / res - 1; t00, t02, t11, t12: the non-zero entries of get_transform(center, scale, res) (:13-37, rot = 0) */
 int dboa_keypoint_transform(const float* kp, int n, double t00, double t02, double t11, double t12, int res, float* out,
                             dboa_stream_t stream);
+/* Grouped input side: the two calls above for the frames of `groups` streams (one camera each), of which those whose bit is
+ * set in `active` take part.  One frame per stream; frames may differ in size and dtype.  dboa_crop_desc: the arguments of
+ * dboa_crop_resize_normalize that describe one frame and its crop (img, is_u8, H, W, ul_x, ul_y, Hc and the wx / sx / Tx,
+ * wy / sy / Ty tables, all device pointers).  `frames` is a HOST array of `groups` descriptors; the active ones are passed to
+ * the kernels by value, so a call makes no host-to-device copy and never synchronises (the descriptors of idle streams are
+ * not read).  Two launches, whatever `groups`: the rows pass over every active frame's Hc * res outputs, then one grid row per
+ * active frame.  tmp: sum over the active frames of Hc * res * 3 floats (tmp_floats: its size).  out (groups,3,res,res): row g
+ * of an active stream is bit-identical to dboa_crop_resize_normalize on frame g alone; the frames of idle streams are not
+ * read and their rows of out are not written.
+ * Before any device access: DBOA_ERR_ARG for a NULL frames, mean3, std3, tmp or out, DBOA_ERR_SHAPE for groups
+ * outside 1..64 or res < 1, DBOA_ERR_ARG for active == 0 or a bit at position >= groups, then, per active descriptor,
+ * DBOA_ERR_ARG for a NULL pointer and DBOA_ERR_SHAPE for H, W, Hc, Tx or Ty < 1, then DBOA_ERR_ARG for too small a tmp. */
+typedef struct dboa_crop_desc {
+    const void* img;
+    const float* wx;
+    const int* sx;
+    const float* wy;
+    const int* sy;
+    int is_u8, H, W, ul_x, ul_y, Hc, Tx, Ty;
+} dboa_crop_desc;
+int dboa_crop_resize_normalize_groups(const dboa_crop_desc* frames, int groups, unsigned long long active, int res, const float* mean3,
+                                      const float* std3, float* tmp, long long tmp_floats, float* out, dboa_stream_t stream);
+/* kp (groups,n,3) detections of every stream -> rows [0, n) of out (groups,49,3) as dboa_keypoint_transform (bit for bit), rows
+ * [n, 49) zeroed; t4: HOST array (groups,4) of each stream's t00, t02, t11, t12.  Streams whose bit is clear in `active`: kp
+ * not read, out not written.  DBOA_ERR_ARG for a NULL pointer, DBOA_ERR_SHAPE for groups outside 1..64, n outside 0..49 or
+ * res < 1, then DBOA_ERR_ARG for active == 0 or a bit at position >= groups; all before any device access.  One launch. */
+int dboa_keypoint_transform_groups(const float* kp, int n, const double* t4, int res, float* out, int groups, unsigned long long active,
+                                   dboa_stream_t stream);
 
 /* ---- evaluation metrics (dynaboa_benchmark.py:217-240, utils/pose_utils.py:9-64) -----------------
  * pred_verts, gt_verts_joints (gender-selected SMPL mesh), gt_verts_pve (neutral mesh): (B,NV,3);
