@@ -11,12 +11,14 @@ Two entry points per frame:
   (see fused.py).  This is what ``bench.py`` times.
 """
 import os.path as osp
+import random
 
 import numpy as np
 import torch
 
 from . import _lib, constants
 from .base_adaptor import BaseAdaptor
+from .fused import Step, _ArenaModel, fused_adapt
 
 
 RESULT_FILES = ('lowerlevel_kp2dloss.pt', 'upperlevel_kp2dloss.pt', 'res.pt', 'lower_res.pt', 'steps_statistic_res.pt', 'feat_sims.pt',
@@ -49,10 +51,15 @@ def write_records(exppath, step, rec):
 
 
 class Adaptor(BaseAdaptor):
+    kp_range = (25, 24)          # joints of the 2D and motion terms (fused.Step)
+    motion_lead = 0              # the motion term is live while global_step + motion_lead - interval > 0 (before save_hist)
+
     def __init__(self, options):
         super().__init__(options)
         self.model.eval()        # the reference driver does this before every frame (dynaboa_benchmark.py:89)
         self.reset_records()
+        self.fused_eval = 'final'                          # adapt's evaluations: 'none', 'final' or 'all'
+        self.phase_events = None                           # a list: adapt records CUDA events at its phase boundaries
 
     def reset_records(self):
         n = len(self.dataloader)
@@ -171,16 +178,13 @@ class Adaptor(BaseAdaptor):
         return out, ev
 
     def inference(self, batch, model, need_feature=False):
-        image, gt_pose, gt_betas, gender = batch['image'], batch['pose'], batch['betas'], batch['gender']
+        image = batch['image']
         model.eval()
         with torch.no_grad():
             out = model(image, need_feature)
             pred_rotmat, pred_shape, pred_cam = out[0], out[1], out[2]
             pred_vertices = self.decode_smpl_params(pred_rotmat, pred_shape)['vts']
-            gt_vertices = self.smpl_male(global_orient=gt_pose[:, :3], body_pose=gt_pose[:, 3:], betas=gt_betas).vertices
-            gt_vertices_f = self.smpl_female(global_orient=gt_pose[:, :3], body_pose=gt_pose[:, 3:], betas=gt_betas).vertices
-            gt_vertices = torch.where((gender == 1).view(-1, 1, 1), gt_vertices_f, gt_vertices)
-            gt_neutral = self.smpl_neutral(betas=gt_betas, body_pose=gt_pose[:, 3:], global_orient=gt_pose[:, :3], pose2rot=True).vertices
+            gt_vertices, gt_neutral = self._gt_meshes(batch)
             # H36M-regressor joints, MPJPE, Procrustes PA-MPJPE and PVE in two launches; ONE 3-float read-back per sample
             # (the reference copies joints and both meshes to the host and runs a numpy SVD per sample: :217-240)
             metrics = self.eval_metrics(pred_vertices, gt_vertices, gt_neutral).cpu().numpy()
@@ -215,9 +219,53 @@ class Adaptor(BaseAdaptor):
             _lib.call('dboa_eval_metrics_active', *args, int(groups), (1 << int(groups)) - 1 if active is None else int(active), _lib.stream())
         return out
 
+    def _gt_meshes(self, batch):
+        """The ground-truth meshes of ``batch``: gender-selected (male / female SMPL) and neutral."""
+        pose, betas = batch['pose'], batch['betas']
+        gt = self.smpl_male(global_orient=pose[:, :3], body_pose=pose[:, 3:], betas=betas).vertices
+        gt_f = self.smpl_female(global_orient=pose[:, :3], body_pose=pose[:, 3:], betas=betas).vertices
+        gt = torch.where((batch['gender'] == 1).view(-1, 1, 1), gt_f, gt)
+        return gt, self.smpl_neutral(betas=betas, body_pose=pose[:, 3:], global_orient=pose[:, :3], pose2rot=True).vertices
+
+    # ------------------------------------------------------------------ the same step without autograd (fused.py)
     def adapt(self, batch):
-        from .fused import fused_adapt
-        return fused_adapt(self, batch)
+        """One frame through ``fused.fused_adapt``, its records filed under the reference's names; returns ``inference``'s."""
+        import torch.distributed as dist
+        s, opt = self._step or self._make_step(), self.optimizer
+        s.eval_mode, s.phase_events = self.fused_eval, self.phase_events
+        s.grad_sync = opt.grad_sync if (opt.grad_sync is not None and dist.is_initialized() and dist.get_world_size() > 1) else None
+        f = fused_adapt(s, batch, 1, [self.global_step])
+        self.fit_losses.update({k: v[0] for k, v in f.fit.items()})
+        self.kp2dlosses_lower += [v[0] for v in f.lower]
+        if 'ul/s2dloss' in f.fit:
+            self.kp2dlosses_upper[self.global_step] = f.fit['ul/s2dloss'][0]
+        self.last_upper_loss = f.upper_loss[0]
+        if f.picks is not None:
+            self.last_retrieval = f.picks[0]
+        if f.steps is not None:
+            self.feat_sims[self.global_step], self.optimized_step = f.sims[0], f.steps[0]
+            self.optim_step_record.append(f.steps[0])
+        return f.result
+
+    def _make_step(self):
+        o = self.options
+        model = getattr(self.model, 'module', self.model)
+        teacher = self.teacher if o.use_meanteacher else None
+        self._step = Step(o, 1, model.arena, model.grad_arena(), model._buffers, self.smpl_neutral, self.gmm_f,
+                          teacher=None if teacher is None else teacher.arena, teacher_buffers=None if teacher is None else teacher._buffers,
+                          teacher_masks=None if teacher is None else lambda B, device, mask: teacher._masks(B, device),
+                          kp_range=self.kp_range, motion_lead=self.motion_lead, bank=self.bank if o.retrieval else None,
+                          rngs=[random] if o.retrieval else None, save_hist=lambda image, kp, mask: self.save_hist(image, kp),
+                          get_hist=lambda live: self.get_hist(), adam=self._adam, evaluate=self._evaluate, reduce_terms=self._reduce_terms)
+        return self._step
+
+    def _adam(self, mask, teacher=None, alpha=0.0):
+        if self._step.grad_sync is not None:
+            self.optimizer.reduced = True                  # the level's last backward all-reduces on the communication stream
+        self.optimizer.step(teacher=None if teacher is None else self.teacher, alpha=alpha)
+
+    def _evaluate(self, batch, arena, mask, inner):
+        return self.inference(batch, self.model if inner is None else _ArenaModel(getattr(self.model, 'module', self.model), arena))
 
 
 class InternetAdaptor(Adaptor):
@@ -225,11 +273,8 @@ class InternetAdaptor(Adaptor):
     ``Adaptor.adaptation`` minus the per-step evaluation, ``inference`` only decodes the mesh and caches ``Pred_<step>.pt``."""
 
     def reset_records(self):
-        self.feat_sims, self.optim_step_record = {}, []
+        super().reset_records()
         self.mpjpe_statistics, self.pampjpe_statistics = [], []
-        self.mpjpe_all_lower = [[] for _ in range(self.options.inner_step)]
-        self.pampjpe_all_lower = [[] for _ in range(self.options.inner_step)]
-        self.history, self.kp2dlosses_lower, self.kp2dlosses_upper = {}, [], {}
 
     def excute(self, max_frames=None, fused=False):
         self.reset_records()

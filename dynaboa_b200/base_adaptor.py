@@ -19,27 +19,18 @@ import numpy as np
 import torch
 
 from . import config, constants, losses, optim
+from .fused import Bank, cosines, retrieve
 from .geometry import batch_rodrigues, project_normalized
 from .hmr import hmr
 from .maml import MAML
 from .prior import MaxMixturePrior
 from .smpl import SMPL
 from . import _lib
-from ._lib import ptr, stream
 
 
 class _NullWriter:
     def add_scalar(self, *a, **k):
         pass
-
-
-def _dense_ptr_tensor(t):
-    """A tensor whose memory is one dense block of ``numel`` floats (permuted views qualify)."""
-    t = t.detach()
-    span = 1 + sum((s - 1) * st for s, st in zip(t.shape, t.stride()))
-    if t.dtype == torch.float32 and span == t.numel():
-        return t
-    return t.float().contiguous()
 
 
 class BaseAdaptor:
@@ -87,16 +78,16 @@ class BaseAdaptor:
         self.index = cl['index']
         bank = torch.load(config.RETRIEVAL_BANK, weights_only=False)
         self.h36m_bank = {k: v.float().to(self.device).contiguous() for k, v in bank.items()}
+        self.bank = Bank(self.centers, self.index, self.h36m_bank, torch.zeros(self.centers.shape[0], dtype=torch.float32, device=self.device))
         self._best = torch.zeros(1, dtype=torch.int32, device=self.device)
-        self._dists = torch.zeros(self.centers.shape[0], dtype=torch.float32, device=self.device)
 
     def get_h36m_data(self, indice):
         return {k: v[indice:indice + 1] for k, v in self.h36m_bank.items()}
 
     def retrieval(self, feature):
         """reference :82-96: nearest cluster centre by cosine distance, then ``random.sample`` inside it."""
-        from .fused import retrieve
-        (self.last_retrieval,), batch = retrieve(self, feature.detach().reshape(1, -1)[:, :2048], [random])
+        (self.last_retrieval,), batch = retrieve(self.bank, feature.detach().reshape(1, -1)[:, :2048], [random], 1, self._best,
+                                                 self.options.sample_num)
         return batch
 
     def set_model_optim(self):
@@ -110,6 +101,7 @@ class BaseAdaptor:
             self.model.load_state_dict({k.replace('module.', ''): v for k, v in checkpoint['model'].items()}, strict=True)
         self.optimizer = optim.FusedAdam(self.model.parameters(), lr=self.options.lr, betas=(self.options.beta1, self.options.beta2),
                                          model=self.model)
+        self._step = None                    # Adaptor.adapt's fused.Step: built again over the new arenas
 
     def set_teacher(self):
         checkpoint = torch.load(self.options.model_file, map_location='cpu', weights_only=False)
@@ -118,6 +110,7 @@ class BaseAdaptor:
             p.requires_grad_(False)
         self.teacher = model.to(self.device)
         self.teacher.load_state_dict({k.replace('module.', ''): v for k, v in checkpoint['model'].items()}, strict=True)
+        self._step = None
         # the reference never calls teacher.eval(): its dropout stays active (SURVEY.md Appendix D)
         if not getattr(self.options, 'teacher_dropout', 1):
             self.teacher.eval()
@@ -177,29 +170,19 @@ class BaseAdaptor:
         pass
 
     def cal_feature_diff(self, features_i, features_j):
-        """reference :211-219.  One launch pair returns, per feature, the sums (a.b, |a|^2, |b|^2); under data-parallel
-        adaptation they are all-reduced over the ranks first (the reference flattens across the batch, :215), so every
-        rank sees the same cosines and takes the same number of dynamic steps -- the gradient all-reduce inside those
-        steps would dead-lock otherwise."""
-        import ctypes as C
-        import torch.distributed as dist
-        n = len(features_i)
-        fa = [_dense_ptr_tensor(t) for t in features_i]
-        fb = [_dense_ptr_tensor(t) for t in features_j]
-        pa = (C.c_void_p * n)(*[t.data_ptr() for t in fa])
-        pb = (C.c_void_p * n)(*[t.data_ptr() for t in fb])
-        ln = (C.c_longlong * n)(*[t.numel() for t in fa])
-        need = _lib.load().dboa_cosine_partial_floats(ln, n)
-        if self._cos_partial is None or self._cos_partial.numel() < need:
-            self._cos_partial = torch.empty(need, dtype=torch.float32, device=self.device)
-        terms = torch.empty(n, 3, dtype=torch.float64, device=self.device)
-        _lib.call('dboa_cosine_terms', pa, pb, ln, n, ptr(self._cos_partial), self._cos_partial.numel(), ptr(terms), stream())
-        if dist.is_available() and dist.is_initialized() and dist.get_world_size(self.dp_group) > 1:
-            dist.all_reduce(terms, op=dist.ReduceOp.SUM, group=self.dp_group)
-        t = terms.cpu()                                                   # the one host sync of the dynamic test
-        cos = (t[:, 0] / (t[:, 1].sqrt().clamp_min(1e-12) * t[:, 2].sqrt().clamp_min(1e-12))).float()
+        """reference :211-219: the cosine of each feature pair, one video of ``fused.cosines`` (the sums all-reduced over the
+        data-parallel ranks first: ``_reduce_terms``)."""
+        cos, self._cos_partial = cosines(features_i, features_j, 1, 1, self._cos_partial, self._reduce_terms)
+        cos, n = cos[0], len(features_i)
         self.fit_losses['feat_sim/cos_sim'] = cos.sum() / (n - 1)        # reference :218 divides by the last index
         return {i: {'cos': float(cos[i])} for i in range(n)}
+
+    def _reduce_terms(self, terms):
+        """Data parallel: the feature test's sums all-reduced over the ranks (the reference flattens across the batch, :215), so
+        every rank takes the same dynamic steps -- the gradient all-reduce inside them would dead-lock otherwise."""
+        import torch.distributed as dist
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size(self.dp_group) > 1:
+            dist.all_reduce(terms, op=dist.ReduceOp.SUM, group=self.dp_group)
 
     # ------------------------------------------------------------------ losses (reference :320-422)
     def cal_shape_prior(self, pred_betas):

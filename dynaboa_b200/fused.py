@@ -12,24 +12,81 @@ What changes relative to the autograd path (``Adaptor.adaptation``), none of it 
 * Adam and the mean-teacher EMA run as one fused sweep; frame and teacher-consistency terms share one loss-head
   launch; the only host syncs are retrieval's cluster index and the ``dynamic_boa`` decision.
 
-The same step adapts G videos at once (``multivideo.MultiVideoAdaptor``): their weight, teacher and gradient arenas are
-(G, P) stacks instead of flat arenas, video g owns the rows [g * b, (g + 1) * b) of every batch, and every network pass and
-loss head is one grouped call.  When only some of the videos advance this frame (``ad.active``, an int whose bit g means video
-g takes part; None: all), the network passes skip the others and the element-wise sweeps touch only the active videos' rows of
-the stacks.  DESIGN.md section 10.
+The step reads a ``Step``, built once by each adaptor: G videos' arenas (flat for ``adaptor.Adaptor``, (G, P) stacks for
+``multivideo.MultiVideoAdaptor``; video g owns the rows [g * b, (g + 1) * b) of every batch, and every pass is one grouped
+call) and callbacks for what stays with the adaptor.  A set of videos is an int whose bit g means video g takes part (all:
+``(1 << G) - 1``); passes and sweeps skip the others.  ``fused_adapt`` returns the records (``Frame``).  DESIGN.md section 10.
 """
+import collections
 import ctypes as C
 import os
-import random
 
 import torch
 
-from . import _lib, hmr as hmr_mod, losses
+from . import _lib, hmr as hmr_mod
 from ._lib import ptr, stream
 
 
 _SIDE = {}
 _TEACHER_OVERLAP = os.environ.get('DBOA_TEACHER_STREAM', '1') != '0'     # 0: teacher forward on the caller's stream
+
+# retrieval's exemplars: cluster centres (K, 2048), each cluster's exemplars, their tensors by name, (K,) distance scratch
+Bank = collections.namedtuple('Bank', 'centers index exemplars dists')
+
+
+class Step:
+    """What the bilevel step reads and owns.
+
+    ``options``; ``G`` videos; ``theta``, ``grad``, ``buffers``: the weight and gradient arenas (flat for one video, (G, P)
+    stacks) and the network's constant buffers; ``teacher``, ``teacher_buffers``: the mean teacher's (None without one);
+    ``teacher_masks(B, device, mask)``: the keep-masks of the teacher forward (or None: no dropout); ``smpl_neutral``,
+    ``gmm_f``: neutral SMPL and the pose prior; ``kp_range``: (first, count) joints of the 2D and motion terms; ``motion_lead``:
+    video g's motion term is live while its frame count + ``motion_lead`` - ``interval`` > 0; ``bank``, ``rngs``: retrieval's ``Bank`` and
+    per-video generators; ``save_hist(image, kp, mask)`` / ``get_hist(live)``: the history frames; ``adam(mask, teacher=None,
+    alpha=0.0)``: Adam (+ EMA into ``teacher``) of the videos in ``mask``; ``evaluate(batch, arena, mask, inner)``: one
+    evaluation of ``arena`` (``inner``: the inner step of fast weights, None for theta); ``reduce_terms(terms)``: the
+    data-parallel sum of the feature test's sums (None: one rank).  Set per frame: ``eval_mode`` ('none', 'final', 'all'),
+    ``grad_sync`` (the data-parallel ``BucketedGradSync`` or None) and ``phase_events`` (a list: CUDA events per phase)."""
+
+    def __init__(self, options, G, theta, grad, buffers, smpl_neutral, gmm_f, teacher=None, teacher_buffers=None, teacher_masks=None,
+                 kp_range=(25, 24), motion_lead=0, bank=None, rngs=None, save_hist=None, get_hist=None, adam=None, evaluate=None,
+                 reduce_terms=None):
+        self.options, self.G, self.theta, self.grad, self.buffers, self.smpl_neutral, self.gmm_f = options, G, theta, grad, buffers, smpl_neutral, gmm_f
+        self.teacher, self.teacher_buffers, self.teacher_masks = teacher, teacher_buffers, teacher_masks
+        self.kp_range, self.motion_lead, self.bank, self.rngs = kp_range, motion_lead, bank, rngs
+        self.save_hist, self.get_hist, self.adam, self.evaluate, self.reduce_terms = save_hist, get_hist, adam, evaluate, reduce_terms
+        self.eval_mode, self.grad_sync, self.phase_events = 'none', None, None
+        # the step's scratch: motion pair images and gradients, cosine partial sums, fast weights, inner gradient, cluster index
+        self._pair = self._bgrad_flat = self._cos_partial = self._fast = self._inner_grad = None
+        self._best = None if bank is None else torch.zeros(G, dtype=torch.int32, device=bank.centers.device)
+
+
+class Frame:
+    """What ``fused_adapt`` returns for the videos in ``mask``, each loss (G,) (unspecified outside them): ``fit`` (the ``fit_losses`` terms; the last
+    upper level's 2D loss is ``ul/s2dloss``), ``lower`` (each lower level's 2D loss), ``upper_loss``; per video ``steps``
+    and ``sims`` (the dynamic loop's trip count and cosines; None without it), ``picks`` (its last retrieval, None where it
+    drew none; None without retrieval); ``result``: the return of the last evaluation of theta."""
+
+    def __init__(self, mask):
+        self.mask, self.fit, self.lower, self.upper_loss = mask, {}, [], None
+        self.steps = self.sims = self.picks = self.result = None
+
+
+def pick(mask, G, a, b=None):
+    """(G,) per video: ``a`` for the videos in ``mask``, ``b`` (None: NaN) for the others; ``a`` itself for every video."""
+    if mask == (1 << G) - 1:
+        return a
+    keep = torch.tensor([bool((mask >> g) & 1) for g in range(G)], device=a.device)
+    return torch.where(keep, a, torch.full_like(a, float('nan')) if b is None else b)
+
+
+def merge(old, new, mask, G):
+    """Records ``old`` updated with the (G,) entries of ``new`` from a level evaluated under ``mask``: an entry already in
+    ``old`` keeps its value for the videos outside ``mask``, whose last evaluation of the frame came earlier."""
+    out = dict(old)
+    for k, v in new.items():
+        out[k] = pick(mask, G, v, old[k]) if k in old else v
+    return out
 
 
 def _side_stream(device):
@@ -38,18 +95,17 @@ def _side_stream(device):
     return _SIDE[device.index]
 
 
-def _mark(ad, name):
-    """Diagnostics (scripts/phase_times.py): when ``ad.phase_events`` is a list, record a CUDA event on the caller's stream."""
-    ev_list = getattr(ad, 'phase_events', None)
-    if ev_list is not None:
+def _mark(s, name):
+    """Diagnostics (scripts/phase_times.py): when ``s.phase_events`` is a list, record a CUDA event on the caller's stream."""
+    if s.phase_events is not None:
         ev = torch.cuda.Event(enable_timing=True)
         ev.record()
-        ev_list.append((name, ev))
+        s.phase_events.append((name, ev))
 
 
-def _groups(arena):
-    """Videos of a weight arena: one for a flat arena, G for a (G, P) stack."""
-    return arena.shape[0] if arena.dim() == 2 else 1
+def _entry(mask, G):
+    """The ``active`` argument of a network pass over ``mask``: None (the ``_groups`` entry point) for every video."""
+    return None if mask == (1 << G) - 1 else mask
 
 
 def runs(mask, G, key=lambda g: 0):
@@ -64,15 +120,13 @@ def runs(mask, G, key=lambda g: 0):
     return out
 
 
-def _active_rows(ad, t):
-    """``t`` itself, or, for a (G, P) stack while only some videos take part, the views of its runs of active videos: element-wise
-    sweeps over them leave the idle videos' rows untouched, and with every video active they are one sweep as before."""
-    act = getattr(ad, 'active', None)
-    return [t] if act is None else [t[a:b] for a, b in runs(act, t.shape[0])]
+def _active_rows(t, mask, G):
+    """``t`` itself for every video, else views of the (G, P) stack ``t``'s runs of videos in ``mask`` (sweeps skip the others)."""
+    return [t] if mask == (1 << G) - 1 else [t[a:b] for a, b in runs(mask, G)]
 
 
 class _Pred:
-    """Everything one forward graph produces (kept for its backward)."""
+    """Everything one forward graph produces (kept for its backward); ``active``: the videos of its backward."""
     __slots__ = ('image', 'rot', 'shape', 'cam', 'tape', 'verts', 'joints', 'smpl_tape', 'p2d', 'B', 'masked', 'groups', 'active')
 
 
@@ -85,17 +139,17 @@ def _smpl_fwd(smpl, betas, rot):
     return verts, joints, tape
 
 
-def forward_graph(ad, arena, buffers, image, masks=None, active=None):
+def forward_graph(s, arena, buffers, image, mask, masks=None):
     p = _Pred()
-    p.image, p.B, p.masked, p.groups, p.active = image, image.shape[0], masks is not None, _groups(arena), active
-    p.rot, p.shape, p.cam, _, p.tape = hmr_mod.raw_forward(arena, buffers, image, masks, groups=p.groups, active=active)
-    p.verts, p.joints, p.smpl_tape = _smpl_fwd(ad.smpl_neutral, p.shape, p.rot)
+    p.image, p.B, p.masked, p.groups, p.active = image, image.shape[0], masks is not None, s.G, mask
+    p.rot, p.shape, p.cam, _, p.tape = hmr_mod.raw_forward(arena, buffers, image, masks, groups=s.G, active=_entry(mask, s.G))
+    p.verts, p.joints, p.smpl_tape = _smpl_fwd(s.smpl_neutral, p.shape, p.rot)
     p.p2d = torch.empty(p.B, 49, 2, dtype=torch.float32, device=image.device)
     _lib.call('dboa_project_fwd', ptr(p.cam), ptr(p.joints), ptr(p.p2d), p.B, 49, stream())
     return p
 
 
-def _loss_head(ad, p, w, kp=None, t_p2d=None, t_j3d=None, t_beta=None, t_R=None, gt_s3d=None, grads=None, nb=None):
+def _loss_head(s, p, w, kp=None, t_p2d=None, t_j3d=None, t_beta=None, t_R=None, gt_s3d=None, grads=None, nb=None):
     """Runs the (optional) pose prior and the multi-term head on the first ``nb`` samples of ``p``, each video's rows on their
     own (per-video means and gradient scaling); returns (terms (G, 9), dp2d, dj3d, dR, dbeta).  ``grads``: preallocated
     (possibly larger-batch) gradient buffers whose leading ``nb`` rows are written."""
@@ -109,7 +163,7 @@ def _loss_head(ad, p, w, kp=None, t_p2d=None, t_j3d=None, t_beta=None, t_R=None,
     prior_b = None
     if w[2] != 0.0:
         prior_b = torch.empty(B, dtype=torch.float32, device=dev)
-        g = ad.gmm_f
+        g = s.gmm_f
         _lib.call('dboa_pose_prior', ptr(p.rot), ptr(g.means), ptr(g.precisions), ptr(g.neg_log_weights), ptr(prior_b), ptr(dR),
                   float(w[2]) / (B // G), B, stream())                   # per-video mean: scale w / b
     a = _lib.LossArgsStruct()
@@ -125,7 +179,7 @@ def _loss_head(ad, p, w, kp=None, t_p2d=None, t_j3d=None, t_beta=None, t_R=None,
     for i in range(8):
         a.w[i] = float(w[i])
     a.dR_accumulate = 1 if prior_b is not None else 0
-    a.kp_first, a.kp_count = getattr(ad, 'kp_range', (25, 24))      # joints of the re-projection term (webcam client: (0, 25))
+    a.kp_first, a.kp_count = s.kp_range                             # joints of the re-projection term (webcam client: (0, 25))
     _lib.call('dboa_loss_multi', C.byref(a), stream())
     return terms, dp2d, dj3d, dR, dbeta
 
@@ -135,90 +189,79 @@ def _zero(t):
     _lib.call('dboa_fill_zero', ptr(t), t.numel() * t.element_size(), stream())
 
 
-def backward_graph(ad, arena, p, dp2d, dj3d, dR, dbeta, grad_arena, sync=None):
-    """d(loss)/d(p2d, joints, R, beta) -> accumulate d(loss)/d(weights) into ``grad_arena``.  ``sync``: the data-parallel
-    ``BucketedGradSync`` when this is the LAST graph accumulated into the outer gradient: its buckets are all-reduced on the
-    communication stream while the rest of this backward runs."""
+def backward_graph(s, arena, p, dp2d, dj3d, dR, dbeta, grad_arena, sync=None):
+    """d(loss)/d(p2d, joints, R, beta) -> accumulate d(loss)/d(weights) of the videos ``p.active`` into ``grad_arena``.
+    ``sync``: the data-parallel ``BucketedGradSync`` when this is the LAST graph accumulated into the outer gradient: its
+    buckets are all-reduced on the communication stream while the rest of this backward runs."""
     B, dev = p.B, p.rot.device
     dcam = torch.empty(B, 3, dtype=torch.float32, device=dev)
     _lib.call('dboa_project_bwd', ptr(p.cam), ptr(p.joints), ptr(dp2d), ptr(dj3d), ptr(dcam), B, 49, 1, 0, stream())
     scratch = torch.empty(_lib.load().dboa_smpl_scratch_floats(B), dtype=torch.float32, device=dev)
-    _lib.call('dboa_smpl_backward', ad.smpl_neutral._struct_ref(), ptr(p.rot), B, ptr(p.smpl_tape), ptr(dj3d), ptr(scratch), ptr(dR),
+    _lib.call('dboa_smpl_backward', s.smpl_neutral._struct_ref(), ptr(p.rot), B, ptr(p.smpl_tape), ptr(dj3d), ptr(scratch), ptr(dR),
               ptr(dbeta), 1, stream())
     if sync is not None:
         sync.arm()
-    hmr_mod.raw_backward(arena, p.tape, B, p.masked, dR, dbeta, dcam, grad_arena, groups=p.groups, active=p.active)
+    hmr_mod.raw_backward(arena, p.tape, B, p.masked, dR, dbeta, dcam, grad_arena, groups=p.groups, active=_entry(p.active, p.groups))
     if sync is not None:
         sync.after_backward(grad_arena)
-        ad.optimizer.reduced = True
 
 
-def retrieve(ad, rows, rngs, active=None):
-    """reference :82-96 for every video: the nearest cluster centre of video g's feature row ``rows[g]`` by cosine distance
-    (one host synchronisation for all videos), then ``rngs[g].sample`` inside that cluster.  Returns the (cluster, picks) of
-    every video and the picked exemplar rows, video after video.  ``active`` (bit mask, None: all): an idle video draws
-    nothing, gets None and placeholder rows (exemplar 0)."""
-    on = [active is None or bool((active >> g) & 1) for g in range(len(rows))]
+def retrieve(bank, rows, rngs, mask, best, n):
+    """reference :82-96 for every video in ``mask``: the nearest cluster centre of video g's feature row ``rows[g]`` by cosine
+    distance (into ``best[g]``; one host synchronisation for all videos), then ``rngs[g].sample`` of ``n`` exemplars inside
+    that cluster.  Returns the (cluster, picks) of every video and the picked exemplar rows, video after video; a video
+    outside ``mask`` draws nothing, gets None and placeholder rows (exemplar 0)."""
+    on = [bool((mask >> g) & 1) for g in range(len(rows))]
     for g, f in enumerate(rows):
-        if not on[g]:
-            continue
-        f = f.contiguous()
-        _lib.call('dboa_retrieval_nearest', ptr(f), ptr(ad.centers), ad.centers.shape[0], 2048, C.c_void_p(ad._best.data_ptr() + 4 * g),
-                  ptr(ad._dists), stream())
-    picked = [(c, rng.sample(ad.index[c], ad.options.sample_num)) if a else None for c, rng, a in zip(ad._best.tolist(), rngs, on)]
-    idx = torch.as_tensor([i for p in picked for i in (p[1] if p else [0] * ad.options.sample_num)], dtype=torch.long, device=rows.device)
-    return picked, {k: v.index_select(0, idx) for k, v in ad.h36m_bank.items()}
+        if on[g]:
+            _lib.call('dboa_retrieval_nearest', ptr(f.contiguous()), ptr(bank.centers), bank.centers.shape[0], 2048,
+                      C.c_void_p(best.data_ptr() + 4 * g), ptr(bank.dists), stream())
+    picked = [(c, rng.sample(bank.index[c], n)) if a else None for c, rng, a in zip(best.tolist(), rngs, on)]
+    idx = torch.as_tensor([i for p in picked for i in (p[1] if p else [0] * n)], dtype=torch.long, device=rows.device)
+    return picked, {k: v.index_select(0, idx) for k, v in bank.exemplars.items()}
 
 
-def level_backward(ad, arena, buffers, image, kp, lower, grad_arena, main=None, sync=None):
-    """One level of the bilevel problem (reference base_adaptor.py:222-317) on weights ``arena``, a flat arena or a (G, P)
-    stack of G videos' arenas: evaluates the level's loss of every video and accumulates its gradient into ``grad_arena``
-    (same layout; ``sync``: data-parallel bucketed all-reduce to attach to the last graph of the level).  ``main`` is an
-    already computed forward of ``image`` with these weights (re-used when given).  Returns (the loss, a device scalar for
-    a flat arena and (G,) for a stack; the forward whose first rows belong to ``image``).
+def level_backward(s, out, arena, image, kp, lower, grad_arena, mask, live, main=None, sync=None):
+    """One level of the bilevel problem (reference base_adaptor.py:222-317) for the videos in ``mask`` on weights ``arena``:
+    evaluates the level's loss of every video and accumulates its gradient into ``grad_arena`` (``sync``: data-parallel
+    bucketed all-reduce to attach to the last graph of the level).  ``live``: the videos whose motion term is live.
+    ``main`` is an already computed forward of ``image`` with these weights (re-used when given).  The level's records go to
+    the ``Frame`` ``out``, where a video of the frame outside ``mask`` keeps its earlier ones.  Returns (the (G,) loss, the
+    forward whose first rows belong to ``image``).
 
     With one video, when the motion loss is live and no forward is supplied, the current and the history frame go through
     ONE batched forward / backward (same weights, independent samples), and the teacher forward runs on a side stream.
     With several, the history frame gets its own grouped pass and the teacher runs on the caller's stream."""
-    o = ad.options
+    o, G = s.options, s.G
     tag = 'll' if lower else 'ul'
     nb = image.shape[0]
-    G = _groups(arena)
-    per_video = arena.shape[:-1]                                # shape of the losses recorded and returned: () or (G,)
     use_frame = o.use_frame_losses_lower if lower else o.use_frame_losses_upper
     use_temporal = o.use_temporal_losses_lower if lower else o.use_temporal_losses_upper
-    act = getattr(ad, 'active', None)                           # videos taking part (bit mask; None: all)
-    # videos whose motion term is live (bit mask): all of them or none, by the frame count, unless the adaptor keeps one per video
-    every = (1 << G) - 1
-    live = getattr(ad, 'motion_active', None)
-    if live is None:
-        live = every if (ad.global_step - o.interval) > 0 else 0
+    live &= mask
     motion = bool(use_temporal and o.use_motion and live)
-    live = None if live == every else live
+    fit = {}
     # the teacher forward is independent of the fast-weight forward: issue it on a side stream so that the two chains
     # of small, latency-bound kernels overlap on the GPU (each one alone leaves most SMs idle at batch 1)
     tpred, side = None, None
     if use_temporal and o.use_meanteacher:
-        teacher = ad.teacher
         if _TEACHER_OVERLAP and G == 1:
             side = _side_stream(image.device)
             side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):                           # None: the caller's stream
-            tpred = forward_graph(ad, teacher.arena, teacher._buffers, image, teacher._masks(nb, image.device), act)
+            tpred = forward_graph(s, s.teacher, s.teacher_buffers, image, mask, s.teacher_masks(nb, image.device, mask))
     if motion:
-        hist_image, hist_kp = ad.get_hist()
+        hist_image, hist_kp = s.get_hist(live)
         if main is None and G == 1:
-            pair = getattr(ad, '_pair', None)                   # persistent (2 nb, 3, 224, 224) staging: rows [nb:] = history frame
-            if pair is None or pair.shape[0] != 2 * nb or pair.device != image.device:
-                pair = ad._pair = torch.empty(2 * nb, 3, 224, 224, dtype=torch.float32, device=image.device)
-            half = image.numel() * 4
+            if s._pair is None or s._pair.shape[0] != 2 * nb or s._pair.device != image.device:    # rows [nb:] = history frame
+                s._pair = torch.empty(2 * nb, 3, 224, 224, dtype=torch.float32, device=image.device)
+            pair, half = s._pair, image.numel() * 4
             _lib.call('dboa_copy_async', ptr(pair), ptr(image), half, stream())
             _lib.call('dboa_copy_async', C.c_void_p(pair.data_ptr() + half), ptr(hist_image.contiguous()), half, stream())
-            main = forward_graph(ad, arena, buffers, pair)
+            main = forward_graph(s, arena, s.buffers, pair, mask)
     if main is None:
-        main = forward_graph(ad, arena, buffers, image, active=act)
+        main = forward_graph(s, arena, s.buffers, image, mask)
     batched = main.B > nb
-    hist = forward_graph(ad, arena, buffers, hist_image, active=live) if motion and not batched else None
+    hist = forward_graph(s, arena, s.buffers, hist_image, live) if motion and not batched else None
     w = [0.0] * 8
     targets = {}
     if use_frame:
@@ -233,102 +276,101 @@ def level_backward(ad, arena, buffers, image, kp, lower, grad_arena, main=None, 
         tw = o.teacherloss_weight
         w[3], w[4], w[5], w[6] = 5 * tw, 5 * tw, 0.001 * tw, 1 * tw
         targets = dict(t_p2d=t.p2d, t_j3d=t.joints, t_beta=t.shape, t_R=t.rot)
-    _mark(ad, f'{tag}: forward(s) issued')
+    _mark(s, f'{tag}: forward(s) issued')
     grads = None
     if batched:                                                 # gradients of the 2 nb rows in ONE zeroed buffer (rows [nb:] only get the motion term)
         Bm = main.B
         sizes = (Bm * 49 * 2, Bm * 49 * 3, Bm * 24 * 9, Bm * 10)
-        flat = getattr(ad, '_bgrad_flat', None)
-        if flat is None or flat.numel() != sum(sizes) or flat.device != image.device:
-            flat = ad._bgrad_flat = torch.empty(sum(sizes), dtype=torch.float32, device=image.device)
+        if s._bgrad_flat is None or s._bgrad_flat.numel() != sum(sizes) or s._bgrad_flat.device != image.device:
+            s._bgrad_flat = torch.empty(sum(sizes), dtype=torch.float32, device=image.device)
+        flat = s._bgrad_flat
         _zero(flat)
-        e = [0, sizes[0], sizes[0] + sizes[1], sizes[0] + sizes[1] + sizes[2]]
-        grads = (flat[e[0]:e[1]].view(Bm, 49, 2), flat[e[1]:e[2]].view(Bm, 49, 3), flat[e[2]:e[3]].view(Bm, 24, 3, 3), flat[e[3]:].view(Bm, 10))
-    terms, dp2d, dj3d, dR, dbeta = _loss_head(ad, main, w, kp=kp if use_frame else None, grads=grads, nb=nb, **targets)
-    terms = terms.view(*per_video, 9)
-    total = terms[..., 8]
+        grads = tuple(t.view(Bm, *sh) for t, sh in zip(flat.split(sizes), ((49, 2), (49, 3), (24, 3, 3), (10,))))
+    terms, dp2d, dj3d, dR, dbeta = _loss_head(s, main, w, kp=kp if use_frame else None, grads=grads, nb=nb, **targets)
+    total = terms[:, 8]
     if use_frame:
-        ad.fit_losses[f'{tag}/s2dloss'], ad.fit_losses[f'{tag}/shape_prior'], ad.fit_losses[f'{tag}/pose_prior'] = terms[..., 0], terms[..., 1], terms[..., 2]
-        (ad.kp2dlosses_lower.append(terms[..., 0]) if lower else ad.kp2dlosses_upper.__setitem__(ad.global_step, terms[..., 0]))
+        fit[f'{tag}/s2dloss'], fit[f'{tag}/shape_prior'], fit[f'{tag}/pose_prior'] = terms[:, 0], terms[:, 1], terms[:, 2]
+        if lower:
+            out.lower.append(terms[:, 0])
     if motion:
-        mterm = torch.empty(per_video, dtype=torch.float32, device=image.device)
+        mterm = torch.empty(G, dtype=torch.float32, device=image.device)
         p_hist = main.p2d[nb:] if batched else hist.p2d
         dph = dp2d[nb:] if batched else torch.empty_like(hist.p2d)
-        kf, kn = getattr(ad, 'kp_range', (25, 24))
+        kf, kn = s.kp_range
         margs = (ptr(main.p2d), ptr(p_hist), ptr(kp), ptr(hist_kp.contiguous()), float(o.motionloss_weight), ptr(mterm), ptr(dp2d), ptr(dph),
                  nb, 1, kf, kn, G)
-        if live is None:
+        if live == (1 << G) - 1:
             _lib.call('dboa_loss_motion_groups', *margs, stream())
         else:
             _lib.call('dboa_loss_motion_active', *margs, live, stream())
         if not batched:
-            backward_graph(ad, arena, hist, dph, torch.zeros_like(hist.joints), torch.zeros_like(hist.rot), torch.zeros_like(hist.shape),
+            backward_graph(s, arena, hist, dph, torch.zeros_like(hist.joints), torch.zeros_like(hist.rot), torch.zeros_like(hist.shape),
                            grad_arena)
         total = total + mterm * o.motionloss_weight
-        ad.fit_losses['ul/motion_loss'] = mterm
-    _mark(ad, f'{tag}: loss head')
+        fit['ul/motion_loss'] = mterm
+    _mark(s, f'{tag}: loss head')
     mix = bool(o.retrieval and (o.lower_level_mixtrain if lower else o.upper_level_mixtrain))
-    backward_graph(ad, arena, main, dp2d, dj3d, dR, dbeta, grad_arena, sync=None if mix else sync)
-    _mark(ad, f'{tag}: backward')
+    backward_graph(s, arena, main, dp2d, dj3d, dR, dbeta, grad_arena, sync=None if mix else sync)
+    _mark(s, f'{tag}: backward')
     if o.retrieval:
         rows = hmr_mod._feature_views(main.tape, main.B)[5][:nb].reshape(G, -1, 2048)[:, 0]      # each video's first sample
-        picked, ex = retrieve(ad, rows, getattr(ad, 'rngs', [random]), act)
-        if per_video:
-            ad.last_retrieval = [p if p is not None else q for p, q in zip(picked, ad.last_retrieval)]
-        else:
-            ad.last_retrieval = picked[0]
+        picked, ex = retrieve(s.bank, rows, s.rngs, mask, s._best, o.sample_num)
+        out.picks = [p if p is not None else q for p, q in zip(picked, out.picks or picked)]
         if mix:
-            e = forward_graph(ad, arena, buffers, ex['img'], active=act)
+            e = forward_graph(s, arena, s.buffers, ex['img'], mask)
             n = e.B
             gt_R = torch.empty(n, 24, 3, 3, dtype=torch.float32, device=image.device)
             _lib.call('dboa_rodrigues', ptr(ex['pose'].reshape(-1, 3).contiguous()), ptr(gt_R), n * 24, 0, stream())
             lw = o.labelloss_weight
-            eterms, a, b, c, d = _loss_head(ad, e, [5 * lw, 0, 0, 0, 0, 0.001 * lw, 1 * lw, 5 * lw], kp=ex['keypoints'], t_beta=ex['betas'],
+            eterms, a, b, c, d = _loss_head(s, e, [5 * lw, 0, 0, 0, 0, 0.001 * lw, 1 * lw, 5 * lw], kp=ex['keypoints'], t_beta=ex['betas'],
                                             t_R=gt_R, gt_s3d=ex['pose_3d'])
-            backward_graph(ad, arena, e, a, b, c, d, grad_arena, sync=sync)
-            eterms = eterms.view(*per_video, 9)
-            total = total + eterms[..., 8]
-            ad.fit_losses[f'{tag}/labled_loss'] = eterms[..., 8]
+            backward_graph(s, arena, e, a, b, c, d, grad_arena, sync=sync)
+            total = total + eterms[:, 8]
+            fit[f'{tag}/labled_loss'] = eterms[:, 8]
+    out.fit = merge(out.fit, fit, mask | ~out.mask & ((1 << G) - 1), G)
     return total, main
 
 
-def feature_cosines(ad, tape_a, tape_b, B):
-    fa, fb = hmr_mod._feature_views(tape_a, B), hmr_mod._feature_views(tape_b, B)
-    return ad.cal_feature_diff(fa, fb)
-
-
-def feature_test(ad, a, b, stacked, mask):
-    """The dynamic loop's feature test between the forwards ``a`` and ``b``: {video: {i: {'cos': c}}} of every video in ``mask``
-    (a bit mask).  One arena: ``cal_feature_diff`` (it all-reduces under data parallelism).  A (G, P) stack: one
-    ``dboa_cosine_terms_active`` call over the videos in ``mask`` and one copy to the host; each video's cosines and its
-    ``fit_losses['feat_sim/cos_sim']`` entry are formed from its own sums exactly as ``cal_feature_diff`` forms them."""
-    if not stacked:
-        return {0: feature_cosines(ad, a.tape, b.tape, a.B)}
-    from .base_adaptor import _dense_ptr_tensor
-    G, n = a.groups, 15
-    fa = [_dense_ptr_tensor(t) for t in hmr_mod._feature_views(a.tape, a.B)]      # xc (row stride HEAD_LD) is made dense
-    fb = [_dense_ptr_tensor(t) for t in hmr_mod._feature_views(b.tape, b.B)]
+def cosines(features_a, features_b, G, mask, partial, reduce_terms=None):
+    """The cosines between the feature pairs (``features_a[i]``, ``features_b[i]``) of every video in ``mask``, each video's
+    rows on their own: one ``dboa_cosine_terms_active`` call for the sums (a.b, |a|^2, |b|^2), summed over the data-parallel
+    ranks by ``reduce_terms`` when given, and one copy to the host.  Returns ((G, n) float32 host cosines, unspecified outside
+    ``mask``; the scratch ``partial`` (None: none yet) to pass next time)."""
+    def dense(t):                      # one dense block of numel floats (permuted views qualify; xc, of row stride HEAD_LD, does not)
+        t = t.detach()
+        return t if t.dtype == torch.float32 and 1 + sum((a - 1) * b for a, b in zip(t.shape, t.stride())) == t.numel() else t.float().contiguous()
+    n, fa, fb = len(features_a), [dense(t) for t in features_a], [dense(t) for t in features_b]
     pa = (C.c_void_p * n)(*[t.data_ptr() for t in fa])
     pb = (C.c_void_p * n)(*[t.data_ptr() for t in fb])
     ln = (C.c_longlong * n)(*[t.numel() for t in fa])
     need = _lib.load().dboa_cosine_partial_floats_groups(ln, n, G)
     _lib.check(0 if need > 0 else need, 'dboa_cosine_partial_floats_groups')
-    part = getattr(ad, '_cos_partial', None)
-    if part is None or part.numel() < need or part.device != a.rot.device:
-        part = ad._cos_partial = torch.empty(need, dtype=torch.float32, device=a.rot.device)
-    terms = torch.empty(G, n, 3, dtype=torch.float64, device=a.rot.device)
-    _lib.call('dboa_cosine_terms_active', pa, pb, ln, n, ptr(part), part.numel(), ptr(terms), stream(), G, mask)
-    host = terms.cpu()                                                # the one host sync of this test, for every video
-    prev = ad.fit_losses.get('feat_sim/cos_sim')
+    dev = fa[0].device
+    if partial is None or partial.numel() < need or partial.device != dev:
+        partial = torch.empty(need, dtype=torch.float32, device=dev)
+    terms = torch.empty(G, n, 3, dtype=torch.float64, device=dev)
+    _lib.call('dboa_cosine_terms_active', pa, pb, ln, n, ptr(partial), partial.numel(), ptr(terms), stream(), G, mask)
+    if reduce_terms is not None:
+        reduce_terms(terms)
+    t = terms.cpu()                                                   # the one host sync of the test, for every video
+    return (t[..., 0] / (t[..., 1].sqrt().clamp_min(1e-12) * t[..., 2].sqrt().clamp_min(1e-12))).float(), partial
+
+
+def feature_test(s, fit, a, b, mask):
+    """The dynamic loop's feature test between the forwards ``a`` and ``b``: {video: {i: {'cos': c}}} of the videos in ``mask``,
+    and their ``feat_sim/cos_sim`` in ``fit`` ((G,) host tensor; the others keep theirs, NaN at first), as ``cal_feature_diff``."""
+    G = s.G
+    cos, s._cos_partial = cosines(hmr_mod._feature_views(a.tape, a.B), hmr_mod._feature_views(b.tape, b.B), G, mask, s._cos_partial,
+                                  s.reduce_terms)
+    n = cos.shape[1]
+    prev = fit.get('feat_sim/cos_sim')
     rec = torch.full((G,), float('nan')) if prev is None else prev.clone()
     out = {}
     for g in range(G):
         if (mask >> g) & 1:
-            t = host[g]
-            cos = (t[:, 0] / (t[:, 1].sqrt().clamp_min(1e-12) * t[:, 2].sqrt().clamp_min(1e-12))).float()
-            rec[g] = cos.sum() / (n - 1)
-            out[g] = {i: {'cos': float(cos[i])} for i in range(n)}
-    ad.fit_losses['feat_sim/cos_sim'] = rec
+            rec[g] = cos[g].sum() / (n - 1)                           # reference :218 divides by the last index
+            out[g] = {i: {'cos': float(cos[g, i])} for i in range(n)}
+    fit['feat_sim/cos_sim'] = rec
     return out
 
 
@@ -344,110 +386,73 @@ def _continuing(o, sims, steps):
     return mask
 
 
-def _keep_records(ad, old, mask, G):
-    """After a level evaluated under ``mask``: every ``fit_losses`` / ``kp2dlosses_upper`` entry of ``old`` (the records before
-    that level) keeps its value for the videos outside ``mask``, whose last evaluation of the frame came earlier."""
-    keep = torch.tensor([bool((mask >> g) & 1) for g in range(G)])
-    for rec, prev in zip((ad.fit_losses, ad.kp2dlosses_upper), old):
-        for k, v in prev.items():
-            if rec[k] is not v:
-                rec[k] = torch.where(keep.to(v.device), rec[k], v)
-
-
-def fused_adapt(ad, batch):
-    """One adapted frame (reference dynaboa_benchmark.py:126-201) of every video of ``ad``: probe forward, ``inner_step`` SGD
-    steps of the lower level, the upper level, one Adam + EMA teacher sweep, then the optional ``dynamic_boa`` loop.
-
-    Reads from ``ad``: ``model`` (``arena``, ``_buffers``, ``grad_arena()``), ``teacher`` (``arena``, ``_buffers``,
-    ``_masks(B, device)``) and ``optimizer`` (``step(teacher=, alpha=)``, ``grad_sync``), whose arenas are flat for one video
-    and (G, P) stacks for G videos; ``save_hist`` / ``get_hist``; ``global_step``; the records the level writes."""
-    o = ad.options
+def fused_adapt(s, batch, mask, frames):
+    """One adapted frame (reference dynaboa_benchmark.py:126-201) of the videos in ``mask``: probe forward, ``inner_step``
+    SGD steps of the lower level, the upper level, one Adam + EMA teacher sweep, then the optional ``dynamic_boa`` loop.
+    ``frames[g]``: the frames video g adapted before this one (its motion term's clock).  Returns the ``Frame``."""
+    o, G, theta, buffers, grad = s.options, s.G, s.theta, s.buffers, s.grad
+    out = Frame(mask)
     image, kp = batch['image'].contiguous().float(), batch['smpl_j2d'].contiguous().float()
-    ad.save_hist(image, kp)
-    model = getattr(ad.model, 'module', ad.model)
-    theta, buffers = model.arena, model._buffers
-    opt = ad.optimizer
-    grad = model.grad_arena()
-    teacher = ad.teacher if o.use_meanteacher else None
-    evaluate = getattr(ad, 'fused_eval', 'final')
+    s.save_hist(image, kp, mask)
+    live = sum(1 << g for g in range(G) if (mask >> g) & 1 and frames[g] + s.motion_lead - o.interval > 0)
+    evaluate, sync = s.eval_mode, s.grad_sync
     with torch.no_grad():
-        _mark(ad, 'start')
-        probe = forward_graph(ad, theta, buffers, image, active=getattr(ad, 'active', None))       # init_features (reference :132-133)
-        _mark(ad, 'probe forward')
-        import torch.distributed as tdist
-        sync = opt.grad_sync if (opt.grad_sync is not None and tdist.is_initialized() and tdist.get_world_size() > 1) else None
+        _mark(s, 'start')
+        probe = forward_graph(s, theta, buffers, image, mask)             # init_features (reference :132-133)
+        _mark(s, 'probe forward')
         if not o.use_boa:
             _zero(grad)
-            ad.last_upper_loss, _ = level_backward(ad, theta, buffers, image, kp, True, grad, main=probe, sync=sync)
-            opt.step()
-            return ad.inference(batch, ad.model) if evaluate != 'none' else None
+            out.upper_loss, _ = level_backward(s, out, theta, image, kp, True, grad, mask, live, main=probe, sync=sync)
+            s.adam(mask)
+            if evaluate != 'none':
+                out.result = s.evaluate(batch, theta, mask, None)
+            return out
         fast, cur = theta, probe
-        if not hasattr(ad, '_fast_bufs'):
-            ad._fast_bufs = [torch.empty_like(theta), torch.empty_like(theta)]
-            ad._inner_grad = torch.empty_like(theta)
+        if s._fast is None:
+            s._fast, s._inner_grad = [torch.empty_like(theta), torch.empty_like(theta)], torch.empty_like(theta)
         for i in range(o.inner_step):
-            for t in _active_rows(ad, ad._inner_grad):
+            for t in _active_rows(s._inner_grad, mask, G):
                 _zero(t)
-            level_backward(ad, fast, buffers, image, kp, True, ad._inner_grad, main=cur if i == 0 else None)
-            _mark(ad, 'lower level (loss + backward)')
-            nxt = ad._fast_bufs[i % 2]
-            for f, g, n in zip(_active_rows(ad, fast), _active_rows(ad, ad._inner_grad), _active_rows(ad, nxt)):
+            level_backward(s, out, fast, image, kp, True, s._inner_grad, mask, live, main=cur if i == 0 else None)
+            _mark(s, 'lower level (loss + backward)')
+            nxt = s._fast[i % 2]
+            for f, g, n in zip(_active_rows(fast, mask, G), _active_rows(s._inner_grad, mask, G), _active_rows(nxt, mask, G)):
                 _lib.call('dboa_sgd_update', ptr(f), ptr(g), ptr(n), float(o.fastlr), f.numel(), stream())
             fast = nxt
-            _mark(ad, 'inner SGD step')
+            _mark(s, 'inner SGD step')
             if evaluate == 'all':
-                ad.inference(batch, _ArenaModel(model, fast))
-        for t in _active_rows(ad, grad):
+                s.evaluate(batch, fast, mask, i)
+        for t in _active_rows(grad, mask, G):
             _zero(t)
-        ad.last_upper_loss, _ = level_backward(ad, fast, buffers, image, kp, False, grad, sync=sync)
-        _mark(ad, 'upper level (forward + loss + backward)')
-        opt.step(teacher=teacher, alpha=o.alpha)                    # Adam + EMA teacher, one sweep
-        _mark(ad, 'Adam + EMA')
-        result = None
+        out.upper_loss, _ = level_backward(s, out, fast, image, kp, False, grad, mask, live, sync=sync)
+        _mark(s, 'upper level (forward + loss + backward)')
+        s.adam(mask, s.teacher, o.alpha)                                  # Adam + EMA teacher, one sweep
+        _mark(s, 'Adam + EMA')
         if evaluate == 'all' or (evaluate == 'final' and not o.dynamic_boa):
-            result = ad.inference(batch, ad.model)
+            out.result = s.evaluate(batch, theta, mask, None)
         if o.dynamic_boa:
             # every video runs the reference's loop (:161-192) on its own: the videos still in it (bit mask `loop`) make one
-            # grouped pass per iteration, and the decisions of all of them share one host sync.  One arena: one bit.
-            stacked, G = theta.dim() == 2, _groups(theta)
-            every = (1 << G) - 1
-            frame = getattr(ad, 'active', None)
-            frame_bits = every if frame is None else frame
-            after = forward_graph(ad, theta, buffers, image, active=frame)
-            sims = feature_test(ad, probe, after, stacked, frame_bits)
-            trace, steps = {g: [s] for g, s in sims.items()}, dict.fromkeys(sims, 0)
-            if not stacked:
-                ad.feat_sims[ad.global_step] = trace[0]
-            loop = _continuing(o, sims, steps)
+            # grouped pass per iteration, and the decisions of all of them share one host sync
+            after = forward_graph(s, theta, buffers, image, mask)
+            sims = feature_test(s, out.fit, probe, after, mask)
+            out.sims, out.steps = {g: [x] for g, x in sims.items()}, dict.fromkeys(sims, 0)
+            loop = _continuing(o, sims, out.steps)
             while loop:
-                act = None if loop == every else loop
-                if stacked:
-                    ad.active = act                         # the level, its draws, Adam and the motion mask follow the loop
-                old = (dict(ad.fit_losses), dict(ad.kp2dlosses_upper)) if loop != frame_bits else None
-                for t in _active_rows(ad, grad):
+                for t in _active_rows(grad, loop, G):
                     _zero(t)
-                after.active = act                          # its backward runs under the loop, not under its forward's wider mask
-                level_backward(ad, theta, buffers, image, kp, False, grad, main=after, sync=sync)   # 'after' was computed with the current theta
-                if old is not None:
-                    _keep_records(ad, old, loop, G)
-                opt.step(teacher=teacher, alpha=o.alpha)
-                before, after = after, forward_graph(ad, theta, buffers, image, active=act)
-                sims = feature_test(ad, before, after, stacked, loop)
-                for g, s in sims.items():
-                    trace[g].append(s)
+                after.active = loop                         # its backward runs under the loop, not under its forward's wider mask
+                level_backward(s, out, theta, image, kp, False, grad, loop, live, main=after, sync=sync)   # 'after' was computed with the current theta
+                s.adam(loop, s.teacher, o.alpha)
+                before, after = after, forward_graph(s, theta, buffers, image, loop)
+                sims = feature_test(s, out.fit, before, after, loop)
+                for g, x in sims.items():
+                    out.sims[g].append(x)
                 if evaluate == 'all':
-                    result = ad.inference(batch, ad.model)
-                loop = _continuing(o, sims, steps)
-            if stacked:
-                ad.active = frame
-                ad.optimized_step = [steps.get(g) for g in range(G)]
-                ad.loop_feat_sims = [trace.get(g) for g in range(G)]
-            else:
-                ad.optimized_step = steps[0]
-                ad.optim_step_record.append(steps[0])
+                    out.result = s.evaluate(batch, theta, loop, None)
+                loop = _continuing(o, sims, out.steps)
             if evaluate == 'final':
-                result = ad.inference(batch, ad.model)
-        return result
+                out.result = s.evaluate(batch, theta, mask, None)
+        return out
 
 
 class _ArenaModel:

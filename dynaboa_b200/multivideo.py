@@ -1,6 +1,6 @@
 """Several independent videos adapted in lockstep on one GPU: ``fused.fused_adapt`` over (G, P) stacks of weight arenas, with
 every network forward and backward one grouped call (``dboa_hmr_forward_groups`` / ``dboa_hmr_backward_groups``).  This module
-holds only the per-video state.
+holds the per-video state, hands the step a ``fused.Step`` over it and files the records the step returns per slot.
 
 Each video keeps the reference's semantics: its own theta, Adam moments and step count, teacher, fast weights, gradient,
 history ring, motion warm-up, teacher dropout masks and retrieval picks.  The G weight arenas (and the teachers', the moments',
@@ -12,14 +12,13 @@ G slots are a pool: a slot whose batch is None sits the frame out (its CTAs retu
 import ctypes as C
 import os
 import random
-from types import SimpleNamespace
 
 import numpy as np
 import torch
 
 from . import _lib, hmr as hmr_mod
 from ._lib import ptr, stream
-from .fused import fused_adapt, runs
+from .fused import Step, _entry, fused_adapt, pick, runs
 
 EVAL_MODES = ('none', 'final', 'all')
 GT_KEYS = ('pose', 'betas', 'gender')
@@ -45,6 +44,14 @@ def check_options(options, n_videos, dynamic_loop=False):
         rows = max(rows, int(options.sample_num))
     if G * rows > 64:
         raise ValueError(f'{G} videos x {rows} rows per grouped call exceed the 64 samples of the network tape')
+
+
+def slot_records(frame, G, prev_upper_loss):
+    """A pool's (``fit_losses``, ``kp2dlosses_lower``, ``last_upper_loss``) of the ``fused.Frame`` ``frame``: NaN for the slots
+    outside the frame, except in ``last_upper_loss``, where they keep ``prev_upper_loss``."""
+    on = frame.mask
+    return ({k: pick(on, G, v) for k, v in frame.fit.items()}, [pick(on, G, v) for v in frame.lower],
+            pick(on, G, frame.upper_loss, prev_upper_loss))
 
 
 class MultiVideoAdaptor:
@@ -74,6 +81,7 @@ class MultiVideoAdaptor:
     and reads its frame ``video_steps[g] + motion_lead - interval``; ``feat_sims[g]`` and the upper-level 2D losses are keyed by
     ``video_steps[g] + motion_lead``.  The webcam client advances its step before the levels (1: webcam.MultiWebcamAdaptor)."""
 
+    kp_range = (25, 24)
     motion_lead = 0
 
     def __init__(self, options, n_videos, dynamic_loop=False):
@@ -82,19 +90,11 @@ class MultiVideoAdaptor:
         self.G = G = int(n_videos)
         self.options = o = options
         self.base = base = self._make_base(options)    # checkpoint, SMPL, prior, exemplar bank; never adapted, so it keeps the checkpoint
-        self.smpl_neutral, self.gmm_f = base.smpl_neutral, base.gmm_f
-        if o.retrieval:
-            self.centers, self.index, self.h36m_bank, self._dists = base.centers, base.index, base.h36m_bank, base._dists
-            self._best = torch.zeros(G, dtype=torch.int32, device=base.device)
         model = base.model.module
         self.thetas = torch.empty(G, model.arena.numel(), device=model.arena.device)
         self.buffers = model._buffers
         self.teachers = torch.empty_like(self.thetas) if o.use_meanteacher else None
         self.m, self.v, self.grad = torch.empty_like(self.thetas), torch.empty_like(self.thetas), torch.zeros_like(self.thetas)
-        # what fused_adapt reads from a single-video adaptor's model, teacher and optimizer, over the (G, P) stacks
-        self.model = SimpleNamespace(arena=self.thetas, _buffers=self.buffers, grad_arena=lambda: self.grad)
-        self.teacher = SimpleNamespace(arena=self.teachers, _buffers=self.buffers, _masks=self._teacher_masks)
-        self.optimizer = SimpleNamespace(step=self._adam_ema, grad_sync=None)
         self.fused_eval = 'none'
         self.global_step = 0
         self.mask_provider = None
@@ -103,8 +103,6 @@ class MultiVideoAdaptor:
         self.teacher_dropout = bool(getattr(o, 'teacher_dropout', 1))
         self.step_counts, self.video_steps, self.histories, self.rngs = [0] * G, [0] * G, [{} for _ in range(G)], [None] * G
         self.optim_step_record, self.feat_sims, self.optimized_step = [[] for _ in range(G)], [{} for _ in range(G)], [None] * G
-        self._on = (1 << G) - 1            # slots taking part now (bit mask): the frame's, narrowed by the dynamic loop
-        self._live = 0                     # slots of the current frame whose motion term is live (bit mask)
         self._frames = self._hist = None   # persistent staging of the current frame's and the history frame's rows
         self._pending = []                 # device records of the frames adapted since the records were last formed
         self._gt = None                    # the current frame's ground-truth meshes (gender-selected, neutral)
@@ -113,6 +111,10 @@ class MultiVideoAdaptor:
         self.mpjpe_all_lower, self.pampjpe_all_lower = [None] * G, [None] * G
         self.mpjpe_statistics, self.pampjpe_statistics = [{} for _ in range(G)], [{} for _ in range(G)]
         self.kp2dloss_lower_all, self.kp2dloss_upper_all = [[] for _ in range(G)], [{} for _ in range(G)]
+        self._step = Step(o, G, self.thetas, self.grad, self.buffers, base.smpl_neutral, base.gmm_f, teacher=self.teachers,
+                          teacher_buffers=self.buffers, teacher_masks=self._teacher_masks, kp_range=self.kp_range,
+                          motion_lead=self.motion_lead, bank=base.bank if o.retrieval else None, rngs=self.rngs,
+                          save_hist=self._save_hist, get_hist=self._get_hist, adam=self._adam_ema, evaluate=self._evaluate)
         for g in range(G):
             self.start(g)
 
@@ -125,15 +127,9 @@ class MultiVideoAdaptor:
         """Put a new video into slot g: theta and teacher from the checkpoint, zero Adam moments, step and frame counts, an empty
         history, empty records, and ``rngs[g] = random.Random(seed)`` (default ``options.seed * 1000 + g``).  The records of
         the frames adapted so far are formed on the host first (one synchronisation, if any are pending)."""
-        if not isinstance(g, int) or not 0 <= g < self.G:
-            raise ValueError(f'slot {g!r} is not one of the {self.G} slots')
+        self._reset_weights(g)
         self._form_records()
-        self.thetas[g].copy_(self.base.model.module.arena.detach())
-        if self.teachers is not None:
-            self.teachers[g].copy_(self.base.teacher.arena.detach())
-        self.m[g].zero_()
-        self.v[g].zero_()
-        self.step_counts[g] = self.video_steps[g] = 0
+        self.video_steps[g] = 0
         self.histories[g].clear()
         self.rngs[g] = random.Random(self.options.seed * 1000 + g if seed is None else seed)
         self.optim_step_record[g], self.feat_sims[g], self.optimized_step[g] = [], {}, None
@@ -143,23 +139,20 @@ class MultiVideoAdaptor:
         self.mpjpe_statistics[g], self.pampjpe_statistics[g] = {}, {}
         self.kp2dloss_lower_all[g], self.kp2dloss_upper_all[g] = [], {}
 
+    def _reset_weights(self, g):
+        """Slot g's theta and teacher back to the checkpoint and a fresh Adam (zero moments, step count 0)."""
+        if not isinstance(g, int) or not 0 <= g < self.G:
+            raise ValueError(f'slot {g!r} is not one of the {self.G} slots')
+        self.thetas[g].copy_(self.base.model.module.arena.detach())
+        if self.teachers is not None:
+            self.teachers[g].copy_(self.base.teacher.arena.detach())
+        self.m[g].zero_()
+        self.v[g].zero_()
+        self.step_counts[g] = 0
+
     def theta(self, g):
         """View of video g's weights (flat arena layout)."""
         return self.thetas[g]
-
-    @property
-    def active(self):
-        """What fused_adapt reads and narrows: None while every slot takes part, else the bit mask of the slots taking part."""
-        return None if self._on == (1 << self.G) - 1 else self._on
-
-    @active.setter
-    def active(self, mask):
-        self._on = (1 << self.G) - 1 if mask is None else mask
-
-    @property
-    def motion_active(self):
-        """Slots taking part now whose motion term is live (bit mask)."""
-        return self._on & self._live
 
     def _check_runtime(self):
         opt = self.base.optimizer
@@ -171,18 +164,18 @@ class MultiVideoAdaptor:
     def _slots(self, mask):
         return [g for g in range(self.G) if (mask >> g) & 1]
 
-    def save_hist(self, image, s2d):
-        """One copy of the frame's staged rows, kept by every active slot under its own frame count."""
+    def _save_hist(self, image, s2d, on):
+        """One copy of the frame's staged rows, kept by every slot in ``on`` under its own frame count."""
         frame = (image.clone(), s2d.clone())
-        for g in self._slots(self._on):
+        for g in self._slots(on):
             h, k = self.histories[g], self.video_steps[g]
             h[k] = frame
             h.pop(k - self.options.interval - 1, None)
 
-    def get_hist(self):
-        """The history rows of the slots whose motion term is live, each from its own frame ``interval - motion_lead`` frames
-        back; the rows of the other slots are placeholders."""
-        live = self._slots(self.motion_active)
+    def _get_hist(self, live):
+        """The history rows of the slots in ``live``, each from its own frame ``interval - motion_lead`` frames back; the rows
+        of the other slots are placeholders."""
+        live = self._slots(live)
         frames = [self.histories[g][self.video_steps[g] + self.motion_lead - self.options.interval] for g in live]
         if len(live) == self.G and all(f is frames[0] for f in frames):
             return frames[0]                                     # one pool frame holds every slot's history rows
@@ -194,28 +187,27 @@ class MultiVideoAdaptor:
                 _lib.call('dboa_copy_async', C.c_void_p(dst.data_ptr() + g * n), C.c_void_p(src.data_ptr() + g * n), n, stream())
         return self._hist
 
-    def _teacher_masks(self, B, device):
+    def _teacher_masks(self, B, device, on):
         if not self.teacher_dropout:
             return None
         b, per = B // self.G, []
         for g in range(self.G):
-            if not (self._on >> g) & 1:
+            if not (on >> g) & 1:
                 per.append(torch.ones(3, 2, b, 1024, device=device))       # placeholder rows: no draw for an idle slot
                 continue
             m = self.mask_provider(g, b, device) if self.mask_provider is not None else None
             per.append(m if m is not None else (torch.rand(3, 2, b, 1024, device=device) >= 0.5).float() * 2.0)
         return torch.cat(per, 2)
 
-    def _adam_ema(self, teacher=None, alpha=0.0):
-        """Adam + EMA teacher of the active slots, each at its own step count: one sweep per run of consecutive active slots
-        that share a step count (one sweep over the whole stack while every slot runs in step)."""
+    def _adam_ema(self, on, teacher=None, alpha=0.0):
+        """Adam + EMA into the teacher stack ``teacher`` of the slots in ``on``, each at its own step count: one sweep per run of
+        consecutive slots that share a step count (one sweep over the whole stack while every slot runs in step)."""
         o = self.options
-        for g in self._slots(self._on):
+        for g in self._slots(on):
             self.step_counts[g] += 1
-        t = None if teacher is None else teacher.arena
-        for a, b in runs(self._on, self.G, key=lambda g: self.step_counts[g]):
+        for a, b in runs(on, self.G, key=lambda g: self.step_counts[g]):
             _lib.call('dboa_adam_ema_scaled', ptr(self.thetas[a:b]), ptr(self.grad[a:b]), ptr(self.m[a:b]), ptr(self.v[a:b]),
-                      ptr(None if t is None else t[a:b]), self.thetas[a:b].numel(), float(o.lr), float(o.beta1), float(o.beta2), 1e-8,
+                      ptr(None if teacher is None else teacher[a:b]), self.thetas[a:b].numel(), float(o.lr), float(o.beta1), float(o.beta2), 1e-8,
                       self.step_counts[a], float(alpha), 1.0, stream())
 
     def _stage(self, batches):
@@ -268,25 +260,20 @@ class MultiVideoAdaptor:
     def _adapt_staged(self, on, batch):
         """The frame of ``adapt`` on rows already staged in ``batch`` (the persistent staging), for the slots in ``on`` (bit
         mask): a subclass that writes the staged rows itself runs the same step through here."""
-        o = self.options
-        self._on = on
-        self._live = sum(1 << g for g in self._slots(on) if self.video_steps[g] + self.motion_lead - o.interval > 0)
-        prev = self.last_upper_loss
-        self.fit_losses, self.kp2dlosses_lower, self.kp2dlosses_upper = {}, [], {}
-        self._evals, self._gt, self._lower_evals = [], None, 0
-        fused_adapt(self, batch)
+        o, G = self.options, self.G
+        self._evals, self._gt = [], None
+        self._step.eval_mode = self.fused_eval
+        f = fused_adapt(self._step, batch, on, self.video_steps)
         self._gt = None
-        if self.active is not None:
-            keep = torch.tensor([bool((on >> g) & 1) for g in range(self.G)], device=prev.device)
-            nan = lambda t: torch.where(keep.to(t.device), t, torch.full_like(t, float('nan')))
-            self.last_upper_loss = torch.where(keep, self.last_upper_loss, prev)
-            self.fit_losses = {k: nan(v) for k, v in self.fit_losses.items()}
-            self.kp2dlosses_lower = [nan(v) for v in self.kp2dlosses_lower]
-            self.kp2dlosses_upper = {k: nan(v) for k, v in self.kp2dlosses_upper.items()}
+        self.fit_losses, self.kp2dlosses_lower, self.last_upper_loss = slot_records(f, G, self.last_upper_loss)
+        self.kp2dlosses_upper = {self.global_step: self.fit_losses['ul/s2dloss']} if 'ul/s2dloss' in self.fit_losses else {}
+        if f.picks is not None:
+            self.last_retrieval = [p if p is not None else q for p, q in zip(f.picks, self.last_retrieval)]
         if o.dynamic_boa:
+            self.optimized_step = [f.steps.get(g) for g in range(G)]
             for g in self._slots(on):
-                self.optim_step_record[g].append(self.optimized_step[g])
-                self.feat_sims[g][self.video_steps[g] + self.motion_lead] = self.loop_feat_sims[g]
+                self.optim_step_record[g].append(f.steps[g])
+                self.feat_sims[g][self.video_steps[g] + self.motion_lead] = f.sims[g]
         self._pending.append((on, {g: self.video_steps[g] for g in self._slots(on)}, self.fused_eval == 'all', self._evals,
                               list(self.kp2dlosses_lower), self.kp2dlosses_upper.get(self.global_step)))
         if len(self._pending) >= PENDING_FRAMES:
@@ -295,26 +282,16 @@ class MultiVideoAdaptor:
             self.video_steps[g] += 1
         self.global_step += 1
 
-    def inference(self, batch, model, need_feature=False):
-        """One evaluation of the stack ``model.arena`` (theta, or the fast weights of the next inner step) on the staged frame,
-        for the slots taking part now: one grouped forward, the neutral SMPL decode and ``dboa_eval_metrics_active``.  The
-        ground-truth meshes are computed at the frame's first evaluation and reused.  The (G b, 3) result stays on the device
-        until the records are formed; returns None."""
-        lower = model.arena is not self.thetas
+    def _evaluate(self, batch, arena, on, inner):
+        """One evaluation of ``arena`` (theta, or the fast weights of inner step ``inner``) for the slots in ``on``: a grouped
+        forward, SMPL decode and ``dboa_eval_metrics_active`` (ground truth from the frame's first), kept on the device."""
         with torch.no_grad():
-            rot, shape, _, _, _ = hmr_mod.raw_forward(model.arena, self.buffers, batch['image'], groups=self.G, active=self.active)
+            rot, shape, _, _, _ = hmr_mod.raw_forward(arena, self.buffers, batch['image'], groups=self.G, active=_entry(on, self.G))
             pred = self.base.decode_smpl_params(rot, shape)['vts']
             if self._gt is None:                             # as Adaptor.inference, for every staged row
-                pose, betas, gender, b = batch['pose'], batch['betas'], batch['gender'], self.base
-                gt = b.smpl_male(global_orient=pose[:, :3], body_pose=pose[:, 3:], betas=betas).vertices
-                gt_f = b.smpl_female(global_orient=pose[:, :3], body_pose=pose[:, 3:], betas=betas).vertices
-                gt = torch.where((gender == 1).view(-1, 1, 1), gt_f, gt)
-                gt_n = self.smpl_neutral(betas=betas, body_pose=pose[:, 3:], global_orient=pose[:, :3], pose2rot=True).vertices
-                self._gt = (gt, gt_n)
-            out = self.base.eval_metrics(pred, *self._gt, groups=self.G, active=self._on)
-        self._evals.append((out, self._on, self._lower_evals if lower else None))
-        if lower:
-            self._lower_evals += 1
+                self._gt = self.base._gt_meshes(batch)
+            out = self.base.eval_metrics(pred, *self._gt, groups=self.G, active=on)
+        self._evals.append((out, on, inner))
 
     def _form_records(self):
         """File the device records of every frame adapted since the last call into the slots' host records: one copy to the

@@ -48,6 +48,7 @@ def webcam_options(o):
 
 class WebcamAdaptor(Adaptor):
     kp_range = (0, 25)
+    motion_lead = 1                                         # save_hist advances global_step before the levels
 
     def __init__(self, options):
         super().__init__(webcam_options(options))
@@ -78,19 +79,14 @@ class WebcamAdaptor(Adaptor):
         """reference :197-218.  ``image``: (H, W, 3) RGB uint8 / float32 frame (numpy or CUDA tensor); ``gtkp2d``: (25, 3) OpenPose
         detections (x, y, confidence) in frame pixels.  Returns the (1, 3, 224, 224) network input, the (1, 49, 3) keypoint
         block (rows 0..24 filled) and the (1, 3) bounding box."""
-        kp = np.array(gtkp2d, dtype=np.float64, copy=True)
-        x0, y0, x1, y1 = kp[:, 0].min(), kp[:, 1].min(), kp[:, 0].max(), kp[:, 1].max()
-        center = [(x1 + x0) / 2, (y1 + y0) / 2]
-        scale = scaleFactor * max(x1 - x0, y1 - y0) / 200
-        bbox = np.stack([center[0], center[1], scale * 200])
-        kp[:, 2] = kp[:, 2] > 0.3
+        center, scale, bbox, kp = _box(gtkp2d, scaleFactor)
         img = image if torch.is_tensor(image) else torch.from_numpy(np.ascontiguousarray(image))
         img = img.to(self.device, non_blocking=True)
         net_in = dataprocess.crop(img, center, scale)
         kp25 = dataprocess.j2d_processing(torch.from_numpy(kp).float().to(self.device), center, scale)
         kp49 = torch.zeros(1, 49, 3, dtype=torch.float32, device=self.device)
         kp49[0, :25] = kp25
-        return net_in.unsqueeze(0), kp49, bbox[None, :]
+        return net_in.unsqueeze(0), kp49, bbox
 
     def online_adaptation(self, ori_image, gtkp2d):
         """reference :221-337: one adaptation step on the frame, then the adapted model's mesh."""
@@ -160,14 +156,7 @@ class MultiWebcamAdaptor(MultiVideoAdaptor):
         """Key ``r`` of the demo for stream g (reference dynaboa_webcam.py:184-194): theta and teacher back to the checkpoint and
         a fresh Adam (zero moments, step count 0).  The stream's history and frame count are kept, so its motion term stays as
         it was; the other streams are left alone."""
-        if not isinstance(g, int) or not 0 <= g < self.G:
-            raise ValueError(f'slot {g!r} is not one of the {self.G} slots')
-        self.thetas[g].copy_(self.base.model.module.arena.detach())
-        if self.teachers is not None:
-            self.teachers[g].copy_(self.base.teacher.arena.detach())
-        self.m[g].zero_()
-        self.v[g].zero_()
-        self.step_counts[g] = 0
+        self._reset_weights(g)
 
     def online_adaptation(self, frames, detections):
         """One tick of every stream (reference :221-337 per stream).  ``frames[g]``: an (H, W, 3) RGB uint8 / float32 frame (numpy

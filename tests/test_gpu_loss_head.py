@@ -546,7 +546,7 @@ def live_rows(live, G, b):
 def test_level_one_video_motion_pair(env, nb, monkeypatch):
     """One video: frame + teacher head on rows [:nb] of a 2 nb-row prediction whose rows [nb:] are the history frame, the
     motion term between them, one backward_graph over all 2 nb rows.  This restates fused.level_backward's batched
-    sequence call by call; test_level_backward runs level_backward itself."""
+    sequence call by call; test_level_backward_step runs level_backward itself."""
     from dynaboa_b200 import fused
     gen = torch.Generator().manual_seed(800 + nb)
     B2, wm = 2 * nb, 0.8
@@ -573,7 +573,7 @@ def test_level_one_video_motion_pair(env, nb, monkeypatch):
 def test_level_grouped_partial_live(env, monkeypatch):
     """Eight videos of two rows: frame + teacher head, the motion term of the live videos only against a separate history
     forward (dboa_loss_motion_active), the history backward and the main backward.  This restates fused.level_backward's
-    grouped sequence call by call; test_level_backward runs level_backward itself."""
+    grouped sequence call by call; test_level_backward_step runs level_backward itself."""
     from dynaboa_b200 import fused
     G, b, wm, live = 8, 2, 0.8, 0b01101001
     nb = G * b
@@ -600,16 +600,6 @@ def test_level_grouped_partial_live(env, monkeypatch):
                                                  [(got[1], refs[0], None, G), (got[0], refs[1], rows, n_live)]))
 
 
-class _Teacher:
-    """The mean teacher as fused.level_backward reads it: weights and buffers (used only as keys here), no dropout."""
-
-    def __init__(self, arena):
-        self.arena, self._buffers = arena, None
-
-    def _masks(self, B, device):
-        return None
-
-
 def fake_network(monkeypatch, outputs):
     """Replaces the network forward: ``outputs[arena.data_ptr()][key]`` is the (rot, shape, cam) of the image row whose
     pixel [0, 0, 0] holds ``key``, so a row keeps its outputs wherever level_backward stages it (the motion pair included)."""
@@ -624,9 +614,9 @@ def fake_network(monkeypatch, outputs):
 
 
 @pytest.mark.parametrize('G,b,live', [(1, 1, 1), (1, 9, 1), (8, 2, 0b01101001)], ids=['pair-b1', 'pair-b9', 'G8-b2-partial'])
-def test_level_backward(env, G, b, live, monkeypatch):
-    """fused.level_backward itself (upper level: frame + teacher + motion, no retrieval) with only the network replaced:
-    its staging of the one-video motion pair or the grouped history forward, its motion call (accumulation, history
+def test_level_backward_step(env, G, b, live, monkeypatch):
+    """fused.level_backward itself on a fused.Step (upper level: frame + teacher + motion, no retrieval) with only the network
+    replaced: its staging of the one-video motion pair or the grouped history forward, its motion call (accumulation, history
     gradient, live mask) and its backward calls, against fp64 autograd of the level loss w.r.t. every network output."""
     from dynaboa_b200 import fused
     from oracle import adaptor_ref
@@ -645,12 +635,13 @@ def test_level_backward(env, G, b, live, monkeypatch):
     kp = head_inputs('frame', nb, gen)['kp']
     hist_kp = head_inputs('frame', nb, gen)['kp']
     o = adaptor_ref.default_options(retrieval=0, lower_level_mixtrain=0, upper_level_mixtrain=0)
-    ad = SimpleNamespace(options=o, smpl_neutral=env.smpl, gmm_f=env.prior, kp_range=(25, 24), teacher=_Teacher(t_arena),
-                         global_step=o.interval + 1, motion_active=live if G > 1 else None, fit_losses={}, kp2dlosses_lower=[],
-                         kp2dlosses_upper={}, get_hist=lambda: (hist_image, hist_kp))
+    # the mean teacher's weights (used only as a key here), no dropout; the motion term of the videos in `live`
+    s = fused.Step(o, G, arena, None, None, env.smpl, env.prior, teacher=t_arena, teacher_masks=lambda B, device, mask: None,
+                   get_hist=lambda live: (hist_image, hist_kp))
+    out = fused.Frame((1 << G) - 1)
     fake_network(monkeypatch, outputs)
     got = capture_backward(monkeypatch)
-    total, _ = fused.level_backward(ad, arena, None, image, kp, False, None)
+    total, _ = fused.level_backward(s, out, arena, image, kp, False, None, (1 << G) - 1, live)
     torch.cuda.synchronize()
     # the teacher's targets are its forward through the same (deterministic) SMPL and projection kernels
     targets = dict(t_p2d=teach.p2d, t_j3d=teach.joints, t_beta=teach.shape, t_R=teach.rot)
@@ -666,7 +657,7 @@ def test_level_backward(env, G, b, live, monkeypatch):
         ref_terms, ref_motion, refs = level_reference(env, [cur, hist], G, nb, kp, hist_kp, targets, TEACHER_W, wm, live, pb)
         rows, n_live = live_rows(live, G, b)
         pairs = [(got[1], refs[0], None, G), (got[0], refs[1], rows, n_live)]
-    errs = level_errors(total, ad.fit_losses['ul/motion_loss'], ref_terms[:, 8] + wm * ref_motion, ref_motion, pairs)
+    errs = level_errors(total, out.fit['ul/motion_loss'], ref_terms[:, 8] + wm * ref_motion, ref_motion, pairs)
     report(f'level_backward G={G} b={b}', errs)
 
 
