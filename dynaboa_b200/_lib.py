@@ -43,6 +43,11 @@ class CropDescStruct(C.Structure):
     _fields_ = [(n, P) for n in ('img', 'wx', 'sx', 'wy', 'sy')] + [(n, I) for n in ('is_u8', 'H', 'W', 'ul_x', 'ul_y', 'Hc', 'Tx', 'Ty')]
 
 
+class RenderDescStruct(C.Structure):
+    _fields_ = ([(n, P) for n in ('verts', 'img', 'out', 'face_ids')]
+                + [('cam4', F * 4), ('rot3x3', F * 9), ('has_rot', I), ('color3', F * 3), ('W', I), ('H', I)])
+
+
 # name -> (restype, argtypes); mirrors include/dynaboa_b200.h one to one
 SIGNATURES = {
     'dboa_version': (C.c_char_p, []),
@@ -124,6 +129,8 @@ SIGNATURES = {
     'dboa_eval_metrics_active': (I, [P, P, P, P, I, I, P, I, P, P, I, I, C.c_ulonglong, P]),
     'dboa_render_scratch_bytes': (L, [I, I, I, I, I]),
     'dboa_render_overlay': (I, [P, P, P, P, I, I, C.POINTER(F), C.POINTER(F), C.POINTER(F), P, I, I, I, P, L, P, P, P]),
+    'dboa_render_scratch_bytes_groups': (L, [C.POINTER(I), C.POINTER(I), I, I, I, I]),
+    'dboa_render_overlay_groups': (I, [C.POINTER(RenderDescStruct), I, P, P, P, I, I, I, P, L, P]),
 }
 
 _ERRORS = {-1: 'DBOA_ERR_ARG', -2: 'DBOA_ERR_SHAPE', -3: 'DBOA_ERR_CUDA', -4: 'DBOA_ERR_UNSUPPORTED'}

@@ -429,5 +429,13 @@ int dboa_render_overlay(const float* verts, const int* faces, const int* vf_offs
     return render_overlay(verts, faces, vf_offsets, vf_faces, NV, NF, cam4, rot3x3, color3, img, W, H, samples, scratch, scratch_bytes, out,
                           face_ids, ST(stream));
 }
+long long dboa_render_scratch_bytes_groups(const int* W, const int* H, int M, int NV, int NF, int samples) {
+    return render_scratch_bytes_groups(W, H, M, NV, NF, samples);
+}
+int dboa_render_overlay_groups(const dboa_render_desc* meshes, int M, const int* faces, const int* vf_offsets, const int* vf_faces, int NV,
+                               int NF, int samples, void* scratch, long long scratch_bytes, dboa_stream_t stream) {
+    if (!meshes || !faces || !vf_offsets || !vf_faces || !scratch) return DBOA_ERR_ARG;
+    return render_overlay_groups(meshes, M, faces, vf_offsets, vf_faces, NV, NF, samples, scratch, scratch_bytes, ST(stream));
+}
 
 }  // extern "C"

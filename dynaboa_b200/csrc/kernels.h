@@ -149,5 +149,8 @@ long long render_scratch_bytes(int W, int H, int NV, int NF, int samples);
 int render_overlay(const float* verts, const int* faces, const int* vf_offsets, const int* vf_faces, int NV, int NF, const float cam4[4],
                    const float rot3x3[9], const float color3[3], const unsigned char* img, int W, int H, int samples, void* scratch,
                    long long scratch_bytes, unsigned char* out, int* face_ids, cudaStream_t st);
+long long render_scratch_bytes_groups(const int* W, const int* H, int M, int NV, int NF, int samples);
+int render_overlay_groups(const dboa_render_desc* meshes, int M, const int* faces, const int* vf_offsets, const int* vf_faces, int NV,
+                          int NF, int samples, void* scratch, long long scratch_bytes, cudaStream_t st);
 
 }  // namespace dboa

@@ -25,6 +25,13 @@
 // key = order-preserving fp32 depth bits << 32 | face id (the result does not depend on launch order) -> resolve, one
 // thread per pixel.  Everything geometric is computed in double or integers, so the oracle (oracle/render_ref.py, numpy
 // float64) reproduces every winning face bit for bit.
+//
+// Several meshes (render_overlay_groups): M <= 64 meshes of one topology, each over its own frame, in the same 6 kernels and
+// 1 memset.  The per-mesh descriptors (RenderGroups) travel by value in a __grid_constant__ kernel parameter.  Vertex, normal
+// and face kernels take the mesh from blockIdx.y, the scan runs one block per mesh, the raster walks the concatenated
+// (mesh, face, tile) pairs of all meshes, the resolve gives each mesh its own run of row blocks.  Per (mesh, pixel, sample)
+// the arithmetic is the one-mesh arithmetic, and no mesh reads another's scratch, so every mesh's out and face_ids are
+// bit-identical to drawing it alone; render_overlay is the M = 1 call.
 #include <math.h>
 
 #include "common.cuh"
@@ -57,23 +64,53 @@ struct Scratch {
     unsigned long long* keys;    // [H][W][S]
 };
 
+struct Shade {
+    double base[3];
+};
+
+// one mesh of a grouped call: 256 bytes, so the table of 64 stays well inside the 32 KB kernel parameter space
+struct RenderMesh {
+    const float* verts;
+    const unsigned char* img;
+    unsigned char* out;
+    int* face_ids;
+    RenderCam c;
+    Shade sh;
+    Scratch s;
+};
+
+struct RenderGroups {
+    RenderMesh m[64];
+    int first_block[65];         // resolve: blocks [first_block[k], first_block[k + 1]) are mesh k's rows
+    int n, NV, NF, S;
+};
+
 size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
-size_t carve(Scratch* s, char* base, int W, int H, int NV, int NF, int S) {
+// Scratch layout: the vertex, face and prefix arrays of mesh 0, 1, ..., M - 1, then the depth keys of mesh 0, 1, ..., M - 1 as
+// one region (one memset clears them all).  Every array starts on 256 bytes; M = 1 is the one-mesh layout.  Returns the
+// byte size, and with s the arrays of each mesh and *keys_off the offset of the key region.
+size_t carve(Scratch* s, char* base, const int* W, const int* H, int M, int NV, int NF, int S, size_t* keys_off = nullptr) {
     size_t off = 0;
     auto take = [&](size_t bytes) { char* p = base ? base + off : nullptr; off += align256(bytes); return p; };
-    char* pr = take((size_t)NV * 3 * sizeof(double));
-    char* nrm = take((size_t)NV * 3 * sizeof(double));
-    char* fx = take((size_t)NV * 2 * sizeof(long long));
-    char* vz = take((size_t)NV * sizeof(double));
-    char* vok = take((size_t)NV * sizeof(int));
-    char* fidx = take((size_t)NF * sizeof(int4));
-    char* fbox = take((size_t)NF * sizeof(int4));
-    char* prefix = take(((size_t)NF + 1) * sizeof(long long));
-    char* keys = take((size_t)W * H * S * sizeof(unsigned long long));
-    if (s) {
-        s->pr = (double*)pr; s->nrm = (double*)nrm; s->fx = (long long*)fx; s->vz = (double*)vz; s->vok = (int*)vok;
-        s->fidx = (int4*)fidx; s->fbox = (int4*)fbox; s->prefix = (long long*)prefix; s->keys = (unsigned long long*)keys;
+    for (int k = 0; k < M; ++k) {
+        char* pr = take((size_t)NV * 3 * sizeof(double));
+        char* nrm = take((size_t)NV * 3 * sizeof(double));
+        char* fx = take((size_t)NV * 2 * sizeof(long long));
+        char* vz = take((size_t)NV * sizeof(double));
+        char* vok = take((size_t)NV * sizeof(int));
+        char* fidx = take((size_t)NF * sizeof(int4));
+        char* fbox = take((size_t)NF * sizeof(int4));
+        char* prefix = take(((size_t)NF + 1) * sizeof(long long));
+        if (s) {
+            s[k].pr = (double*)pr; s[k].nrm = (double*)nrm; s[k].fx = (long long*)fx; s[k].vz = (double*)vz; s[k].vok = (int*)vok;
+            s[k].fidx = (int4*)fidx; s[k].fbox = (int4*)fbox; s[k].prefix = (long long*)prefix;
+        }
+    }
+    if (keys_off) *keys_off = off;
+    for (int k = 0; k < M; ++k) {
+        char* keys = take((size_t)W[k] * H[k] * S * sizeof(unsigned long long));
+        if (s) s[k].keys = (unsigned long long*)keys;
     }
     return off;
 }
@@ -82,9 +119,13 @@ __device__ __forceinline__ double dm(double a, double b) { return __dmul_rn(a, b
 __device__ __forceinline__ double da(double a, double b) { return __dadd_rn(a, b); }
 __device__ __forceinline__ double ds(double a, double b) { return __dadd_rn(a, -b); }
 
-__global__ void render_vertex_kernel(const float* __restrict__ verts, int NV, RenderCam c, Scratch s) {
+__global__ void render_vertex_kernel(const __grid_constant__ RenderGroups g) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= NV) return;
+    if (i >= g.NV) return;
+    const RenderMesh& m = g.m[blockIdx.y];
+    const float* __restrict__ verts = m.verts;
+    const RenderCam& c = m.c;
+    const Scratch& s = m.s;
     const size_t i3 = (size_t)i * 3;
     const double q[3] = {(double)verts[i3], -(double)verts[i3 + 1], -(double)verts[i3 + 2]};
     double p[3] = {q[0], q[1], q[2]};
@@ -102,10 +143,12 @@ __global__ void render_vertex_kernel(const float* __restrict__ verts, int NV, Re
 
 // trimesh Trimesh.vertex_normals: sum over the incident faces of (corner angle) * (unit face normal), normalised.  Faces with
 // zero area contribute nothing; a corner angle below 1e-8 zeroes all three angles of its face (triangles.angles).
-__global__ void render_normal_kernel(const int* __restrict__ faces, int NF, int NV, const int* __restrict__ vf_off,
-                                     const int* __restrict__ vf_faces, Scratch s) {
+__global__ void render_normal_kernel(const int* __restrict__ faces, const int* __restrict__ vf_off, const int* __restrict__ vf_faces,
+                                     const __grid_constant__ RenderGroups g) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int NF = g.NF, NV = g.NV;
     if (i >= NV) return;
+    const Scratch& s = g.m[blockIdx.y].s;
     double acc[3] = {0.0, 0.0, 0.0};
     for (int e = vf_off[i]; e < vf_off[i + 1]; ++e) {
         const int f = vf_faces[e];
@@ -144,9 +187,13 @@ __global__ void render_normal_kernel(const int* __restrict__ faces, int NF, int 
 __device__ __forceinline__ long long floordiv(long long a, long long b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
 
 // cull + bounding box; writes the face's tile count to prefix[f + 1]
-__global__ void render_face_kernel(const int* __restrict__ faces, int NF, int NV, Scratch s, int W, int H) {
+__global__ void render_face_kernel(const int* __restrict__ faces, const __grid_constant__ RenderGroups g) {
     const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    const int NF = g.NF, NV = g.NV;
     if (f >= NF) return;
+    const RenderMesh& m = g.m[blockIdx.y];
+    const Scratch& s = m.s;
+    const int W = m.c.W, H = m.c.H;
     long long count = 0;
     const int i0 = faces[(size_t)f * 3], i1 = faces[(size_t)f * 3 + 1], i2 = faces[(size_t)f * 3 + 2];
     if (i0 >= 0 && i0 < NV && i1 >= 0 && i1 < NV && i2 >= 0 && i2 < NV && s.vok[i0] && s.vok[i1] && s.vok[i2]) {
@@ -169,8 +216,10 @@ __global__ void render_face_kernel(const int* __restrict__ faces, int NF, int NV
     s.prefix[f + 1] = count;
 }
 
-// in-place inclusive scan of prefix[1..NF] by one block (the face count is small; this runs once per draw)
-__global__ void __launch_bounds__(1024) render_scan_kernel(long long* __restrict__ prefix, int NF) {
+// in-place inclusive scan of prefix[1..NF] by one block per mesh (the face count is small; this runs once per draw)
+__global__ void __launch_bounds__(1024) render_scan_kernel(const __grid_constant__ RenderGroups g) {
+    long long* __restrict__ prefix = g.m[blockIdx.x].s.prefix;
+    const int NF = g.NF;
     __shared__ long long warp_tot[32];
     __shared__ long long carry;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -211,11 +260,26 @@ __device__ __forceinline__ bool top_left(long long px, long long py, long long q
 
 __constant__ int c_off4[4][2] = {{-32, -96}, {96, -32}, {-96, 32}, {32, 96}};   // 1/256 pixel: (-2,-6) (6,-2) (-6,2) (2,6) / 16
 
-__global__ void __launch_bounds__(256) render_raster_kernel(int NF, Scratch s, int W, int S) {
-    const long long total = s.prefix[NF];
+// grid-stride over the (mesh, face, tile) pairs of all meshes: mesh k owns the pairs [first[k], first[k + 1])
+__global__ void __launch_bounds__(256) render_raster_kernel(const __grid_constant__ RenderGroups g) {
+    __shared__ long long first[65];
+    const int NF = g.NF, S = g.S, n = g.n;
+    if (threadIdx.x < n) first[threadIdx.x + 1] = g.m[threadIdx.x].s.prefix[NF];
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        first[0] = 0;
+        for (int k = 1; k <= n; ++k) first[k] += first[k - 1];
+    }
+    __syncthreads();
+    const long long total = first[n];
     const int lane = threadIdx.x & 31;
     const long long nwarps = (long long)gridDim.x * (blockDim.x >> 5);
-    for (long long pair = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; pair < total; pair += nwarps) {
+    int mk = 0;                                                        // a warp's pairs only grow: its mesh only advances
+    for (long long gpair = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; gpair < total; gpair += nwarps) {
+        while (first[mk + 1] <= gpair) ++mk;
+        const Scratch s = g.m[mk].s;
+        const int W = g.m[mk].c.W;
+        const long long pair = gpair - first[mk];
         int lo = 0, hi = NF;                                           // last face with prefix[f] <= pair
         while (lo < hi) {
             const int mid = (int)(((long long)lo + hi + 1) >> 1);
@@ -251,10 +315,6 @@ __global__ void __launch_bounds__(256) render_raster_kernel(int NF, Scratch s, i
         }
     }
 }
-
-struct Shade {
-    double base[3];
-};
 
 // pyrender mesh.frag, metallic 0, roughness 1 (see the header), one (pixel, face): returns the three bytes
 __device__ void shade_face(const Scratch& s, int f, int c, int r, const Shade& sh, int out[3]) {
@@ -300,10 +360,22 @@ __device__ void shade_face(const Scratch& s, int f, int c, int r, const Shade& s
     }
 }
 
-__global__ void render_resolve_kernel(Scratch s, Shade sh, const unsigned char* __restrict__ img, int W, int H, int S,
-                                      unsigned char* __restrict__ out, int* __restrict__ face_ids) {
-    const int c = blockIdx.x * blockDim.x + threadIdx.x, r = blockIdx.y;
+// mesh k's (H, ceil(W / 128)) row blocks are the blocks [first_block[k], first_block[k + 1]) of a one-dimensional grid
+__global__ void __launch_bounds__(128) render_resolve_kernel(const __grid_constant__ RenderGroups g) {
+    int lo = 0, hi = g.n - 1;                                          // last mesh whose first block is <= blockIdx.x
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (g.first_block[mid] <= (int)blockIdx.x) lo = mid; else hi = mid - 1;
+    }
+    const RenderMesh& m = g.m[lo];
+    const Scratch& s = m.s;
+    const int W = m.c.W, S = g.S;
+    const int bx = (W + 127) / 128, b = (int)blockIdx.x - g.first_block[lo];
+    const int c = (b % bx) * blockDim.x + threadIdx.x, r = b / bx;
     if (c >= W) return;
+    const unsigned char* __restrict__ img = m.img;
+    unsigned char* __restrict__ out = m.out;
+    int* __restrict__ face_ids = m.face_ids;
     const size_t pix = (size_t)r * W + c;
     int fid[4], byt[4][3], sum[3] = {0, 0, 0}, k = 0;
     for (int q = 0; q < S; ++q) {
@@ -318,7 +390,7 @@ __global__ void render_resolve_kernel(Scratch s, Shade sh, const unsigned char* 
         if (same >= 0)
             for (int j = 0; j < 3; ++j) byt[q][j] = byt[same][j];
         else
-            shade_face(s, fid[q], c, r, sh, byt[q]);
+            shade_face(s, fid[q], c, r, m.sh, byt[q]);
         for (int j = 0; j < 3; ++j) sum[j] += byt[q][j];
     }
     for (int j = 0; j < 3; ++j) out[pix * 3 + j] = k ? (unsigned char)((sum[j] + S / 2) / S) : img[pix * 3 + j];
@@ -326,44 +398,79 @@ __global__ void render_resolve_kernel(Scratch s, Shade sh, const unsigned char* 
 
 }  // namespace
 
-long long render_scratch_bytes(int W, int H, int NV, int NF, int samples) {
-    if (W < 1 || H < 1 || W > 8192 || H > 8192 || NV < 0 || NF < 0) return DBOA_ERR_SHAPE;
+long long render_scratch_bytes_groups(const int* W, const int* H, int M, int NV, int NF, int samples) {
+    if (!W || !H) return DBOA_ERR_ARG;
+    if (M < 1 || M > 64 || NV < 0 || NF < 0) return DBOA_ERR_SHAPE;
+    for (int k = 0; k < M; ++k)
+        if (W[k] < 1 || H[k] < 1 || W[k] > 8192 || H[k] > 8192) return DBOA_ERR_SHAPE;
     if (samples != 1 && samples != 4) return DBOA_ERR_ARG;
-    return (long long)carve(nullptr, nullptr, W, H, NV, NF, samples);
+    return (long long)carve(nullptr, nullptr, W, H, M, NV, NF, samples);
+}
+
+long long render_scratch_bytes(int W, int H, int NV, int NF, int samples) { return render_scratch_bytes_groups(&W, &H, 1, NV, NF, samples); }
+
+int render_overlay_groups(const dboa_render_desc* meshes, int M, const int* faces, const int* vf_offsets, const int* vf_faces, int NV,
+                          int NF, int samples, void* scratch, long long scratch_bytes, cudaStream_t st) {
+    if (!meshes) return DBOA_ERR_ARG;
+    if (M < 1 || M > 64) return DBOA_ERR_SHAPE;
+    int W[64], H[64];
+    for (int k = 0; k < M; ++k) { W[k] = meshes[k].W; H[k] = meshes[k].H; }
+    const long long need = render_scratch_bytes_groups(W, H, M, NV, NF, samples);
+    if (need < 0) return (int)need;
+    for (int k = 0; k < M; ++k)
+        if (!meshes[k].verts || !meshes[k].img || !meshes[k].out) return DBOA_ERR_ARG;
+    if (scratch_bytes < need) return DBOA_ERR_ARG;
+    RenderGroups g;
+    g.n = M; g.NV = NV; g.NF = NF; g.S = samples;
+    Scratch s[64];
+    size_t keys_off = 0;
+    carve(s, (char*)scratch, W, H, M, NV, NF, samples, &keys_off);
+    long long blocks = 0;
+    for (int k = 0; k < M; ++k) {
+        const dboa_render_desc& d = meshes[k];
+        RenderMesh& m = g.m[k];
+        m.verts = d.verts; m.img = d.img; m.out = d.out; m.face_ids = d.face_ids;
+        RenderCam& c = m.c;
+        c.sx = d.cam4[0]; c.sy = d.cam4[1]; c.tx = d.cam4[2]; c.ty = d.cam4[3];
+        c.has_rot = d.has_rot != 0;
+        for (int j = 0; j < 9; ++j) c.R[j] = c.has_rot ? (double)d.rot3x3[j] : (j % 4 == 0 ? 1.0 : 0.0);
+        c.W = W[k]; c.H = H[k]; c.S = samples;
+        for (int j = 0; j < 3; ++j) m.sh.base[j] = d.color3[j];
+        m.s = s[k];
+        g.first_block[k] = (int)blocks;
+        blocks += (long long)ceil_div(W[k], 128) * H[k];
+    }
+    g.first_block[M] = (int)blocks;                                     // <= 64 * 64 * 8192
+    if (NV > 0) {
+        render_vertex_kernel<<<dim3(ceil_div(NV, 128), M), 128, 0, st>>>(g);
+        DBOA_TRY(check_launch());
+        render_normal_kernel<<<dim3(ceil_div(NV, 128), M), 128, 0, st>>>(faces, vf_offsets, vf_faces, g);
+        DBOA_TRY(check_launch());
+    }
+    if (NF > 0) {
+        render_face_kernel<<<dim3(ceil_div(NF, 128), M), 128, 0, st>>>(faces, g);
+        DBOA_TRY(check_launch());
+    }
+    render_scan_kernel<<<M, 1024, 0, st>>>(g);
+    DBOA_TRY(check_launch());
+    if (cudaMemsetAsync((char*)scratch + keys_off, 0xff, (size_t)need - keys_off, st) != cudaSuccess) return DBOA_ERR_CUDA;
+    render_raster_kernel<<<num_sms() * 8, 256, 0, st>>>(g);
+    DBOA_TRY(check_launch());
+    render_resolve_kernel<<<(unsigned)blocks, 128, 0, st>>>(g);
+    return check_launch();
 }
 
 int render_overlay(const float* verts, const int* faces, const int* vf_offsets, const int* vf_faces, int NV, int NF, const float cam4[4],
                    const float rot3x3[9], const float color3[3], const unsigned char* img, int W, int H, int samples, void* scratch,
                    long long scratch_bytes, unsigned char* out, int* face_ids, cudaStream_t st) {
-    const long long need = render_scratch_bytes(W, H, NV, NF, samples);
-    if (need < 0) return (int)need;
-    if (scratch_bytes < need) return DBOA_ERR_ARG;
-    RenderCam c;
-    c.sx = cam4[0]; c.sy = cam4[1]; c.tx = cam4[2]; c.ty = cam4[3];
-    c.has_rot = rot3x3 != nullptr;
-    for (int k = 0; k < 9; ++k) c.R[k] = rot3x3 ? (double)rot3x3[k] : (k % 4 == 0 ? 1.0 : 0.0);
-    c.W = W; c.H = H; c.S = samples;
-    Shade sh;
-    for (int j = 0; j < 3; ++j) sh.base[j] = color3[j];
-    Scratch s;
-    carve(&s, (char*)scratch, W, H, NV, NF, samples);
-    if (NV > 0) {
-        render_vertex_kernel<<<ceil_div(NV, 128), 128, 0, st>>>(verts, NV, c, s);
-        DBOA_TRY(check_launch());
-        render_normal_kernel<<<ceil_div(NV, 128), 128, 0, st>>>(faces, NF, NV, vf_offsets, vf_faces, s);
-        DBOA_TRY(check_launch());
-    }
-    if (NF > 0) {
-        render_face_kernel<<<ceil_div(NF, 128), 128, 0, st>>>(faces, NF, NV, s, W, H);
-        DBOA_TRY(check_launch());
-    }
-    render_scan_kernel<<<1, 1024, 0, st>>>(s.prefix, NF);
-    DBOA_TRY(check_launch());
-    if (cudaMemsetAsync(s.keys, 0xff, (size_t)W * H * samples * sizeof(unsigned long long), st) != cudaSuccess) return DBOA_ERR_CUDA;
-    render_raster_kernel<<<num_sms() * 8, 256, 0, st>>>(NF, s, W, samples);
-    DBOA_TRY(check_launch());
-    render_resolve_kernel<<<dim3(ceil_div(W, 128), H), 128, 0, st>>>(s, sh, img, W, H, samples, out, face_ids);
-    return check_launch();
+    dboa_render_desc d;
+    d.verts = verts; d.img = img; d.out = out; d.face_ids = face_ids;
+    for (int j = 0; j < 4; ++j) d.cam4[j] = cam4[j];
+    d.has_rot = rot3x3 != nullptr;
+    for (int j = 0; j < 9; ++j) d.rot3x3[j] = rot3x3 ? rot3x3[j] : 0.f;
+    for (int j = 0; j < 3; ++j) d.color3[j] = color3[j];
+    d.W = W; d.H = H;
+    return render_overlay_groups(&d, 1, faces, vf_offsets, vf_faces, NV, NF, samples, scratch, scratch_bytes, st);
 }
 
 }  // namespace dboa

@@ -5,7 +5,11 @@ signature and defaults; the drawing is one ``dboa_render_overlay`` call (csrc/re
 ``img`` is an (H, W, 3) uint8 frame: a numpy array gives a numpy result (the reference's contract), a CUDA tensor gives a
 CUDA tensor, so a frame that is already on the device is drawn on and stays there.  The reference builds a new ``Renderer``
 for every frame (base_adaptor.py:441, webcam_utils.py:77), so construction does no work: the device copy of the faces and
-their vertex->face adjacency are cached per faces array, the scratch buffer per (W, H, samples, mesh size).
+their vertex->face adjacency are cached per faces array, the scratch buffer per (frame sizes, samples, mesh size).
+
+``draw_groups`` / ``render_groups`` draw many meshes of one topology, each over its own frame, in one
+``dboa_render_overlay_groups`` call (the adapted and base meshes of every stream of a webcam pool); ``draw`` is its
+one-mesh case.
 """
 import ctypes as C
 import math
@@ -17,7 +21,7 @@ from . import _lib
 from ._lib import ptr, stream
 
 _faces_cache = {}        # (id(faces), NV, device) -> (faces array kept alive, faces, vf_offsets, vf_faces)
-_scratch_cache = {}      # (W, H, samples, NV, NF, device) -> uint8 tensor
+_scratch_cache = {}      # (((W, H), ...), samples, NV, NF, device) -> uint8 tensor
 _smpl_faces = {}         # SMPL model directory -> faces
 
 
@@ -67,42 +71,81 @@ def _device_faces(faces, nv, device):
     return dev
 
 
-def _scratch(W, H, samples, nv, nf, device):
-    key = (W, H, samples, nv, nf, device)
+def _scratch(sizes, samples, nv, nf, device):
+    """Scratch of one grouped call over frames of the (W, H) ``sizes``, cached per (sizes, samples, mesh size, device)."""
+    key = (tuple(sizes), samples, nv, nf, device)
     buf = _scratch_cache.get(key)
     if buf is None:
-        need = _lib.load().dboa_render_scratch_bytes(W, H, nv, nf, samples)
-        _lib.check(int(need) if need < 0 else 0, 'dboa_render_scratch_bytes')
+        M = len(sizes)
+        W, H = (C.c_int * M)(*[w for w, _ in sizes]), (C.c_int * M)(*[h for _, h in sizes])
+        need = _lib.load().dboa_render_scratch_bytes_groups(W, H, M, nv, nf, samples)
+        _lib.check(int(need) if need < 0 else 0, 'dboa_render_scratch_bytes_groups')
         if len(_scratch_cache) >= 4:
             _scratch_cache.clear()
         buf = _scratch_cache[key] = torch.empty(int(need), dtype=torch.uint8, device=device)
     return buf
 
 
-def draw(img, verts, faces, cam4, rot=None, color=(1.0, 1.0, 0.9), samples=4, face_ids=False):
-    """One ``dboa_render_overlay`` call.  img: (H, W, 3) uint8 CUDA tensor; verts: (NV, 3) CUDA tensor; faces: (NF, 3) integer
-    numpy array (cached on the device by identity); cam4 = (sx, sy, tx, ty); rot: optional 3 x 3 rotation applied after
-    Rx(180).  Returns the (H, W, 3) uint8 result, and with ``face_ids`` also the (H, W, samples) int32 winning faces."""
-    _lib.require_cuda(img, verts)
-    if img.dtype != torch.uint8 or img.dim() != 3 or img.shape[2] != 3:
-        raise ValueError(f'img must be an (H, W, 3) uint8 frame, got {tuple(img.shape)} {img.dtype}')
+MAX_MESHES = 64
+
+
+def draw_groups(imgs, verts, faces, cam4s, colors, rots=None, samples=4, face_ids=False):
+    """One ``dboa_render_overlay_groups`` call: M <= 64 meshes of one topology, mesh k drawn over ``imgs[k]``.  imgs: M (H_k,
+    W_k, 3) uint8 CUDA tensors (one tensor may appear several times: entries that share a frame each get their own output);
+    verts: M (NV, 3) CUDA tensors, or one (M, NV, 3) tensor; faces: (NF, 3) integer numpy array; cam4s: host (M, 4) array of
+    (sx, sy, tx, ty); colors: host (M, 3) base colours in 0..1; rots: None or M optional 3 x 3 rotations.  Returns the M (H_k,
+    W_k, 3) results, and with ``face_ids`` also the M (H_k, W_k, samples) int32 winning faces.  Each entry is bit-identical to
+    ``draw`` on that entry alone."""
+    M = len(imgs)
+    if not 1 <= M <= MAX_MESHES:
+        raise ValueError(f'draw_groups draws 1 to {MAX_MESHES} meshes per call, got {M}')
+    cam4s = np.asarray(cam4s, dtype=np.float64).reshape(-1, 4) if len(cam4s) else np.zeros((0, 4))
+    colors = np.asarray(colors, dtype=np.float64).reshape(-1, 3) if len(colors) else np.zeros((0, 3))
+    rots = [None] * M if rots is None else list(rots)
+    if len(verts) != M or len(cam4s) != M or len(colors) != M or len(rots) != M:
+        raise ValueError(f'expected {M} vertex sets, cameras, colours and rotations, one per frame, got {len(verts)}, '
+                         f'{len(cam4s)}, {len(colors)} and {len(rots)}')
     if samples not in (1, 4):
         raise ValueError('samples must be 1 or 4')
-    H, W = int(img.shape[0]), int(img.shape[1])
-    img = img.contiguous()
-    v = verts.detach().reshape(-1, 3).to(device=img.device, dtype=torch.float32).contiguous()
-    nv = v.shape[0]
-    f_dev, vf_off, vf_faces = _device_faces(faces, nv, img.device)
+    for k, img in enumerate(imgs):
+        if not torch.is_tensor(img) or img.dtype != torch.uint8 or img.dim() != 3 or img.shape[2] != 3:
+            raise ValueError(f'entry {k}: img must be an (H, W, 3) uint8 frame, got {tuple(img.shape)} {img.dtype}')
+    _lib.require_cuda(*imgs, *verts)
+    dev = imgs[0].device
+    imgs = [i.contiguous() for i in imgs]
+    vs = [v.detach().reshape(-1, 3).to(device=dev, dtype=torch.float32).contiguous() for v in verts]
+    nv = vs[0].shape[0]
+    if any(v.shape[0] != nv for v in vs):
+        raise ValueError('every mesh of a grouped call has the same number of vertices')
+    f_dev, vf_off, vf_faces = _device_faces(faces, nv, dev)
     nf = f_dev.shape[0]
-    scratch = _scratch(W, H, samples, nv, nf, img.device)
-    out = torch.empty_like(img)
-    ids = torch.empty(H, W, samples, dtype=torch.int32, device=img.device) if face_ids else None
-    cam = (C.c_float * 4)(*[float(c) for c in np.asarray(cam4, dtype=np.float64).reshape(4)])
-    R = None if rot is None else (C.c_float * 9)(*[float(x) for x in np.asarray(rot, dtype=np.float64).reshape(9)])
-    col = (C.c_float * 3)(*[float(c) for c in np.asarray(color, dtype=np.float64).reshape(3)])
-    _lib.call('dboa_render_overlay', ptr(v), ptr(f_dev), ptr(vf_off), ptr(vf_faces), nv, nf, cam, R, col, ptr(img), W, H, samples,
-              ptr(scratch), scratch.numel(), ptr(out), ptr(ids), stream())
-    return (out, ids) if face_ids else out
+    sizes = [(int(i.shape[1]), int(i.shape[0])) for i in imgs]
+    scratch = _scratch(sizes, samples, nv, nf, dev)
+    outs = [torch.empty_like(i) for i in imgs]
+    ids = [torch.empty(i.shape[0], i.shape[1], samples, dtype=torch.int32, device=dev) for i in imgs] if face_ids else [None] * M
+    desc = (_lib.RenderDescStruct * M)()
+    for k in range(M):
+        d = desc[k]
+        d.verts, d.img, d.out, d.face_ids = ptr(vs[k]), ptr(imgs[k]), ptr(outs[k]), ptr(ids[k])
+        d.cam4[:] = [float(c) for c in cam4s[k]]
+        d.has_rot = int(rots[k] is not None)
+        if rots[k] is not None:
+            d.rot3x3[:] = [float(x) for x in np.asarray(rots[k], dtype=np.float64).reshape(9)]
+        d.color3[:] = [float(c) for c in colors[k]]
+        d.W, d.H = sizes[k]
+    _lib.call('dboa_render_overlay_groups', desc, M, ptr(f_dev), ptr(vf_off), ptr(vf_faces), nv, nf, samples, ptr(scratch),
+              scratch.numel(), stream())
+    return (outs, ids) if face_ids else outs
+
+
+def draw(img, verts, faces, cam4, rot=None, color=(1.0, 1.0, 0.9), samples=4, face_ids=False):
+    """The one-mesh case of ``draw_groups``.  img: (H, W, 3) uint8 CUDA tensor; verts: (NV, 3) CUDA tensor; faces: (NF, 3)
+    integer numpy array (cached on the device by identity); cam4 = (sx, sy, tx, ty); rot: optional 3 x 3 rotation applied after
+    Rx(180).  Returns the (H, W, 3) uint8 result, and with ``face_ids`` also the (H, W, samples) int32 winning faces."""
+    _lib.require_cuda(img, verts)
+    r = draw_groups([img], [verts], faces, [np.asarray(cam4, dtype=np.float64).reshape(4)],
+                    [np.asarray(color, dtype=np.float64).reshape(3)], rots=[rot], samples=samples, face_ids=face_ids)
+    return (r[0][0], r[1][0]) if face_ids else r[0]
 
 
 def get_smpl_faces():
@@ -160,3 +203,46 @@ def render(vts, cam, image, bbox, color=[205, 129, 98]):
     renderer = Renderer(resolution=(ori_w, ori_h), orig_img=True, wireframe=False)
     rendered = renderer.render(image, vts[0], ori_pred_cams[0], color=np.array(color) / 255)
     return rendered.flip(-1) if torch.is_tensor(rendered) else rendered[:, :, ::-1]
+
+
+def render_groups(vts, cams, images, bboxes, colors):
+    """``render`` for many meshes at once: entry k draws the first mesh of ``vts[k]`` with the crop camera ``cams[k]`` and box
+    ``bboxes[k]`` over ``images[k]`` (RGB, numpy or CUDA; entries may share a frame) in ``colors[k]`` (0..255), and returns it
+    in BGR order, numpy in -> numpy out, CUDA in -> CUDA out.  Each result is bit-identical to ``render`` on that entry.  The
+    device cameras come to the host in one copy; the meshes are drawn in one ``dboa_render_overlay_groups`` call per 64."""
+    n = len(images)
+    if len(vts) != n or len(cams) != n or len(bboxes) != n or len(colors) != n:
+        raise ValueError(f'expected {n} meshes, cameras, boxes and colours, one per image, got {len(vts)}, {len(cams)}, '
+                         f'{len(bboxes)} and {len(colors)}')
+    if n == 0:
+        return []
+    dev_cams = [k for k, c in enumerate(cams) if torch.is_tensor(c)]
+    host_cams = list(cams)
+    if dev_cams:
+        dts = {cams[k].dtype for k in dev_cams}
+        rows = [cams[k].detach()[:1] for k in dev_cams]
+        flat = torch.cat(rows).cpu().numpy() if len(dts) == 1 else [r.cpu().numpy() for r in rows]
+        for i, k in enumerate(dev_cams):
+            host_cams[k] = flat[i:i + 1]
+    uploads, frames, on_host = {}, [], []
+    for img in images:
+        on_host.append(not torch.is_tensor(img))
+        if on_host[-1]:
+            key = id(img)
+            if key not in uploads:
+                uploads[key] = (img, torch.from_numpy(np.ascontiguousarray(img)).cuda())
+            frames.append(uploads[key][1])
+        else:
+            frames.append(img)
+    cam4s, verts = [], []
+    for k in range(n):
+        ori_h, ori_w = images[k].shape[:2]
+        cam4s.append(convert_crop_cam_to_orig_img(np.asarray(host_cams[k])[:1], bboxes[k], ori_w, ori_h)[0])
+        v = vts[k][0]
+        verts.append((v if torch.is_tensor(v) else torch.from_numpy(np.asarray(v, dtype=np.float32))).to(frames[k].device))
+    cols = [np.array(c) / 255 for c in colors]
+    faces, outs = get_smpl_faces(), []
+    for a in range(0, n, MAX_MESHES):
+        b = min(n, a + MAX_MESHES)
+        outs += draw_groups(frames[a:b], verts[a:b], faces, cam4s[a:b], cols[a:b], samples=Renderer.samples)
+    return [o.cpu().numpy()[:, :, ::-1] if h else o.flip(-1) for o, h in zip(outs, on_host)]

@@ -26,7 +26,7 @@ from types import SimpleNamespace
 import numpy as np
 import torch
 
-from . import config, dataprocess, hmr as hmr_mod
+from . import config, dataprocess, hmr as hmr_mod, render as render_mod
 from .adaptor import Adaptor
 from .hmr import hmr
 from .multivideo import MultiVideoAdaptor
@@ -133,8 +133,10 @@ class MultiWebcamAdaptor(MultiVideoAdaptor):
 
     ``online_adaptation(frames, detections)`` advances every stream that has a frame and detections by one tick: the boxes on
     the host, one grouped crop and one grouped keypoint call into the pool's staging rows, the bilevel step, one masked output
-    forward.  ``adapt_processed`` does the same on already cropped rows.  ``reload(g)`` is the demo's key ``r`` for stream g;
-    ``start(g)`` puts a new camera into slot g.  Per slot, ``video_steps[g]`` counts the stream's frames."""
+    forward.  ``adapt_processed`` does the same on already cropped rows.  ``render(frames, results)`` draws the tick's meshes
+    in one grouped overlay call.  ``reload(g)`` is the demo's key ``r`` for stream g; ``start(g)`` puts a new camera into slot
+    g.  Per slot, ``video_steps[g]`` counts the stream's frames."""
+    colors = ((205, 129, 98), (100, 100, 200))             # adapted and base mesh (reference dynaboa_webcam.py:410,416)
     kp_range = (0, 25)
     motion_lead = 1
 
@@ -245,4 +247,38 @@ class MultiWebcamAdaptor(MultiVideoAdaptor):
             if base is not None:
                 res.update(vts_base=base[0][g:g + 1], cam_base=base[1][g:g + 1])
             out.append(res)
+        return out
+
+    def render(self, frames, results):
+        """The viewer's drawing for one tick (reference dynaboa_webcam.py:409-418 per stream): ``frames`` as passed to
+        ``online_adaptation`` (the (H, W, 3) RGB uint8 frames, numpy or CUDA), ``results`` the list it returned.  Returns per
+        stream ``(rendered, rendered_base)``, BGR like ``render.render`` and on the frame's side (numpy or CUDA);
+        ``rendered_base`` is None without ``test_basemodel``, and a stream without a result gives None.  Every mesh of the tick
+        is drawn in one ``dboa_render_overlay_groups`` call (one per 64 meshes), with all cameras brought to the host in one
+        copy; each image is bit-identical to ``render.render`` on that stream's result alone."""
+        G = self.G
+        if len(frames) != G or len(results) != G:
+            raise ValueError(f'expected {G} frames and {G} results, one per stream, got {len(frames)} and {len(results)}')
+        base = bool(self.options.test_basemodel)
+        vts, cams, images, bboxes, colors, owner = [], [], [], [], [], []
+        for g, (f, res) in enumerate(zip(frames, results)):
+            if res is None:
+                continue
+            if f is None or not _frame_ok(f) or (f.dtype != torch.uint8 if torch.is_tensor(f) else np.dtype(f.dtype) != np.uint8):
+                raise ValueError(f'stream {g}: expected the (H, W, 3) uint8 frame of its result, got '
+                                 f'{None if f is None else (tuple(f.shape), f.dtype)}')
+            for key, col in (('', self.colors[0]), ('_base', self.colors[1])) if base else (('', self.colors[0]),):
+                vts.append(res['vts' + key])
+                cams.append(res['cam' + key])
+                images.append(f)
+                bboxes.append(res['bbox'])
+                colors.append(col)
+                owner.append(g)
+        drawn = render_mod.render_groups(vts, cams, images, bboxes, colors)
+        out = [None] * G
+        for i, g in enumerate(owner):
+            if out[g] is None:
+                out[g] = (drawn[i], None)
+            else:
+                out[g] = (out[g][0], drawn[i])
         return out

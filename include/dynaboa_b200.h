@@ -390,6 +390,33 @@ long long dboa_render_scratch_bytes(int W, int H, int NV, int NF, int samples);
 int dboa_render_overlay(const float* verts, const int* faces, const int* vf_offsets, const int* vf_faces, int NV, int NF, const float cam4[4],
                         const float rot3x3[9], const float color3[3], const unsigned char* img, int W, int H, int samples, void* scratch,
                         long long scratch_bytes, unsigned char* out, int* face_ids, dboa_stream_t stream);
+/* Grouped overlay: M meshes of one topology (faces, vf_offsets, vf_faces, NV, NF) and one sample count, each over its own
+ * frame, in one call: the adapted and the base mesh of every webcam stream of a tick.  dboa_render_desc: the per-mesh
+ * arguments of dboa_render_overlay (verts, img, out and face_ids are device pointers, face_ids may be NULL; has_rot = 0
+ * means no rotation and rot3x3 is not read; W, H the frame size of that mesh).  `meshes` is a HOST array of M descriptors,
+ * passed to the kernels by value, so a call makes no host-to-device copy and never synchronises.  Two entries may read the
+ * same img; the outputs (out, face_ids) must not alias any input or each other.  6 kernel launches and 1 memset, whatever M:
+ * vertices, normals and face set-up take the mesh from the grid's y index, the scan runs one block per mesh, the raster walks
+ * the (mesh, face, tile) pairs of all meshes, the resolve gives every mesh its own row blocks.  Every mesh's out and face_ids
+ * are bit-identical to dboa_render_overlay on that entry alone; M = 1 is dboa_render_overlay.
+ * scratch: dboa_render_scratch_bytes_groups(W, H, M, NV, NF, samples) bytes (W, H: host arrays of the M frame sizes; M = 1
+ * gives dboa_render_scratch_bytes).  Before any device access: DBOA_ERR_ARG for a NULL meshes, faces, vf_offsets, vf_faces or
+ * scratch; DBOA_ERR_SHAPE for M outside 1..64, NV or NF < 0 or any W or H outside 1..8192; then DBOA_ERR_ARG for samples
+ * other than 1 or 4, an entry's NULL verts, img or out, or too small a scratch.  The size query returns the same codes. */
+typedef struct dboa_render_desc {
+    const float* verts;
+    const unsigned char* img;
+    unsigned char* out;
+    int* face_ids;
+    float cam4[4];
+    float rot3x3[9];
+    int has_rot;
+    float color3[3];
+    int W, H;
+} dboa_render_desc;
+long long dboa_render_scratch_bytes_groups(const int* W, const int* H, int M, int NV, int NF, int samples);
+int dboa_render_overlay_groups(const dboa_render_desc* meshes, int M, const int* faces, const int* vf_offsets, const int* vf_faces, int NV,
+                               int NF, int samples, void* scratch, long long scratch_bytes, dboa_stream_t stream);
 
 #ifdef __cplusplus
 }
