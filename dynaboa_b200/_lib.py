@@ -12,7 +12,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('DBOA_LIB_PATH') or os.path.join(_HERE, 'libdynaboa_b200.so')     # the override is for A/B experiments
 
-P, I, L, F = C.c_void_p, C.c_int, C.c_longlong, C.c_float
+P, I, L, F, D = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_double
 
 
 class SmplModelStruct(C.Structure):
@@ -107,9 +107,9 @@ SIGNATURES = {
     'dboa_loss_motion_groups': (I, [P, P, P, P, F, P, P, P, I, I, I, I, I, P]),
     'dboa_loss_motion_active': (I, [P, P, P, P, F, P, P, P, I, I, I, I, I, C.c_ulonglong, P]),
     'dboa_sgd_update': (I, [P, P, P, F, L, P]),
-    'dboa_adam_ema': (I, [P, P, P, P, P, L, F, F, F, F, I, F, P]),
-    'dboa_ema_update': (I, [P, P, L, F, P]),
-    'dboa_adam_ema_scaled': (I, [P, P, P, P, P, L, F, F, F, F, I, F, F, P]),
+    'dboa_adam_ema': (I, [P, P, P, P, P, L, D, D, D, D, I, D, P]),
+    'dboa_ema_update': (I, [P, P, L, D, P]),
+    'dboa_adam_ema_scaled': (I, [P, P, P, P, P, L, D, D, D, D, I, D, F, P]),
     'dboa_fill_zero': (I, [P, L, P]),
     'dboa_copy_async': (I, [P, P, L, P]),
     'dboa_hmr_backward_buckets': (I, [P, P, P]),

@@ -315,13 +315,13 @@ int dboa_sgd_update(const float* p, const float* g, float* out, float lr, long l
     if (!p || !g || !out || n < 0) return DBOA_ERR_ARG;
     return sgd_update(p, g, out, lr, (size_t)n, ST(stream));
 }
-int dboa_adam_ema(float* p, const float* g, float* m, float* v, float* teacher, long long n, float lr, float beta1, float beta2, float eps,
-                  int step, float alpha, dboa_stream_t stream) {
+int dboa_adam_ema(float* p, const float* g, float* m, float* v, float* teacher, long long n, double lr, double beta1, double beta2,
+                  double eps, int step, double alpha, dboa_stream_t stream) {
     if (!p || !g || !m || !v || n < 0) return DBOA_ERR_ARG;
     return adam_ema(p, g, m, v, teacher, (size_t)n, lr, beta1, beta2, eps, step, alpha, 1.0f, ST(stream));
 }
-int dboa_adam_ema_scaled(float* p, const float* g, float* m, float* v, float* teacher, long long n, float lr, float beta1, float beta2, float eps,
-                         int step, float alpha, float gscale, dboa_stream_t stream) {
+int dboa_adam_ema_scaled(float* p, const float* g, float* m, float* v, float* teacher, long long n, double lr, double beta1, double beta2,
+                         double eps, int step, double alpha, float gscale, dboa_stream_t stream) {
     if (!p || !g || !m || !v || n < 0) return DBOA_ERR_ARG;
     return adam_ema(p, g, m, v, teacher, (size_t)n, lr, beta1, beta2, eps, step, alpha, gscale, ST(stream));
 }
@@ -339,7 +339,7 @@ int dboa_hmr_backward_buckets(void* ev0, void* ev1, void* ev2) {
     return DBOA_OK;
 }
 long long dboa_hmr_bucket_offset(int k) { return hmr_bucket_offset(k); }
-int dboa_ema_update(float* teacher, const float* p, long long n, float alpha, dboa_stream_t stream) {
+int dboa_ema_update(float* teacher, const float* p, long long n, double alpha, dboa_stream_t stream) {
     if (!teacher || !p || n < 0) return DBOA_ERR_ARG;
     return ema_update(teacher, p, (size_t)n, alpha, ST(stream));
 }

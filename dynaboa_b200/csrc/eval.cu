@@ -122,14 +122,40 @@ __global__ void eval_metrics_kernel(const float* __restrict__ scratch, const int
         for (int c = 0; c < 3; ++c) a[r][c] = K[r][c];
     svd3_jacobi(a, V);
     int smallest = 0;
+    double sv_max = 0.0;
     for (int c = 0; c < 3; ++c) {
         sv[c] = sqrt(a[0][c] * a[0][c] + a[1][c] * a[1][c] + a[2][c] * a[2][c]);
         if (sv[c] < sv[smallest]) smallest = c;
+        sv_max = fmax(sv_max, sv[c]);
     }
+    // U = the normalised non-zero columns, completed to an orthonormal basis for every rank of the covariance: a zero
+    // column of U S is any unit vector orthogonal to the others (planar joints give rank 2, collinear ones rank 1,
+    // coincident ones 0), so every entry of U is set before R reads it.  A column counts as zero relative to the largest:
+    // for an exactly rank-deficient covariance the Jacobi sweeps leave rounding residue in the spare columns, as small as
+    // 1e-16 of the largest or down in the range where their squares underflow and the rotations stall, and that residue
+    // points along the real columns, not across them
+    const double zero_sv = 1e-12 * sv_max;
+    int rank = 0, nz = 0;
     for (int c = 0; c < 3; ++c) {
-        if (sv[c] > 1e-200) { for (int r = 0; r < 3; ++r) U[r][c] = a[r][c] / sv[c]; }
+        if (sv[c] > zero_sv) {
+            for (int r = 0; r < 3; ++r) U[r][c] = a[r][c] / sv[c];
+            ++rank;
+            nz = c;
+        } else {
+            for (int r = 0; r < 3; ++r) U[r][c] = r == c ? 1.0 : 0.0;  // rank 0: the identity
+        }
     }
-    if (sv[smallest] <= 1e-200) {                                      // rank-deficient covariance: complete U with a cross product
+    if (rank == 1) {                                                   // Gram-Schmidt of the least aligned axis against column nz
+        const int z = (smallest + 1) % 3 != nz ? (smallest + 1) % 3 : (smallest + 2) % 3;   // the zero column other than smallest
+        int k = 0;
+        for (int r = 1; r < 3; ++r)
+            if (fabs(U[r][nz]) < fabs(U[k][nz])) k = r;
+        double e[3] = {0.0, 0.0, 0.0}, len = 0.0;
+        for (int r = 0; r < 3; ++r) { e[r] = (r == k ? 1.0 : 0.0) - U[k][nz] * U[r][nz]; len += e[r] * e[r]; }
+        len = sqrt(len);
+        for (int r = 0; r < 3; ++r) U[r][z] = e[r] / len;
+    }
+    if (sv[smallest] <= zero_sv) {                                     // rank-deficient covariance: complete U with a cross product
         const int c1 = (smallest + 1) % 3, c2 = (smallest + 2) % 3;
         U[0][smallest] = U[1][c1] * U[2][c2] - U[2][c1] * U[1][c2];
         U[1][smallest] = U[2][c1] * U[0][c2] - U[0][c1] * U[2][c2];

@@ -68,15 +68,15 @@ __global__ void __launch_bounds__(256) adam_ema_kernel(float* __restrict__ p, co
         }
     }
 }
-int adam_ema(float* p, const float* g, float* m, float* v, float* teacher, size_t n, float lr, float beta1, float beta2, float eps,
-             int step, float alpha, float gscale, cudaStream_t st) {
+int adam_ema(float* p, const float* g, float* m, float* v, float* teacher, size_t n, double lr, double beta1, double beta2, double eps,
+             int step, double alpha, float gscale, cudaStream_t st) {
     if (n % 4 || step < 1) return DBOA_ERR_ARG;
-    // torch.optim.Adam (single-tensor path) computes these in Python doubles, then casts the scalars
-    double bc1 = 1.0 - pow((double)beta1, step), bc2 = 1.0 - pow((double)beta2, step);
-    float neg_step = (float)(-((double)lr / bc1)), bc2_sqrt = (float)sqrt(bc2);
-    adam_ema_kernel<<<sweep_grid(n / 4), 256, 0, st>>>(p, g, m, v, teacher, n / 4, (float)(1.0 - (double)beta1), beta2,
-                                                       (float)(1.0 - (double)beta2), bc2_sqrt, eps, neg_step, alpha,
-                                                       (float)(1.0 - (double)alpha), gscale);
+    // torch.optim.Adam (single-tensor path) derives these from the hyperparameters in Python doubles, then casts each
+    // scalar once to fp32: so does this, from the caller's doubles (1 - beta2 of a float-rounded beta2 is off by ulps)
+    const double bc1 = 1.0 - pow(beta1, step), bc2 = 1.0 - pow(beta2, step);
+    adam_ema_kernel<<<sweep_grid(n / 4), 256, 0, st>>>(p, g, m, v, teacher, n / 4, (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2),
+                                                       (float)sqrt(bc2), (float)eps, (float)(-(lr / bc1)), (float)alpha,
+                                                       (float)(1.0 - alpha), gscale);
     return check_launch();
 }
 
@@ -88,9 +88,9 @@ __global__ void __launch_bounds__(256) ema_kernel(float* __restrict__ t, const f
         reinterpret_cast<float4*>(t)[i] = tt;
     }
 }
-int ema_update(float* teacher, const float* p, size_t n, float alpha, cudaStream_t st) {
+int ema_update(float* teacher, const float* p, size_t n, double alpha, cudaStream_t st) {
     if (n % 4) return DBOA_ERR_SHAPE;
-    ema_kernel<<<sweep_grid(n / 4), 256, 0, st>>>(teacher, p, n / 4, alpha, (float)(1.0 - (double)alpha));
+    ema_kernel<<<sweep_grid(n / 4), 256, 0, st>>>(teacher, p, n / 4, (float)alpha, (float)(1.0 - alpha));
     return check_launch();
 }
 

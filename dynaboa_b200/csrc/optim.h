@@ -17,9 +17,9 @@ struct CosinePairs {
 };
 
 int sgd_update(const float* p, const float* g, float* out, float lr, size_t n, cudaStream_t st);
-int adam_ema(float* p, const float* g, float* m, float* v, float* teacher, size_t n, float lr, float beta1, float beta2, float eps, int step,
-             float alpha, float gscale, cudaStream_t st);
-int ema_update(float* teacher, const float* p, size_t n, float alpha, cudaStream_t st);
+int adam_ema(float* p, const float* g, float* m, float* v, float* teacher, size_t n, double lr, double beta1, double beta2, double eps,
+             int step, double alpha, float gscale, cudaStream_t st);
+int ema_update(float* teacher, const float* p, size_t n, double alpha, cudaStream_t st);
 // out[i] = cos(a_i, b_i) (NULL to skip); terms[i] = (a.b, |a|^2, |b|^2) in double (NULL to skip): the data-parallel feature test all-reduces them.
 // Per video g whose bit is set in `active`: out[g][i], terms[g][i], each from video g's parts alone; the rows of other videos
 // are not written.  cp.n / groups / active are checked by the caller (n: total lengths, divisible by groups).

@@ -282,12 +282,15 @@ int dboa_loss_motion_active(const float* p_cur, const float* p_hist, const float
 
 /* ---- whole-model sweeps, feature test, retrieval -------------------------------------------- */
 int dboa_sgd_update(const float* p, const float* g, float* out, float lr, long long n, dboa_stream_t stream);   /* l2l maml_update */
-int dboa_adam_ema(float* p, const float* g, float* m, float* v, float* teacher /* or NULL */, long long n, float lr, float beta1,
-                  float beta2, float eps, int step, float alpha, dboa_stream_t stream);     /* base_adaptor.py:126,193-201 */
-int dboa_ema_update(float* teacher, const float* p, long long n, float alpha, dboa_stream_t stream);
+/* Adam + EMA teacher (base_adaptor.py:126,193-201) with the arithmetic of torch's single-tensor Adam: the fp32 scalars of
+ * the sweep (1 - beta1, beta2, 1 - beta2, the bias corrections, the step size, eps, alpha, 1 - alpha) are derived from
+ * these double hyperparameters and each rounded once, as torch derives them from Python floats */
+int dboa_adam_ema(float* p, const float* g, float* m, float* v, float* teacher /* or NULL */, long long n, double lr, double beta1,
+                  double beta2, double eps, int step, double alpha, dboa_stream_t stream);
+int dboa_ema_update(float* teacher, const float* p, long long n, double alpha, dboa_stream_t stream);
 /* Adam(+EMA) on g * gscale: the data-parallel mean of an all-reduced (summed) gradient without a separate sweep */
-int dboa_adam_ema_scaled(float* p, const float* g, float* m, float* v, float* teacher /* or NULL */, long long n, float lr, float beta1,
-                         float beta2, float eps, int step, float alpha, float gscale, dboa_stream_t stream);
+int dboa_adam_ema_scaled(float* p, const float* g, float* m, float* v, float* teacher /* or NULL */, long long n, double lr, double beta1,
+                         double beta2, double eps, int step, double alpha, float gscale, dboa_stream_t stream);
 /* stream-ordered fill / device-to-device copy on the copy engine (gradient arenas, frame staging: no ATen kernels in a step) */
 int dboa_fill_zero(void* dst, long long bytes, dboa_stream_t stream);
 int dboa_copy_async(void* dst, const void* src, long long bytes, dboa_stream_t stream);
