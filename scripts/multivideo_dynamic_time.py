@@ -15,21 +15,12 @@ Both arms draw the same teacher masks and retrieval seeds per (video, frame).
     python scripts/multivideo_dynamic_time.py [--frames 8] [--warmup 6] [--groups 1 2 4 8] [--out FILE]"""
 import argparse
 import json
-import os
 import random
-import subprocess
 import sys
-import tempfile
 
 import torch
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, REPO)
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name(0)
+from gpu_timing import CARD_FIELDS, asset_dir, card, device_frames, restart, snapshot, timed_window
 
 
 def main():
@@ -42,38 +33,26 @@ def main():
     if not torch.cuda.is_available():
         sys.exit('multivideo_dynamic_time.py needs a GPU')
     from bench import N_EXEMPLARS, WORKLOADS, default_options
-    from dynaboa_b200 import config, synthetic
+    from dynaboa_b200 import config
     from dynaboa_b200.adaptor import Adaptor
     from dynaboa_b200.multivideo import MultiVideoAdaptor
-    work = tempfile.mkdtemp(prefix='dboa_dyn_')
-    synthetic.write_asset_dir(os.path.join(work, 'data'), n_exemplars=N_EXEMPLARS)
-    config.set_data_root(os.path.join(work, 'data'))
+    work = asset_dir('dboa_dyn_', n_exemplars=N_EXEMPLARS)
     n = args.warmup + args.frames
     opts = lambda name: default_options(expdir=work, expname=name, model_file=config.BASE_MODEL, synthetic_frames=n, **WORKLOADS['c5'])
     cap = opts('x').optim_steps
     Gmax = max(args.groups)
-    streams = [synthetic.SyntheticStream(length=n, batch_size=1, rank=g) for g in range(Gmax)]
-    frames = [[{k: v.cuda() if torch.is_tensor(v) else v for k, v in s[t].items()} for t in range(n)] for s in streams]
+    frames = device_frames(Gmax, n)                                           # frames[g][t]
     # teacher keep-masks per (video, frame, teacher forward), made before anything is timed
     gen = torch.Generator().manual_seed(0)
     masks = {(g, t, c): ((torch.rand(3, 2, 1, 1024, generator=gen) >= 0.5).float() * 2.0).cuda()
              for g in range(Gmax) for t in range(n) for c in range(1 + cap)}
     seed = lambda g, t: 7919 * g + t
     info = card()
-    print(f'card (name, power limit): {info}', flush=True)
-
-    def timed(fn, ts):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for t in ts:
-            fn(t)
-        e1.record()
-        e1.synchronize()
-        return e0.elapsed_time(e1)
+    print(f'card ({CARD_FIELDS}): {info}', flush=True)
 
     single = Adaptor(opts('single'))
     single.fused_eval = 'none'
-    snap = (single.model.module.arena.clone(), single.teacher.arena.clone())
+    snap = snapshot(single)
     rows = []
     for G in args.groups:
         # grouped
@@ -96,7 +75,7 @@ def main():
             mv.adapt([frames[g][t] for g in range(G)])
         for t in range(args.warmup):
             pool_step(t)
-        pool_ms = timed(pool_step, range(args.warmup, n))
+        pool_ms = timed_window(pool_step, range(args.warmup, n))
         pool_trips = [rec[args.warmup:] for rec in mv.optim_step_record]
         del mv
         torch.cuda.empty_cache()
@@ -104,10 +83,8 @@ def main():
         seq_ms, seq_trips = 0.0, []
         for g in range(G):
             ad = single
-            ad.model.module.arena.copy_(snap[0])
-            ad.teacher.arena.copy_(snap[1])
-            ad.optimizer.m.zero_(); ad.optimizer.v.zero_(); ad.optimizer.step_count = 0
-            ad.history, ad.optim_step_record, ad.feat_sims = {}, [], {}
+            restart(ad, snap)
+            ad.optim_step_record, ad.feat_sims = [], {}
 
             def one(t, g=g, ad=ad):
                 c = {'i': 0}
@@ -122,7 +99,7 @@ def main():
                 ad.adapt(frames[g][t])
             for t in range(args.warmup):
                 one(t)
-            seq_ms += timed(one, range(args.warmup, n))
+            seq_ms += timed_window(one, range(args.warmup, n))
             seq_trips.append(list(ad.optim_step_record[args.warmup:]))
         F = args.frames
         loops = lambda trips: [[min(x, cap) for x in r] for r in trips]

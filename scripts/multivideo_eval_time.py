@@ -10,31 +10,11 @@ The videos are ``SyntheticStream(rank=g)``, fetched to the device before anythin
     python scripts/multivideo_eval_time.py [--frames 12] [--warmup 3] [--groups 1 4 8 16] [--c5-groups 4] [--out FILE]"""
 import argparse
 import json
-import os
-import subprocess
 import sys
-import tempfile
 
 import torch
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, REPO)
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.sm,clocks.max.sm', '--format=csv,noheader'], capture_output=True,
-                       text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name(0)
-
-
-def timed(fn, n):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for t in range(n):
-        fn(t)
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1)
+from gpu_timing import CARD_FIELDS, asset_dir, card, device_frames, restart, snapshot, timed_window
 
 
 def main():
@@ -48,19 +28,16 @@ def main():
     if not torch.cuda.is_available():
         sys.exit('multivideo_eval_time.py needs a GPU')
     from bench import N_EXEMPLARS, WORKLOADS, default_options
-    from dynaboa_b200 import config, synthetic
+    from dynaboa_b200 import config
     from dynaboa_b200.adaptor import Adaptor
     from dynaboa_b200.multivideo import MultiVideoAdaptor
-    work = tempfile.mkdtemp(prefix='dboa_eval_')
-    synthetic.write_asset_dir(os.path.join(work, 'data'), n_exemplars=N_EXEMPLARS)
-    config.set_data_root(os.path.join(work, 'data'))
+    work = asset_dir('dboa_eval_', n_exemplars=N_EXEMPLARS)
     n = args.warmup + args.frames
     opts = lambda name, w: default_options(expdir=work, expname=name, model_file=config.BASE_MODEL, synthetic_frames=n, **WORKLOADS[w])
     Gmax = max(args.groups + [args.c5_groups])
-    frames = [[{k: v.cuda() if torch.is_tensor(v) else v for k, v in synthetic.SyntheticStream(length=n, batch_size=1, rank=g)[t].items()}
-               for t in range(n)] for g in range(Gmax)]
+    frames = device_frames(Gmax, n)                                           # frames[g][t]
     info = card()
-    print(f'card (name, power limit, SM clock, max SM clock): {info}', flush=True)
+    print(f'card ({CARD_FIELDS}): {info}', flush=True)
     rows = []
 
     def pool_ms(G, mode, w):
@@ -69,7 +46,7 @@ def main():
         step = lambda t: mv.adapt([frames[g][t] for g in range(G)])
         for t in range(args.warmup):
             step(t)
-        ms = timed(lambda t: step(args.warmup + t), args.frames) / args.frames
+        ms = timed_window(step, range(args.warmup, n)) / args.frames
         mv.records(0)
         del mv
         torch.cuda.empty_cache()
@@ -78,19 +55,17 @@ def main():
     def sequential_ms(G):
         ad = Adaptor(opts(f'seq_{G}', 'c2'))
         ad.fused_eval = 'final'
-        snap = (ad.model.module.arena.clone(), ad.teacher.arena.clone())
+        snap = snapshot(ad)
         total = 0.0
         for g in range(G):
-            ad.model.module.arena.copy_(snap[0]); ad.teacher.arena.copy_(snap[1])
-            ad.optimizer.m.zero_(); ad.optimizer.v.zero_(); ad.optimizer.step_count = 0
-            ad.history = {}
+            restart(ad, snap)
 
             def step(t):
                 ad.global_step = t
                 ad.adapt(frames[g][t])
             for t in range(args.warmup):
                 step(t)
-            total += timed(lambda t: step(args.warmup + t), args.frames)
+            total += timed_window(step, range(args.warmup, n))
         del ad
         torch.cuda.empty_cache()
         return total / args.frames

@@ -10,33 +10,13 @@ measurement:
     python scripts/multivideo_pool_time.py [--frames 12] [--warmup 3] [--videos 24] [--seed 0] [--out FILE]"""
 import argparse
 import json
-import os
 import random
-import subprocess
 import sys
-import tempfile
 import time
 
 import torch
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, REPO)
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.sm,clocks.max.sm', '--format=csv,noheader'], capture_output=True,
-                       text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name(0)
-
-
-def timed(fn, n):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for t in range(n):
-        fn(t)
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1)
+from gpu_timing import CARD_FIELDS, asset_dir, card, device_frames, fetch, restart, snapshot, stream, timed_window
 
 
 def main():
@@ -50,23 +30,19 @@ def main():
     if not torch.cuda.is_available():
         sys.exit('multivideo_pool_time.py needs a GPU')
     from bench import WORKLOADS, default_options
-    from dynaboa_b200 import config, synthetic
+    from dynaboa_b200 import config
     from dynaboa_b200.adaptor import Adaptor
     from dynaboa_b200.multivideo import MultiVideoAdaptor
     G = 8
-    work = tempfile.mkdtemp(prefix='dboa_pool_')
-    synthetic.write_asset_dir(os.path.join(work, 'data'))
-    config.set_data_root(os.path.join(work, 'data'))
+    work = asset_dir('dboa_pool_')
     opts = lambda name, n: default_options(expdir=work, expname=name, model_file=config.BASE_MODEL, synthetic_frames=n, **WORKLOADS['c2'])
-    fetch = lambda s, t: {k: v.cuda() if torch.is_tensor(v) else v for k, v in s[t].items()}
     info = card()
-    print(f'card (name, power limit, SM clock, max SM clock): {info}', flush=True)
+    print(f'card ({CARD_FIELDS}): {info}', flush=True)
     rows = []
 
     # (a) occupancy
     n = args.warmup + args.frames
-    streams = [synthetic.SyntheticStream(length=n, batch_size=1, rank=g) for g in range(G)]
-    frames = [[fetch(s, t) for s in streams] for t in range(n)]
+    frames = [list(f) for f in zip(*device_frames(G, n))]                    # frames[t][g]
     ad = Adaptor(opts('single', n))
     ad.fused_eval = 'none'
 
@@ -75,14 +51,14 @@ def main():
         ad.adapt(frames[t][0])
     for t in range(args.warmup):
         single(t)
-    single_ms = timed(lambda t: single(args.warmup + t), args.frames) / args.frames
+    single_ms = timed_window(single, range(args.warmup, n)) / args.frames
     occ = {}
     for k in range(1, G + 1):
         mv = MultiVideoAdaptor(opts(f'occ{k}', n), G)
         step = lambda t: mv.adapt([frames[t][g] if g < k else None for g in range(G)])
         for t in range(args.warmup):
             step(t)
-        occ[k] = timed(lambda t: step(args.warmup + t), args.frames) / args.frames
+        occ[k] = timed_window(step, range(args.warmup, n)) / args.frames
         del mv
         torch.cuda.empty_cache()
     r = {'measurement': 'occupancy', 'workload': 'c2', 'G': G, 'steps': args.frames, 'single_video_ms_per_frame': round(single_ms, 3),
@@ -94,8 +70,8 @@ def main():
     # (b) pool
     rng = random.Random(args.seed)
     lengths = [rng.randint(4, 40) for _ in range(args.videos)]
-    vstreams = [synthetic.SyntheticStream(length=L, batch_size=1, rank=100 + i) for i, L in enumerate(lengths)]
-    vframes = [[fetch(s, t) for t in range(L)] for s, L in zip(vstreams, lengths)]
+    vstreams = [stream(100 + i, L) for i, L in enumerate(lengths)]
+    vframes = [[fetch(s[t]) for t in range(L)] for s, L in zip(vstreams, lengths)]
 
     def pool(mv):
         steps = mv.global_step
@@ -103,12 +79,10 @@ def main():
         return done, mv.global_step - steps
 
     def sequential(ad):
-        snap = (ad.model.module.arena.clone(), ad.teacher.arena.clone())
+        snap = snapshot(ad)
         done = 0
         for v, L in enumerate(lengths):
-            ad.model.module.arena.copy_(snap[0]); ad.teacher.arena.copy_(snap[1])
-            ad.optimizer.m.zero_(); ad.optimizer.v.zero_(); ad.optimizer.step_count = 0
-            ad.history = {}
+            restart(ad, snap)
             for t in range(L):
                 ad.global_step = t
                 ad.adapt(vframes[v][t])

@@ -8,31 +8,11 @@ CUDA events around `frames` frames of every video after `warmup` untimed ones; t
 dropout stays live, as in bench.py's C2 workload."""
 import argparse
 import json
-import os
-import subprocess
 import sys
-import tempfile
 
 import torch
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, REPO)
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'], capture_output=True,
-                       text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name(0)
-
-
-def timed(fn, n):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for t in range(n):
-        fn(t)
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1)
+from gpu_timing import CARD_FIELDS, asset_dir, card, device_frames, timed_window
 
 
 def main():
@@ -45,24 +25,21 @@ def main():
     if not torch.cuda.is_available():
         sys.exit('multivideo_time.py needs a GPU')
     from bench import WORKLOADS, default_options
-    from dynaboa_b200 import config, synthetic
+    from dynaboa_b200 import config
     from dynaboa_b200.adaptor import Adaptor
     from dynaboa_b200.multivideo import MultiVideoAdaptor
-    work = tempfile.mkdtemp(prefix='dboa_mv_')
-    synthetic.write_asset_dir(os.path.join(work, 'data'))
-    config.set_data_root(os.path.join(work, 'data'))
+    work = asset_dir('dboa_mv_')
     n = args.warmup + args.frames
     info = card()
-    print(f'card: {info}', flush=True)
+    print(f'card ({CARD_FIELDS}): {info}', flush=True)
     rows = []
     for G in args.groups:
         opts = lambda g: default_options(expdir=work, expname=f'g{G}_{g}', model_file=config.BASE_MODEL, synthetic_frames=n, **WORKLOADS['c2'])
-        streams = [synthetic.SyntheticStream(length=n, batch_size=1, rank=g) for g in range(G)]
-        frames = [[{k: v.cuda() if torch.is_tensor(v) else v for k, v in s[t].items()} for s in streams] for t in range(n)]
+        frames = [list(f) for f in zip(*device_frames(G, n))]                # frames[t][g]
         mv = MultiVideoAdaptor(opts(0), G)
         for t in range(args.warmup):
             mv.adapt(frames[t])
-        grouped_ms = timed(lambda t: mv.adapt(frames[args.warmup + t]), args.frames)
+        grouped_ms = timed_window(lambda t: mv.adapt(frames[t]), range(args.warmup, n))
         del mv
         torch.cuda.empty_cache()
         singles = []
@@ -77,7 +54,7 @@ def main():
                 ad.adapt(frames[t][g])
         for t in range(args.warmup):
             seq(t)
-        seq_ms = timed(lambda t: seq(args.warmup + t), args.frames)
+        seq_ms = timed_window(seq, range(args.warmup, n))
         del singles
         torch.cuda.empty_cache()
         r = {'G': G, 'workload': 'c2', 'frames_per_video': args.frames,

@@ -14,36 +14,13 @@ joints around a person-sized box, so every stream has a person in view on every 
     python scripts/multiwebcam_time.py [--ticks 20] [--warmup 6] [--groups 1 2 4 8] [--out FILE]"""
 import argparse
 import json
-import os
-import subprocess
 import sys
-import tempfile
 from types import SimpleNamespace
 
 import numpy as np
 import torch
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, REPO)
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.sm,clocks.max.sm', '--format=csv,noheader'], capture_output=True,
-                       text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name(0)
-
-
-def timed(fn, n):
-    """Mean ms of fn(t) over n calls, each between two CUDA events and followed by a device sync."""
-    total = 0.0
-    for t in range(n):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn(t)
-        e1.record()
-        torch.cuda.synchronize()
-        total += e0.elapsed_time(e1)
-    return total / n
+from gpu_timing import CARD_FIELDS, asset_dir, card, timed_each
 
 
 def streams(G, n, seed=0):
@@ -65,11 +42,9 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit('multiwebcam_time.py needs a GPU')
-    from dynaboa_b200 import config, synthetic
+    from dynaboa_b200 import config
     from dynaboa_b200.webcam import MultiWebcamAdaptor, WebcamAdaptor
-    work = tempfile.mkdtemp(prefix='dboa_webcam_')
-    synthetic.write_asset_dir(os.path.join(work, 'data'))
-    config.set_data_root(os.path.join(work, 'data'))
+    work = asset_dir('dboa_webcam_')
     opts = lambda name: SimpleNamespace(expdir=work, expname=name, tensorboard=0, model_file=config.BASE_MODEL, seed=22, lr=3e-6, beta1=0.5,
                                         beta2=0.9, use_boa=1, fastlr=8e-6, s2dloss_weight=10.0, shape_prior_weight=2e-6,
                                         pose_prior_weight=1e-4, use_meanteacher=1, alpha=0.1, teacherloss_weight=0.1, use_motion=1,
@@ -77,15 +52,15 @@ def main():
                                         test_basemodel=0)
     n = args.warmup + args.ticks
     info = card()
-    print(f'card (name, power limit, SM clock, max SM clock): {info}', flush=True)
+    print(f'card ({CARD_FIELDS}): {info}', flush=True)
     rows = []
     for G in args.groups:
         frames, dets = streams(G, n, seed=G)
         mv = MultiWebcamAdaptor(opts(f'pool{G}'), G)
         for t in range(args.warmup):
             mv.online_adaptation(frames[t], dets[t])
-        pool = timed(lambda t: mv.online_adaptation(frames[args.warmup + t], dets[args.warmup + t]), args.ticks)
-        side = timed(lambda t: mv.input_side(frames[args.warmup + t], dets[args.warmup + t]), args.ticks)
+        pool = timed_each(lambda t: mv.online_adaptation(frames[args.warmup + t], dets[args.warmup + t]), args.ticks)
+        side = timed_each(lambda t: mv.input_side(frames[args.warmup + t], dets[args.warmup + t]), args.ticks)
         del mv
         torch.cuda.empty_cache()
         singles = [WebcamAdaptor(opts(f'single{G}_{g}')) for g in range(G)]
@@ -95,12 +70,12 @@ def main():
                 ad.online_adaptation(frames[t][g], dets[t][g])
         for t in range(args.warmup):
             seq(t)
-        sequential = timed(lambda t: seq(args.warmup + t), args.ticks)
+        sequential = timed_each(lambda t: seq(args.warmup + t), args.ticks)
 
         def seq_side(t):
             for g, ad in enumerate(singles):
                 ad.dataprocess(frames[args.warmup + t][g], dets[args.warmup + t][g][0], scaleFactor=1.2)
-        side_seq = timed(seq_side, args.ticks)
+        side_seq = timed_each(seq_side, args.ticks)
         del singles
         torch.cuda.empty_cache()
         r = {'G': G, 'ticks': args.ticks, 'pool_ms_per_tick': round(pool, 2), 'sequential_ms_per_G_frames': round(sequential, 2),

@@ -3,54 +3,21 @@
 A webcam pool tick of G streams draws 2 G meshes: per stream the adapted and the base mesh, each over its own copy of the
 stream's frame.  For G in {1, 2, 4, 8, 16}, frames of 640 x 480, 1280 x 720 and 1920 x 1080, 1 and 4 samples and two meshes
 (the synthetic SMPL mesh posed by an HMR forward of the synthetic base model -- its faces join random vertices, so it is a
-worst case for fill -- and the closed UV sphere of tests/test_gpu_render.py), the two ways are alternated in one process
+worst case for fill -- and the closed UV sphere of tests/harness.py), the two ways are alternated in one process
 after warm-up.  Each round is timed with CUDA events and with the host clock, both from the first launch to the end of the
-last kernel; the medians over the rounds are printed with the card's name and power limit.
+last kernel; the medians over the rounds are printed with the card (name, power limit, SM clocks).
 
     python scripts/render_groups_time.py [--rounds 15] [--sizes 640x480,1280x720,1920x1080] [--streams 1,2,4,8,16]
 """
 import argparse
 import json
-import os
-import subprocess
-import sys
-import tempfile
-import time
 
 import numpy as np
 import torch
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, REPO)
-sys.path.insert(0, os.path.join(REPO, 'tests'))
-from dynaboa_b200 import config, render, synthetic  # noqa: E402
-from dynaboa_b200.hmr import hmr  # noqa: E402
-from dynaboa_b200.smpl import SMPL  # noqa: E402
-from test_gpu_render import sphere  # noqa: E402
-
-
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader', '-i', '0'], capture_output=True,
-                           text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        q = ''
-    return q or torch.cuda.get_device_name(0)
-
-
-def posed_smpl():
-    work = tempfile.mkdtemp(prefix='dboa_render_groups_time_')
-    synthetic.write_asset_dir(os.path.join(work, 'data'))
-    config.set_data_root(os.path.join(work, 'data'))
-    m = hmr(synthetic.make_mean_params()).cuda()
-    m.load_state_dict({k.replace('module.', ''): v for k, v in synthetic.make_basemodel()['model'].items()}, strict=True)
-    m.eval()
-    x = torch.randn(1, 3, 224, 224, generator=torch.Generator().manual_seed(7)).cuda()
-    with torch.no_grad():
-        rot, shape, _ = m(x)
-        verts = SMPL(config.SMPL_MODEL_DIR, create_transl=False).cuda()(
-            betas=shape, body_pose=rot[:, 1:], global_orient=rot[:, 0].unsqueeze(1), pose2rot=False).vertices[0].contiguous()
-    return verts, render.get_smpl_faces()
+from gpu_timing import asset_dir, card, posed_smpl_mesh, timed_once
+from dynaboa_b200 import render  # noqa: E402  (importable once gpu_timing has put the repository on sys.path)
+from harness import sphere  # noqa: E402
 
 
 def tick(G, W, H, verts, seed):
@@ -70,17 +37,6 @@ def tick(G, W, H, verts, seed):
     return imgs, vs, cams, cols
 
 
-def timed(fn):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    e0.record()
-    fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1), (time.perf_counter() - t0) * 1e3
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--rounds', type=int, default=15)
@@ -89,7 +45,8 @@ def main():
     args = ap.parse_args()
     assert torch.cuda.is_available(), 'render_groups_time.py needs a GPU'
     sv, sf = sphere()
-    meshes = {'smpl': posed_smpl(), 'sphere': (torch.from_numpy(sv).cuda(), sf)}
+    asset_dir('dboa_render_groups_time_')
+    meshes = {'smpl': posed_smpl_mesh()[:2], 'sphere': (torch.from_numpy(sv).cuda(), sf)}
     name = card()
     sizes = [tuple(int(x) for x in s.split('x')) for s in args.sizes.split(',')]
     for mesh, (verts, faces) in meshes.items():
@@ -110,8 +67,8 @@ def main():
                         grouped()
                     t_single, t_group = [], []
                     for _ in range(args.rounds):
-                        t_single.append(timed(singles))
-                        t_group.append(timed(grouped))
+                        t_single.append(timed_once(singles))
+                        t_group.append(timed_once(grouped))
                     s_ev, s_wall = np.median([t[0] for t in t_single]), np.median([t[1] for t in t_single])
                     g_ev, g_wall = np.median([t[0] for t in t_group]), np.median([t[1] for t in t_group])
                     print(json.dumps({'card': name, 'mesh': mesh, 'W': W, 'H': H, 'samples': samples, 'streams': G, 'meshes': 2 * G,

@@ -1,31 +1,22 @@
 """End-to-end bilevel adaptation on the GPU against trajectories recorded from the reference's own
 ``BaseAdaptor`` / ``Adaptor`` code (tests/golden/adapt_*.npz, see oracle/make_golden.py): configs C2
 (1 inner step), C3 (3 inner steps + retrieval minibatch) and C5 (dynamic re-adaptation loop)."""
-import ast
 import os
 import random
-from types import SimpleNamespace
 
 import numpy as np
 import pytest
 import torch
 
 from conftest import rel_err
+from harness import adapt_options, fetch
 
 pytestmark = pytest.mark.gpu
 
 
-def make_options(tmp, golden_options_repr, **extra):
-    o = dict(ast.literal_eval(golden_options_repr))
-    o.update(expdir=str(tmp), expname='run', tensorboard=0, synthetic_frames=8, cache_results=0)
-    o.update(extra)
-    return SimpleNamespace(**o)
-
-
 def build_adaptor(asset_dir, tmp, gd):
-    from dynaboa_b200 import config
     from dynaboa_b200.adaptor import Adaptor
-    opts = make_options(tmp, str(gd['options']), model_file=config.BASE_MODEL)
+    opts = adapt_options(tmp, gd)
     return Adaptor(opts), opts
 
 
@@ -40,7 +31,7 @@ def run_and_compare(asset_dir, tmp_path, golden, tag, fused):
     masks_all = torch.from_numpy(gd['teacher_masks']).float()
     n_outer = 0
     for t in range(n_frames):
-        batch = {k: v.cuda() if torch.is_tensor(v) else v for k, v in stream[t].items()}
+        batch = fetch(stream[t])
         random.seed(1000 + t)
         calls = {'i': 0}
 
@@ -133,7 +124,7 @@ def test_output_forward_on_side_stream_is_equivalent(asset_dir, tmp_path, golden
         stream = synthetic.SyntheticStream(length=6, batch_size=opts.batch_size)
         outs = []
         for t in range(6):
-            batch = {k: v.cuda() if torch.is_tensor(v) else v for k, v in stream[t].items()}
+            batch = fetch(stream[t])
             ad.global_step, ad.fit_losses = t, {}
             ad.adapt(batch)
             if overlap:

@@ -19,6 +19,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from harness import FWD_TOL, GRAD_L2, GRAD_TOL, nchw, rel, structure
+
 pytestmark = pytest.mark.gpu
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -30,16 +32,6 @@ CONFIGS = ([DEFAULT + (B,) for B in (1, 2, 3, 8, 9, 17, 22, 64)]
                                  ('fused_fwd', 3, 1, 0, False), ('fused_bwd', 3, 0, 1, False)) for B in (1, 9, 64)]
            + [('masked', 3, 0, 0, True, B) for B in (1, 9)])
 IDS = [f'{c[0]}-B{c[5]}' for c in CONFIGS]
-
-# Forward bounds, each relative to the largest value of the layer's fp64 result ('stats': mean error in units of the
-# group's standard deviation, and relative rstd error).  Worst measured over CONFIGS on an H100 80GB HBM3 (400 W):
-# y 2.8e-6 (CUDA-core convs, B = 64), stats 1.9e-7, a 2.4e-7, head 3.4e-7, rotmat 6.1e-7.
-FWD_TOL = {'y': 6e-6, 'stats': 5e-7, 'a': 6e-7, 'head': 1e-6, 'out': 2e-6}
-# Backward: max |g - ref| <= GRAD_TOL * max |ref| for every one of the 169 tensors, and whole-arena relative L2 below
-# GRAD_L2.  Worst measured: 1.6e-5 per tensor (tensor-core mode 1, B = 64) and 2.0e-6 relative L2 (dropout, B = 9).
-GRAD_TOL = 5e-5
-GRAD_L2 = 1e-5
-
 
 @pytest.fixture(scope='module')
 def model():
@@ -54,17 +46,6 @@ def model():
     lib.dboa_set_tensor_core_conv(3)          # library defaults: later test modules must not inherit this module's modes
     lib.dboa_set_fused_forward(0)
     lib.dboa_set_fused_backward(0)
-
-
-def structure():
-    """Convolution geometry plus the bottleneck blocks as (c1, c2, c3, downsample or None) conv indices."""
-    from dynaboa_b200.hmr import conv_geometry
-    geo = conv_geometry()
-    blocks = []
-    for i, g in enumerate(geo):
-        if g[0].endswith('.conv1'):
-            blocks.append([i, i + 1, i + 2, i + 3 if i + 3 < len(geo) and 'downsample' in geo[i + 3][0] else None])
-    return geo, blocks
 
 
 def run_forward(m, cfg):
@@ -84,10 +65,6 @@ def run_forward(m, cfg):
     return x, masks, tape, (rot, shape, cam)
 
 
-def nchw(t):
-    return t.permute(0, 3, 1, 2).double()
-
-
 def gn_stats(y):
     v = y.reshape(y.shape[0], 4, -1)
     return v.mean(-1), (v.var(-1, unbiased=False) + 1e-5).rsqrt()
@@ -97,11 +74,6 @@ def gn_apply(y, mean, rstd, gamma, beta):
     B, C = y.shape[:2]
     v = ((y.reshape(B, 4, -1) - mean[..., None]) * rstd[..., None]).reshape(y.shape)
     return v * gamma.double().view(1, C, 1, 1) + beta.double().view(1, C, 1, 1)
-
-
-def rel(a, ref, scale=None):
-    s = ref.abs().max() if scale is None else scale
-    return float((a.double() - ref).abs().max() / s.clamp_min(1e-30))
 
 
 @pytest.mark.parametrize('cfg', CONFIGS, ids=IDS)

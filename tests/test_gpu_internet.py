@@ -12,32 +12,10 @@ import pytest
 import torch
 
 from conftest import rel_err
-from oracle import ref_harness
+from harness import DRIVER, FLAGS, N, SHADOWED, make_video
 
 pytestmark = pytest.mark.gpu
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DRIVER = os.path.join(ref_harness.REF or '', 'dynaboa_internet.py')
-SHADOWED = ('constants', 'config', 'model', 'utils', 'base_adaptor', 'boa_dataset', 'learn2learn')
-FLAGS = dict(inner_step=1, retrieval=0, lower_level_mixtrain=0, upper_level_mixtrain=0, dynamic_boa=0)
-N = 3
-
-
-def make_video(root):
-    """N frames 240 x 320 (smooth content, moving box), 49 keypoints projected inside the box, reference npz layout."""
-    import cv2
-    os.makedirs(os.path.join(root, 'images'), exist_ok=True)
-    rng = np.random.default_rng(11)
-    base = cv2.GaussianBlur(rng.uniform(0, 255, size=(240, 320, 3)).astype(np.float32), (0, 0), 3)
-    names, centers, scales, parts, frames = [], [], [], [], []
-    for t in range(N):
-        frame = np.clip(np.roll(base, 3 * t, axis=1) + rng.normal(0, 2, base.shape), 0, 255).astype(np.uint8)
-        name = f'f{t:03d}.png'
-        cv2.imwrite(os.path.join(root, 'images', name), frame[:, :, ::-1])
-        center, scale = np.array([150.0 + 4 * t, 118.0 + t]), 0.9 + 0.01 * t
-        kp = np.concatenate([center + rng.uniform(-70, 70, size=(49, 2)), np.ones((49, 1))], 1)
-        names.append(name); centers.append(center); scales.append(scale); parts.append(kp); frames.append(frame)
-    np.savez(os.path.join(root, 'video.npz'), imgname=np.array(names), center=np.stack(centers), scale=np.array(scales), part=np.stack(parts))
-    return frames, centers, scales, parts
 
 
 def oracle_trajectory(frames, centers, scales, parts, masks):

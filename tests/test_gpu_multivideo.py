@@ -10,7 +10,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from test_gpu_hmr_layers import FWD_TOL, GRAD_TOL, nchw, rel, structure
+from harness import FWD_TOL, GRAD_TOL, hmr_model, inputs, nchw, rel, stacked, structure
 
 pytestmark = pytest.mark.gpu
 
@@ -22,31 +22,7 @@ IDS = [f'G{g}-b{b}-tc{m}' + ('-masked' if k else '') for g, b, m, k in CONFIGS]
 
 @pytest.fixture(scope='module')
 def model():
-    from dynaboa_b200 import _lib, synthetic
-    from dynaboa_b200.hmr import hmr
-    from oracle import hmr_ref
-    lib = _lib.load()
-    m = hmr(synthetic.make_mean_params()).cuda()
-    m.load_state_dict(hmr_ref.strip_prefix(synthetic.make_basemodel()['model']), strict=True)
-    m.eval()
-    prev = lib.dboa_get_fused_forward(), lib.dboa_get_fused_backward()
-    lib.dboa_set_fused_forward(0)
-    lib.dboa_set_fused_backward(0)
-    yield m
-    lib.dboa_set_tensor_core_conv(3)          # library default: later test modules must not inherit this module's mode
-    lib.dboa_set_fused_forward(prev[0])
-    lib.dboa_set_fused_backward(prev[1])
-
-
-def stacked(m, G, seed):
-    """(G, P) arena stack: video g's weights are the checkpoint's scaled element-wise by 1 + 0.05 N(0, 1) (seeded per video;
-    the zero padding of the arena stays zero)."""
-    P = m.arena.numel()
-    out = torch.empty(G, P, device='cuda')
-    for g in range(G):
-        gen = torch.Generator(device='cuda').manual_seed(seed + g)
-        out[g] = m.arena * (1 + 0.05 * torch.randn(P, generator=gen, device='cuda'))
-    return out
+    yield from hmr_model()
 
 
 def run(m, arenas, x, masks, d, groups):
@@ -58,14 +34,6 @@ def run(m, arenas, x, masks, d, groups):
     raw_backward(arenas, tape, B, masks is not None, d[0], d[1], d[2], grad, groups=groups)
     torch.cuda.synchronize()
     return (rot, shape, cam), tape, grad
-
-
-def inputs(B, seed, masked):
-    g = torch.Generator().manual_seed(seed)
-    x = torch.randn(B, 3, 224, 224, generator=g).cuda()
-    masks = (torch.rand(3, 2, B, 1024, generator=g) >= 0.5).float().cuda() * 2 if masked else None
-    d = [torch.randn(B, 24, 3, 3, generator=g).cuda(), torch.randn(B, 10, generator=g).cuda(), torch.randn(B, 3, generator=g).cuda()]
-    return x, masks, d
 
 
 @pytest.mark.parametrize('cfg', CONFIGS, ids=IDS)

@@ -9,25 +9,16 @@
   of its single-video run.
 - Schedule invariance with the loop, and two runs bit for bit."""
 import ctypes as C
-import random
 
 import pytest
 import torch
 
 from conftest import rel_err
-from test_gpu_adapt import make_options
-from test_gpu_multivideo_adapt import masks_for, seed_for
-from test_gpu_multivideo_pool import video_masks
+from harness import MIXED_THRESHOLD, N_FRAMES, PoolRun, SingleRun, bits, masks_for, pool_options, seed_for, stream
 
 pytestmark = pytest.mark.gpu
 COS_CHUNK = 256 * 16
 SENTINEL = 0x7ff8dead0000beef                  # a NaN payload no kernel writes
-# cos_sim_threshold for videos 0..3 (SyntheticStream(rank=g), video_masks, seeds 7919 g + t) at adapt_c5.npz's options over 8
-# frames, calibrated once on an H100 80GB HBM3: the single-video loops run different numbers of iterations in frames 1 and 2
-# (trip counts [1, 1, 2, 1] and [0, 0, 0, 3]), and the closest of all 1 - cos12 decisions lies 2.1 % from it.
-# test_mixed_trip_counts_follow_the_single_video_runs checks both.
-MIXED_THRESHOLD = 7e-5
-N_FRAMES = 8
 
 
 # ------------------------------------------------------------------ kernel
@@ -72,10 +63,6 @@ def sums(a, b, n, groups=None, active=None):
     return terms
 
 
-def bits(t):
-    return t.contiguous().view(torch.int64)
-
-
 @pytest.mark.parametrize('kind', ['features', 'odd'])
 @pytest.mark.parametrize('G', [1, 2, 4, 8])
 def test_each_video_is_the_one_video_call_on_its_parts(G, kind):
@@ -113,87 +100,11 @@ def test_each_video_is_the_one_video_call_on_its_parts(G, kind):
 
 
 # ------------------------------------------------------------------ adaptor
-class Videos:
-    """A MultiVideoAdaptor with the dynamic loop whose slots carry (video id, stream, own frame); teacher masks
-    ``masks(vid, t, call)`` and retrieval seeds ``seed(vid, t)`` follow the video."""
-
-    def __init__(self, opts, G, masks=video_masks, seed=lambda vid, t: 7919 * vid + t):
-        from dynaboa_b200.multivideo import MultiVideoAdaptor
-        self.mv = MultiVideoAdaptor(opts, G, dynamic_loop=True)
-        self.masks, self.seed = masks, seed
-        self.slot, self.calls = [None] * G, [0] * G
-        self.mv.mask_provider = self.provider
-
-    def provider(self, g, B, dev):
-        vid, _, t = self.slot[g]
-        m = self.masks(vid, t, self.calls[g])
-        self.calls[g] += 1
-        return m.to(dev)
-
-    def start(self, g, vid, stream):
-        self.mv.start(g)
-        self.slot[g] = [vid, stream, 0]
-
-    def step(self, run):
-        """One pool frame: the slots in `run` advance by one frame of their video.  Returns {slot: (vid, own frame, batch)}."""
-        batches, done = [None] * self.mv.G, {}
-        for g in run:
-            vid, s, t = self.slot[g]
-            batches[g] = {k: v.cuda() if torch.is_tensor(v) else v for k, v in s[t].items()}
-            self.calls[g] = 0
-            self.mv.rngs[g].seed(self.seed(vid, t))
-            done[g] = (vid, t, batches[g])
-        self.mv.adapt(batches)
-        for g in run:
-            self.slot[g][2] += 1
-        return done
-
-    def state(self, g):
-        mv = self.mv
-        return [mv.thetas[g].clone(), mv.teachers[g].clone(), mv.m[g].clone(), mv.v[g].clone()]
-
-
-class Single:
-    """``Adaptor.adapt`` of one video with the same teacher masks and retrieval seeds."""
-
-    def __init__(self, opts, vid, masks=video_masks, seed=lambda vid, t: 7919 * vid + t):
-        from dynaboa_b200.adaptor import Adaptor
-        self.ad = Adaptor(opts)
-        self.ad.fused_eval = 'none'
-        self.vid, self.masks, self.seed = vid, masks, seed
-
-    def step(self, t, batch):
-        calls, ad = {'i': 0}, self.ad
-
-        def provider(B, dev):
-            m = self.masks(self.vid, t, calls['i'])
-            calls['i'] += 1
-            return m.to(dev)
-        ad.teacher.mask_provider = provider
-        random.seed(self.seed(self.vid, t))
-        ad.global_step, ad.fit_losses = t, {}
-        ad.model.eval()
-        ad.adapt(batch)
-
-
-def c5_options(tmp, golden, name, threshold=None):
-    from dynaboa_b200 import config
-    o = make_options(tmp / name, str(golden('adapt_c5')['options']), model_file=config.BASE_MODEL)
-    assert o.dynamic_boa
-    if threshold is not None:
-        o.cos_sim_threshold = threshold
-    return o
-
-
-def stream(vid, n):
-    from dynaboa_b200 import synthetic
-    return synthetic.SyntheticStream(length=n, batch_size=1, rank=vid)
-
-
 @pytest.mark.parametrize('threshold', [None, MIXED_THRESHOLD], ids=['golden', 'mixed'])
 def test_one_video_is_the_single_video_loop(asset_dir, tmp_path, golden, threshold):
-    p = Videos(c5_options(tmp_path, golden, 'mv', threshold), 1)
-    s = Single(c5_options(tmp_path, golden, 'ad', threshold), 0)
+    extra = {} if threshold is None else {'cos_sim_threshold': threshold}
+    p = PoolRun(pool_options(tmp_path, golden, 'c5', 'mv', **extra), 1, dynamic_loop=True)
+    s = SingleRun(pool_options(tmp_path, golden, 'c5', 'ad', **extra), 0)
     p.start(0, 0, stream(0, N_FRAMES))
     for t in range(N_FRAMES):
         batch = p.step([0])[0][2]
@@ -233,9 +144,9 @@ def test_golden_c5_videos_follow_their_trajectories(asset_dir, tmp_path, golden)
     from oracle.make_golden import sample_indices
     gd = golden('adapt_c5')
     masks = lambda vid, t, call: masks_for(vid, t, call, gd)
-    p = Videos(c5_options(tmp_path, golden, 'mv'), 4, masks=masks, seed=seed_for)
+    p = PoolRun(pool_options(tmp_path, golden, 'c5', 'mv'), 4, dynamic_loop=True, masks=masks, seed=seed_for)
     o = p.mv.options
-    singles = {g: Single(c5_options(tmp_path, golden, f'v{g}'), g, masks=masks, seed=seed_for) for g in range(1, 4)}
+    singles = {g: SingleRun(pool_options(tmp_path, golden, 'c5', f'v{g}'), g, masks=masks, seed=seed_for) for g in range(1, 4)}
     n_frames = gd['upper_loss'].shape[0]
     for g in range(4):
         p.start(g, g, stream(g, n_frames))
@@ -272,9 +183,9 @@ def test_mixed_trip_counts_follow_the_single_video_runs(asset_dir, tmp_path, gol
     """G = 4 over 8 frames (the motion term goes live) at MIXED_THRESHOLD: each video takes exactly the trip counts of its
     single-video run, and its theta stays within 4 lr n_outer of it, n_outer counting that video's own Adam steps."""
     thr = MIXED_THRESHOLD
-    p = Videos(c5_options(tmp_path, golden, 'mv', thr), 4)
+    p = PoolRun(pool_options(tmp_path, golden, 'c5', 'mv', cos_sim_threshold=thr), 4, dynamic_loop=True)
     o = p.mv.options
-    singles = {g: Single(c5_options(tmp_path, golden, f'v{g}', thr), g) for g in range(4)}
+    singles = {g: SingleRun(pool_options(tmp_path, golden, 'c5', f'v{g}', cos_sim_threshold=thr), g) for g in range(4)}
     for g in range(4):
         p.start(g, g, stream(g, N_FRAMES))
     n_outer, mixed = [0] * 4, []
@@ -300,7 +211,7 @@ def test_a_looping_video_does_not_depend_on_its_slot_or_schedule(asset_dir, tmp_
     their own trip counts: theta, teacher, m, v, upper loss, trip counts and cosines bit for bit.  A slot that sits a frame out
     keeps its arenas bit for bit."""
     X, thr = 5, MIXED_THRESHOLD
-    a = Videos(c5_options(tmp_path, golden, 'a', thr), 4)
+    a = PoolRun(pool_options(tmp_path, golden, 'c5', 'a', cos_sim_threshold=thr), 4, dynamic_loop=True)
     a.start(0, X, stream(X, N_FRAMES))
     traj_a = []
     for _ in range(N_FRAMES):
@@ -308,7 +219,7 @@ def test_a_looping_video_does_not_depend_on_its_slot_or_schedule(asset_dir, tmp_
         traj_a.append(a.state(0) + [a.mv.last_upper_loss[0].clone()])
     rec_a = (list(a.mv.optim_step_record[0]), dict(a.mv.feat_sims[0]))
     del a
-    b = Videos(c5_options(tmp_path, golden, 'b', thr), 4)
+    b = PoolRun(pool_options(tmp_path, golden, 'c5', 'b', cos_sim_threshold=thr), 4, dynamic_loop=True)
     total = N_FRAMES + 3
     b.start(0, 11, stream(11, total))
     b.start(1, 12, stream(12, total))
@@ -347,7 +258,7 @@ def test_a_looping_video_does_not_depend_on_its_slot_or_schedule(asset_dir, tmp_
 def test_two_runs_are_bit_identical(asset_dir, tmp_path, golden):
     runs = []
     for r in range(2):
-        p = Videos(c5_options(tmp_path, golden, f'r{r}', MIXED_THRESHOLD), 4)
+        p = PoolRun(pool_options(tmp_path, golden, 'c5', f'r{r}', cos_sim_threshold=MIXED_THRESHOLD), 4, dynamic_loop=True)
         for g in range(4):
             p.start(g, g, stream(g, 4))
         for _ in range(4):

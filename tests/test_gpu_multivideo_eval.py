@@ -20,8 +20,7 @@ import pytest
 import torch
 
 from conftest import rel_err
-from test_gpu_multivideo_dynamic import MIXED_THRESHOLD, N_FRAMES, Single, Videos, c5_options, stream
-from test_gpu_multivideo_pool import Pool, options, video_masks
+from harness import MIXED_THRESHOLD, N_FRAMES, PoolRun, SingleRun, bits, fetch, pool_options, stream, video_masks
 
 pytestmark = pytest.mark.gpu
 SENTINEL = 0x7fc0dead                  # a NaN payload no kernel writes
@@ -52,10 +51,6 @@ def meshes(B, seed):
     pred = (gt * 1.1 + rng.randn(B, NV, 3) * 0.08).astype(np.float32)
     gtn = (gt + rng.randn(B, NV, 3) * 0.02).astype(np.float32)
     return [torch.from_numpy(t).cuda() for t in (pred, gt, gtn, J)]
-
-
-def bits(t):
-    return t.contiguous().view(torch.int32)
 
 
 @pytest.mark.parametrize('b', [1, 2])
@@ -161,18 +156,19 @@ def counts(x):
     return None
 
 
+def options_for(workload, tmp, golden, name):
+    extra = {} if workload == 'c2' else {'cos_sim_threshold': MIXED_THRESHOLD}
+    return pool_options(tmp, golden, workload, name, **extra)
+
+
 def pool_for(workload, tmp, golden, name, G, mode):
-    if workload == 'c2':
-        p = Pool(options(tmp, golden, 'c2', name), G)
-    else:
-        p = Videos(c5_options(tmp, golden, name, MIXED_THRESHOLD), G)
+    p = PoolRun(options_for(workload, tmp, golden, name), G, dynamic_loop=(workload == 'c5'))
     p.mv.fused_eval = mode
     return p
 
 
 def single_for(workload, tmp, golden, name, vid, mode):
-    o = options(tmp, golden, 'c2', name) if workload == 'c2' else c5_options(tmp, golden, name, MIXED_THRESHOLD)
-    s = Single(o, vid)
+    s = SingleRun(options_for(workload, tmp, golden, name), vid)
     s.ad.fused_eval = mode
     return s
 
@@ -322,11 +318,11 @@ def test_run_gives_each_video_its_own_results(asset_dir, tmp_path, golden):
     from dynaboa_b200.adaptor import RESULT_FILES, Adaptor
     videos = [synthetic.SyntheticStream(length=n, batch_size=1, rank=v) for v, n in enumerate(LENGTHS)]
     names = [f'video{v}' for v in range(len(LENGTHS))]
-    mv = runner(options(tmp_path, golden, 'c2', 'pool'))
+    mv = runner(pool_options(tmp_path, golden, 'c2', 'pool'))
     out = mv.run(videos, exppath=str(tmp_path / 'pool'), names=names)
     assert [s['name'] for s in out] == names and [s['frames'] for s in out] == LENGTHS
     assert mv.slot_video == [None] * 4
-    alone = runner(options(tmp_path, golden, 'c2', 'alone'))
+    alone = runner(pool_options(tmp_path, golden, 'c2', 'alone'))
     empty = synthetic.SyntheticStream(length=0, batch_size=1)
     for v, n in enumerate(LENGTHS):
         # video v at index v of the queue (so its seed and masks are those of the pool run), behind empty videos
@@ -338,7 +334,7 @@ def test_run_gives_each_video_its_own_results(asset_dir, tmp_path, golden):
                 assert x.read() == y.read(), (v, f)
         assert not any((tmp_path / 'alone' / f'e{i}').exists() for i in range(v))
     for v in (1, 2):                                  # lengths 8 and 2: the single-video driver's files on a video that long
-        o = options(tmp_path, golden, 'c2', f'excute{v}')
+        o = pool_options(tmp_path, golden, 'c2', f'excute{v}')
         o.synthetic_frames = LENGTHS[v]
         ad = Adaptor(o)
         ad.fused_eval = 'final'
@@ -380,7 +376,7 @@ def test_evaluation_adds_no_host_synchronisation(asset_dir, tmp_path, golden):
     masks = {(g, t): video_masks(g, t, 0).cuda() for g in range(4) for t in range(n)}
     p.mv.mask_provider = lambda g, B, dev: masks[(g, p.mv.video_steps[g])]
     for g in range(4):
-        p.start(g, g, [{k: v.cuda() if torch.is_tensor(v) else v for k, v in f.items()} for f in stream(g, n)])
+        p.start(g, g, [fetch(f) for f in stream(g, n)])
     for _ in range(warm):
         p.step(range(4))
     torch.cuda.synchronize()

@@ -16,8 +16,7 @@ import pytest
 import torch
 
 from conftest import rel_err
-from test_gpu_adapt import make_options
-from test_gpu_multivideo import inputs, model, stacked      # noqa: F401  (model is a fixture)
+from harness import PoolRun, SingleRun, bits, hmr_model, inputs, pool_options, stacked, stream
 
 pytestmark = pytest.mark.gpu
 
@@ -29,8 +28,9 @@ IDS = [f'G{g}-b{b}-tc{m}' + ('-masked' if k else '') + f'-{a if isinstance(a, st
 SENTINEL = 0x7fc0dead                  # a NaN payload no kernel writes
 
 
-def bits(t):
-    return t.contiguous().view(torch.int32) if t.dtype == torch.float32 else t.contiguous()
+@pytest.fixture(scope='module')
+def model():
+    yield from hmr_model()
 
 
 def call(m, arenas, x, masks, d, G, active, tape_fill, grad):
@@ -133,66 +133,11 @@ def test_motion_mask():
 
 
 # ------------------------------------------------------------------ adaptor
-def video_masks(vid, t, call):
-    """Teacher keep-masks of video `vid`, its own frame t, teacher forward `call`."""
-    gen = torch.Generator().manual_seed(1000003 * vid + 1009 * t + call)
-    return (torch.rand(3, 2, 1, 1024, generator=gen) >= 0.5).float() * 2.0
-
-
-class Pool:
-    """A MultiVideoAdaptor whose slots carry (video id, stream, own frame); teacher masks and retrieval seeds follow the video."""
-
-    def __init__(self, opts, G):
-        from dynaboa_b200.multivideo import MultiVideoAdaptor
-        self.mv = MultiVideoAdaptor(opts, G)
-        self.slot = [None] * G
-        self.calls = [0] * G
-        self.mv.mask_provider = self.provider
-
-    def provider(self, g, B, dev):
-        vid, _, t = self.slot[g]
-        m = video_masks(vid, t, self.calls[g])
-        self.calls[g] += 1
-        return m.to(dev)
-
-    def start(self, g, vid, stream):
-        self.mv.start(g)
-        self.slot[g] = [vid, stream, 0]
-
-    def step(self, run):
-        """One pool frame: the slots in `run` advance by one frame of their video.  Returns {slot: (vid, own frame, batch)}."""
-        batches, done = [None] * self.mv.G, {}
-        for g in run:
-            vid, s, t = self.slot[g]
-            batches[g] = {k: v.cuda() if torch.is_tensor(v) else v for k, v in s[t].items()}
-            self.calls[g] = 0
-            self.mv.rngs[g].seed(7919 * vid + t)
-            done[g] = (vid, t, batches[g])
-        self.mv.adapt(batches)
-        for g in run:
-            self.slot[g][2] += 1
-        return done
-
-    def state(self, g):
-        mv = self.mv
-        return [mv.thetas[g].clone(), mv.teachers[g].clone(), mv.m[g].clone(), mv.v[g].clone()]
-
-
-def options(tmp, golden, tag, name):
-    from dynaboa_b200 import config
-    gd = golden(f'adapt_{tag}')
-    o = make_options(tmp / name, str(gd['options']), model_file=config.BASE_MODEL)
-    assert not o.dynamic_boa
-    return o
-
-
 @pytest.mark.parametrize('tag,n_frames', [('c2', 8), ('c3', 2)])
 def test_a_video_does_not_depend_on_its_slot_or_schedule(asset_dir, tmp_path, golden, tag, n_frames):
-    from dynaboa_b200 import synthetic
     X = 5
-    stream = lambda vid, n: synthetic.SyntheticStream(length=n, batch_size=1, rank=vid)
     # A: X alone in slot 0 from pool frame 0
-    a = Pool(options(tmp_path, golden, tag, 'a'), 4)
+    a = PoolRun(pool_options(tmp_path, golden, tag, 'a'), 4)
     a.start(0, X, stream(X, n_frames))
     traj_a = []
     for _ in range(n_frames):
@@ -201,7 +146,7 @@ def test_a_video_does_not_depend_on_its_slot_or_schedule(asset_dir, tmp_path, go
     del a
     # B: X in slot 2 from pool frame 3; slot 0 runs one long video, slot 1 pauses, slot 2 first runs a 3-frame video, slot 3
     # finishes a 2-frame video and is refilled at pool frame 4
-    b = Pool(options(tmp_path, golden, tag, 'b'), 4)
+    b = PoolRun(pool_options(tmp_path, golden, tag, 'b'), 4)
     total = n_frames + 3
     b.start(0, 11, stream(11, total))
     b.start(1, 12, stream(12, total))
@@ -231,16 +176,14 @@ def test_a_video_does_not_depend_on_its_slot_or_schedule(asset_dir, tmp_path, go
 
 
 def test_every_pool_video_follows_its_own_single_video_run(asset_dir, tmp_path, golden):
-    from dynaboa_b200 import synthetic
-    from dynaboa_b200.adaptor import Adaptor
     lengths = [3, 8, 2, 5, 6, 4]                     # videos 0..5 through 4 slots, each slot refilled when its video ends
-    p = Pool(options(tmp_path, golden, 'c2', 'pool'), 4)
+    p = PoolRun(pool_options(tmp_path, golden, 'c2', 'pool'), 4)
     o = p.mv.options
     queue = list(range(len(lengths)))
     singles, frames = {}, {}
     for g in range(4):
         vid = queue.pop(0)
-        p.start(g, vid, synthetic.SyntheticStream(length=lengths[vid], batch_size=1, rank=vid))
+        p.start(g, vid, stream(vid, lengths[vid]))
     seen = set()
     while True:
         for g in range(4):                           # refill finished slots
@@ -248,7 +191,7 @@ def test_every_pool_video_follows_its_own_single_video_run(asset_dir, tmp_path, 
                 p.slot[g] = None
                 if queue:
                     vid = queue.pop(0)
-                    p.start(g, vid, synthetic.SyntheticStream(length=lengths[vid], batch_size=1, rank=vid))
+                    p.start(g, vid, stream(vid, lengths[vid]))
         run = [g for g in range(4) if p.slot[g] is not None]
         if not run:
             break
@@ -259,20 +202,9 @@ def test_every_pool_video_follows_its_own_single_video_run(asset_dir, tmp_path, 
         for g, (vid, t, batch) in done.items():
             seen.add(vid)
             if vid not in singles:
-                singles[vid] = Adaptor(options(tmp_path, golden, 'c2', f'v{vid}'))
-                singles[vid].fused_eval = 'none'
-            ad = singles[vid]
-            calls = {'i': 0}
-
-            def provider(B, dev, vid=vid, t=t, calls=calls):
-                m = video_masks(vid, t, calls['i'])
-                calls['i'] += 1
-                return m.to(dev)
-            ad.teacher.mask_provider = provider
-            random.seed(7919 * vid + t)
-            ad.global_step, ad.fit_losses = t, {}
-            ad.model.eval()
-            ad.adapt(batch)
+                singles[vid] = SingleRun(pool_options(tmp_path, golden, 'c2', f'v{vid}'), vid)
+            singles[vid].step(t, batch)
+            ad = singles[vid].ad
             ref_up = float(ad.last_upper_loss)
             assert abs(float(up[g]) - ref_up) <= 1e-3 * abs(ref_up), (vid, t, float(up[g]), ref_up)
             ref = ad.predict(batch['image'])
@@ -286,10 +218,9 @@ def test_every_pool_video_follows_its_own_single_video_run(asset_dir, tmp_path, 
 
 
 def test_start_restores_the_checkpoint(asset_dir, tmp_path, golden):
-    from dynaboa_b200 import synthetic
-    p = Pool(options(tmp_path, golden, 'c2', 's'), 2)
+    p = PoolRun(pool_options(tmp_path, golden, 'c2', 's'), 2)
     for g in range(2):
-        p.start(g, g, synthetic.SyntheticStream(length=2, batch_size=1, rank=g))
+        p.start(g, g, stream(g, 2))
     for _ in range(2):
         p.step([0, 1])
     mv = p.mv

@@ -7,25 +7,18 @@
 - G = 4 at the golden's options: stream 0 against the golden, streams 1..3 against their own WebcamAdaptor runs; the motion term
   goes live from frame `interval` on.
 - Streams that sit ticks out, change slot and meet other streams' starts and pauses; reload(g); online_adaptation end to end."""
-import ast
-from types import SimpleNamespace
-
 import numpy as np
 import pytest
 import torch
 
 from conftest import rel_err
+from harness import SIZES, bits, cam_options, state, webcam_pool
 
 pytestmark = pytest.mark.gpu
 SENTINEL = 0x7fc0dead                  # a NaN payload no kernel writes
 
 
-def bits(t):
-    return t.contiguous().view(torch.int32)
-
-
 # ------------------------------------------------------------------ grouped input side
-SIZES = [(240, 320), (1080, 1920), (720, 1280), (480, 640), (300, 400), (1080, 1920), (256, 256), (600, 800)]
 
 
 def scene(G, seed):
@@ -121,22 +114,9 @@ def test_grouped_keypoints_are_the_one_stream_transform(G, active):
 
 
 # ------------------------------------------------------------------ the pool
-def golden_options(tmp, gd, **extra):
-    from dynaboa_b200 import config
-    o = dict(ast.literal_eval(str(gd['options'])))
-    o.update(expdir=str(tmp), expname='cam', tensorboard=0, model_file=config.BASE_MODEL)
-    o.update(extra)
-    return SimpleNamespace(**o)
-
-
 def single(tmp, gd, name, **extra):
     from dynaboa_b200.webcam import WebcamAdaptor
-    return WebcamAdaptor(golden_options(tmp / name, gd, **extra))
-
-
-def pool(tmp, gd, G, name, **extra):
-    from dynaboa_b200.webcam import MultiWebcamAdaptor
-    return MultiWebcamAdaptor(golden_options(tmp / name, gd, **extra), G, dynamic_loop=True)
+    return WebcamAdaptor(cam_options(tmp / name, gd, **extra))
 
 
 def stream_inputs(gd, vid, n):
@@ -155,10 +135,6 @@ def stream_inputs(gd, vid, n):
     return out
 
 
-def state(mv, g):
-    return [mv.thetas[g].clone(), mv.teachers[g].clone(), mv.m[g].clone(), mv.v[g].clone()]
-
-
 def single_state(ad):
     return [ad.model.module.arena, ad.teacher.arena, ad.optimizer.m, ad.optimizer.v]
 
@@ -171,7 +147,7 @@ def tick(mv, inputs):
 def test_one_stream_is_the_webcam_adaptor(asset_dir, tmp_path, golden):
     gd = golden('adapt_webcam')
     n = gd['kp25'].shape[0]
-    mv, ad = pool(tmp_path, gd, 1, 'mv'), single(tmp_path, gd, 'ad')
+    mv, ad = webcam_pool(tmp_path, gd, 1, 'mv'), single(tmp_path, gd, 'ad')
     for t, (img, kp) in enumerate(stream_inputs(gd, 0, n)):
         res = tick(mv, [(img, kp)])[0]
         ref = ad.adapt_processed(img, kp)
@@ -186,7 +162,7 @@ def test_four_streams_follow_the_golden_and_their_own_runs(asset_dir, tmp_path, 
     from oracle.make_golden import sample_indices
     gd = golden('adapt_webcam')
     n = gd['kp25'].shape[0]
-    mv = pool(tmp_path, gd, 4, 'mv')
+    mv = webcam_pool(tmp_path, gd, 4, 'mv')
     o = mv.options
     singles = {g: single(tmp_path, gd, f's{g}') for g in range(1, 4)}
     inputs = [stream_inputs(gd, g, n) for g in range(4)]
@@ -222,7 +198,7 @@ def test_streams_that_drop_out(asset_dir, tmp_path, golden):
     X, n = 5, 7
     xs = stream_inputs(gd, X, n)
     gaps = {2, 4}                                            # X's ticks with no person in view
-    a = pool(tmp_path, gd, 4, 'a')
+    a = webcam_pool(tmp_path, gd, 4, 'a')
     ad = single(tmp_path, gd, 'ad')
     o = a.options
     traj_a, n_outer = [], 0
@@ -241,7 +217,7 @@ def test_streams_that_drop_out(asset_dir, tmp_path, golden):
         assert float((a.theta(0) - ad.model.module.arena).abs().max()) <= 4 * o.lr * n_outer, t
         traj_a.append(state(a, 0) + [res[0]['vts'].clone(), res[0]['cam'].clone()])
     del a, ad
-    b = pool(tmp_path, gd, 4, 'b')
+    b = webcam_pool(tmp_path, gd, 4, 'b')
     others = {g: stream_inputs(gd, 10 + g, n + 3) for g in range(4)}
     traj_b = []
     for f in range(n + 3):
@@ -270,7 +246,7 @@ def test_streams_that_drop_out(asset_dir, tmp_path, golden):
 def test_reload_keeps_history_and_frame_count(asset_dir, tmp_path, golden):
     gd = golden('adapt_webcam')
     n = 5
-    mv = pool(tmp_path, gd, 2, 'mv')
+    mv = webcam_pool(tmp_path, gd, 2, 'mv')
     o = mv.options
     ad = single(tmp_path, gd, 'ad')
     ins = [stream_inputs(gd, 0, n), stream_inputs(gd, 1, n)]
@@ -324,7 +300,7 @@ def test_online_adaptation_end_to_end(asset_dir, tmp_path, golden):
     ticks[1][0][2] = None                                    # camera 2 sees nobody at tick 1
     runs = []
     for r in range(2):
-        mv = pool(tmp_path, gd, 3, f'r{r}', test_basemodel=1, dynamic_boa=0)
+        mv = webcam_pool(tmp_path, gd, 3, f'r{r}', test_basemodel=1, dynamic_boa=0)
         outs = []
         for t, (frames, dets) in enumerate(ticks):
             res = mv.online_adaptation(frames, dets)

@@ -11,37 +11,12 @@ import numpy as np
 import pytest
 import torch
 
+from harness import (CAM, COLOR, DRIVER, FLAGS, N, SHADOWED, check_against_oracle, frame, gpu_draw, make_video, posed_smpl_mesh, px_verts,
+                     quad, sphere)
 from oracle import render_ref
-from test_gpu_internet import DRIVER, FLAGS, N, SHADOWED, make_video
-from test_render import CAM, px_verts, quad
 
 pytestmark = pytest.mark.gpu
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-COLOR = (205 / 255, 129 / 255, 98 / 255)
-
-
-def frame(H, W, seed=0):
-    return np.random.default_rng(seed).integers(0, 256, size=(H, W, 3), dtype=np.uint8)
-
-
-def gpu_draw(img, verts, faces, cam4, rot=None, color=COLOR, samples=4):
-    from dynaboa_b200 import render
-    out, ids = render.draw(torch.from_numpy(img).cuda(), torch.as_tensor(verts).cuda(), faces, cam4, rot=rot, color=color,
-                           samples=samples, face_ids=True)
-    return out.cpu().numpy(), ids.cpu().numpy()
-
-
-def check_against_oracle(img, verts, faces, cam4, rot=None, color=COLOR, samples=4, min_covered=1):
-    out, ids = gpu_draw(img, verts, faces, cam4, rot, color, samples)
-    ref_out, ref_ids = render_ref.render(img, np.asarray(verts), faces, cam4, rot=rot, color=color, samples=samples)
-    mism = ids != ref_ids
-    assert not mism.any(), f'{mism.sum()} samples pick a different face than the oracle, first at {np.argwhere(mism)[0]}'
-    covered = (ids >= 0).any(2)
-    assert covered.sum() >= min_covered
-    assert np.array_equal(out[~covered], img[~covered])
-    diff = np.abs(out.astype(int) - ref_out.astype(int))[covered]
-    assert diff.max() <= 1, f'byte differs by {diff.max()}'
-    return out, ids
 
 
 def analytic_scenes():
@@ -54,45 +29,11 @@ def analytic_scenes():
     return px_verts(pts, 64, 48), np.array(fa + fb + fc + fd + [[16, 17, 18]])
 
 
-def sphere(n_lat=24, n_lon=48, radius=0.6):
-    """Closed UV sphere, faces wound counter-clockwise seen from outside."""
-    v = [(0.0, 0.0, radius)]
-    for i in range(1, n_lat):
-        th = np.pi * i / n_lat
-        for j in range(n_lon):
-            ph = 2 * np.pi * j / n_lon
-            v.append((radius * np.sin(th) * np.cos(ph), radius * np.sin(th) * np.sin(ph), radius * np.cos(th)))
-    v.append((0.0, 0.0, -radius))
-    f, last = [], len(v) - 1
-    ring = lambda i, j: 1 + (i - 1) * n_lon + (j % n_lon)
-    for j in range(n_lon):
-        f.append((0, ring(1, j), ring(1, j + 1)))
-        f.append((last, ring(n_lat - 1, j + 1), ring(n_lat - 1, j)))
-    for i in range(1, n_lat - 1):
-        for j in range(n_lon):
-            f.append((ring(i, j), ring(i + 1, j), ring(i + 1, j + 1)))
-            f.append((ring(i, j), ring(i + 1, j + 1), ring(i, j + 1)))
-    return np.array(v, dtype=np.float32), np.array(f, dtype=np.int64)
-
-
 @pytest.fixture(scope='module')
 def posed_smpl(asset_dir):
-    """The synthetic SMPL mesh posed by an HMR forward of the synthetic base model on a seeded image, and the camera of a
-    400-pixel crop of a 1920 x 1080 frame (a fixed crop camera: the random-weight regressor's own camera is arbitrary)."""
-    from dynaboa_b200 import config, render, synthetic
-    from dynaboa_b200.hmr import hmr
-    from dynaboa_b200.smpl import SMPL
-    from oracle import hmr_ref
-    m = hmr(synthetic.make_mean_params()).cuda()
-    m.load_state_dict(hmr_ref.strip_prefix(synthetic.make_basemodel()['model']), strict=True)
-    m.eval()
-    x = torch.randn(1, 3, 224, 224, generator=torch.Generator().manual_seed(7)).cuda()
-    with torch.no_grad():
-        rot, shape, _ = m(x)
-        smpl = SMPL(config.SMPL_MODEL_DIR, create_transl=False).cuda()
-        verts = smpl(betas=shape, body_pose=rot[:, 1:], global_orient=rot[:, 0].unsqueeze(1), pose2rot=False).vertices[0]
-    cam4 = render.convert_crop_cam_to_orig_img(np.array([[0.9, 0.05, 0.1]]), np.array([[900.0, 560.0, 400.0]]), 1920, 1080)[0]
-    return verts.cpu().numpy(), render.get_smpl_faces(), cam4
+    """harness.posed_smpl_mesh with the vertices on the host."""
+    verts, faces, cam4 = posed_smpl_mesh()
+    return verts.cpu().numpy(), faces, cam4
 
 
 @pytest.mark.parametrize('samples', [1, 4])

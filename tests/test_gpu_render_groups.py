@@ -13,11 +13,17 @@ import numpy as np
 import pytest
 import torch
 
+from harness import SIZES, check_against_oracle, frame, posed_smpl_mesh, sphere, webcam_pool
 from oracle import render_ref
-from test_gpu_multiwebcam import SIZES, pool
-from test_gpu_render import check_against_oracle, frame, posed_smpl, sphere  # noqa: F401  (posed_smpl: fixture)
 
 pytestmark = pytest.mark.gpu
+
+
+@pytest.fixture(scope='module')
+def posed_smpl(asset_dir):
+    """harness.posed_smpl_mesh with the vertices on the host."""
+    verts, faces, cam4 = posed_smpl_mesh()
+    return verts.cpu().numpy(), faces, cam4
 
 
 def entries(verts, M, seed):
@@ -73,7 +79,7 @@ def grouped(es, faces, samples):
 
 @pytest.mark.parametrize('samples', [1, 4])
 @pytest.mark.parametrize('M', [1, 2, 5, 16, 64])
-def test_each_mesh_is_itself_drawn_alone(posed_smpl, M, samples):  # noqa: F811
+def test_each_mesh_is_itself_drawn_alone(posed_smpl, M, samples):
     verts, faces, _ = posed_smpl
     es = entries(torch.from_numpy(verts).cuda(), M, M * 10 + samples)
     before = {id(e[0]): e[0].clone() for e in es}
@@ -127,7 +133,7 @@ def test_two_grouped_entries_match_the_oracle(samples):
 
 
 @pytest.mark.parametrize('M', [1, 64])
-def test_deterministic_and_six_launches(posed_smpl, M):  # noqa: F811
+def test_deterministic_and_six_launches(posed_smpl, M):
     from dynaboa_b200 import _lib
     verts, faces, _ = posed_smpl
     es = entries(torch.from_numpy(verts).cuda(), M, 3)
@@ -159,7 +165,7 @@ def webcam_ticks(seed):
 def test_pool_render_is_render_per_stream(asset_dir, tmp_path, golden, test_basemodel):
     from dynaboa_b200 import render
     gd = golden('adapt_webcam')
-    mv = pool(tmp_path, gd, 4, 'mv', test_basemodel=test_basemodel, dynamic_boa=0)
+    mv = webcam_pool(tmp_path, gd, 4, 'mv', test_basemodel=test_basemodel, dynamic_boa=0)
     frames, dets = webcam_ticks(4)
     res = mv.online_adaptation(frames, dets)
     assert res[2] is None

@@ -2,14 +2,12 @@
 tests/golden/adapt_webcam.npz -- the trajectory of the reference class itself, executed unmodified on CPU by
 oracle/make_golden.py ``golden_webcam`` (OpenPose joints 0..24 in the 2D / motion terms, teacher in eval mode, dynamic loop) --
 and its GPU input side (bounding box from the detections, confidence threshold, crop) against the CPU restatement."""
-import ast
-from types import SimpleNamespace
-
 import numpy as np
 import pytest
 import torch
 
 from conftest import rel_err
+from harness import cam_options
 
 pytestmark = pytest.mark.gpu
 
@@ -22,12 +20,8 @@ def L():
 
 
 def make_adaptor(tmp, gd, **extra):
-    from dynaboa_b200 import config
     from dynaboa_b200.webcam import WebcamAdaptor
-    o = dict(ast.literal_eval(str(gd['options'])))
-    o.update(expdir=str(tmp), expname='cam', tensorboard=0, model_file=config.BASE_MODEL)
-    o.update(extra)
-    return WebcamAdaptor(SimpleNamespace(**o))
+    return WebcamAdaptor(cam_options(tmp, gd, **extra))
 
 
 def test_webcam_adaptor_follows_the_reference_class(asset_dir, tmp_path, golden):

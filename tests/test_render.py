@@ -6,27 +6,10 @@ import os
 import numpy as np
 import pytest
 
+from harness import CAM, px_verts, quad
 from oracle import render_ref
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def px_verts(pts, W, H):
-    """Vertices whose window position is (u, r) pixels and whose ndc_z is d, under cam4 = (1, 1, 0, 0) and no rotation."""
-    pts = np.asarray(pts, dtype=np.float64)
-    return np.stack([2 * pts[:, 0] / W - 1, 2 * pts[:, 1] / H - 1, pts[:, 2]], 1).astype(np.float32)
-
-
-CAM = np.array([1.0, 1.0, 0.0, 0.0])
-
-
-def quad(x0, y0, x1, y1, d, first=0, flip=False):
-    """Two front-facing triangles (image-space signed area < 0) sharing the diagonal (x0, y0)-(x1, y1)."""
-    pts = [(x0, y0, d), (x1, y0, d), (x1, y1, d), (x0, y1, d)]
-    f = [[0, 3, 2], [0, 2, 1]]
-    if flip:
-        f = [[a, c, b] for a, b, c in f]
-    return pts, (np.array(f) + first).tolist()
 
 
 def raster(pts, faces, W, H, samples):
