@@ -2,12 +2,14 @@
 and no test module imports another.
 
 - Helpers: ``bits``, ``fetch``, ``stream``, ``golden_options`` and its presets, ``state``.
+- The device-free ABI tests: ``built_lib``, the stand-in pointer ``FAKE``, the ``ERR_*`` codes, ``cpu_options`` and ``idle_pool``.
 - The per-video pool runs: ``video_masks`` / ``video_seed`` and the golden-aware ``masks_for`` / ``seed_for``, ``PoolRun`` (a
   MultiVideoAdaptor whose slots carry videos) and ``SingleRun`` (the same video through the single-video ``Adaptor.adapt``).
 - The grouped HMR plan tests: the ``model`` fixture body, ``stacked``, ``inputs`` and the fp64 bounds of the layer tests.
 - Rendering: the analytic scene helpers, ``sphere``, ``posed_smpl_mesh``, ``check_against_oracle``, and the synthetic Internet
   video of the unchanged-driver tests."""
 import ast
+import ctypes
 import os
 import random
 from types import SimpleNamespace
@@ -15,6 +17,7 @@ from types import SimpleNamespace
 import numpy as np
 import torch
 
+from dynaboa_b200 import _lib
 from oracle import ref_harness
 
 
@@ -71,6 +74,36 @@ def cam_options(tmp, gd, **overrides):
 def webcam_pool(tmp, gd, G, name, **overrides):
     from dynaboa_b200.webcam import MultiWebcamAdaptor
     return MultiWebcamAdaptor(cam_options(tmp / name, gd, **overrides), G, dynamic_loop=True)
+
+
+# ------------------------------------------------------------------ device-free ABI tests
+# stand-in device pointer: every call it is passed to rejects its arguments before a pointer is dereferenced or a device touched
+FAKE = ctypes.c_void_p(0x1000)
+# the codes of _lib._ERRORS, which test_cabi.py holds to the header's DBOA_ERR_* (None for a name the binding lacks: no status is None)
+_CODE = {name: code for code, name in _lib._ERRORS.items()}
+ERR_ARG, ERR_SHAPE, ERR_CUDA, ERR_UNSUPPORTED = (_CODE.get('DBOA_ERR_' + n) for n in ('ARG', 'SHAPE', 'CUDA', 'UNSUPPORTED'))
+
+
+def built_lib():
+    """The library, built for sm_90a and loaded with its ctypes signatures: the body of the device-free modules' ``lib`` fixtures."""
+    from dynaboa_b200 import build
+    build.build()
+    return _lib.load()
+
+
+def cpu_options(workload, **extra):
+    """bench.py's options of `workload` with ``extra`` on top, for checks that run before any device or file is touched."""
+    from bench import WORKLOADS, default_options
+    return default_options(expdir='/nonexistent', expname='x', model_file='unused', synthetic_frames=2,
+                           **{**WORKLOADS[workload], **extra})
+
+
+def idle_pool(cls, G, **attrs):
+    """A ``cls`` pool (MultiVideoAdaptor, MultiWebcamAdaptor) of G slots with ``attrs`` set and no device: only its checks that
+    run before any device work can be called."""
+    pool = cls.__new__(cls)
+    vars(pool).update(G=G, **attrs)
+    return pool
 
 
 # ------------------------------------------------------------------ per-video pool runs

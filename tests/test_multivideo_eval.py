@@ -1,6 +1,5 @@
-"""Evaluation of a MultiVideoAdaptor pool without a device: the binding of dboa_eval_metrics_active and its argument errors
-(returned on the host before any device access), the ground-truth checks of ``adapt``, and the shared result writer."""
-import ctypes
+"""Evaluation of a MultiVideoAdaptor pool without a device: the argument errors of dboa_eval_metrics_active (returned on the host
+before any device access), the ground-truth checks of ``adapt``, and the shared result writer."""
 import os
 from types import SimpleNamespace
 
@@ -8,16 +7,13 @@ import joblib
 import numpy as np
 import pytest
 
-from dynaboa_b200 import _lib, build
-
-DBOA_ERR_ARG, DBOA_ERR_SHAPE = -1, -2
-FAKE = ctypes.c_void_p(0x1000)        # stand-in device pointers: every case below is rejected before one is dereferenced
+from dynaboa_b200.multivideo import MultiVideoAdaptor
+from harness import ERR_ARG, ERR_SHAPE, FAKE, built_lib, idle_pool
 
 
 @pytest.fixture(scope='module')
 def lib():
-    build.build()
-    return _lib.load()
+    return built_lib()
 
 
 def metrics_active(lib, NJ=17, n_map=14, B=4, groups=2, active=0b11, null=None):
@@ -27,28 +23,21 @@ def metrics_active(lib, NJ=17, n_map=14, B=4, groups=2, active=0b11, null=None):
     return lib.dboa_eval_metrics_active(p[0], p[1], p[2], p[3], NJ, 6890, p[4], n_map, p[5], p[6], B, groups, active, None)
 
 
-def test_binding():
-    P, I, U = ctypes.c_void_p, ctypes.c_int, ctypes.c_ulonglong
-    sig = _lib.SIGNATURES
-    one = sig['dboa_eval_metrics'][1]
-    assert sig['dboa_eval_metrics_active'] == (I, one[:-1] + [I, U, P])
-
-
 @pytest.mark.parametrize('null', range(7))
 def test_null_pointers(lib, null):
-    assert metrics_active(lib, null=null) == DBOA_ERR_ARG
+    assert metrics_active(lib, null=null) == ERR_ARG
 
 
 @pytest.mark.parametrize('kw', [dict(NJ=0), dict(NJ=33), dict(n_map=0), dict(n_map=33), dict(B=0), dict(B=-1), dict(groups=0), dict(groups=65),
                                 dict(groups=-1), dict(B=6, groups=4), dict(B=1, groups=2), dict(B=64, groups=128)])
 def test_shape_errors(lib, kw):
-    assert metrics_active(lib, **kw) == DBOA_ERR_SHAPE
-    assert metrics_active(lib, active=0, **kw) == DBOA_ERR_SHAPE             # the shape is checked before the mask
+    assert metrics_active(lib, **kw) == ERR_SHAPE
+    assert metrics_active(lib, active=0, **kw) == ERR_SHAPE             # the shape is checked before the mask
 
 
 @pytest.mark.parametrize('groups,active', [(2, 0), (2, 0b100), (4, 0b10000), (4, 1 << 63), (1, 0b10), (1, 0), (8, 1 << 8)])
 def test_mask_errors(lib, groups, active):
-    assert metrics_active(lib, B=8, groups=groups, active=active) == DBOA_ERR_ARG
+    assert metrics_active(lib, B=8, groups=groups, active=active) == ERR_ARG
 
 
 def test_the_one_video_call_keeps_its_errors(lib):
@@ -57,32 +46,25 @@ def test_the_one_video_call_keeps_its_errors(lib):
                                                                           None if null == 4 else p[4], n_map, None if null == 5 else p[5],
                                                                           None if null == 6 else p[6], B, None)
     for i in range(7):
-        assert call(null=i) == DBOA_ERR_ARG
-    assert call(NJ=33) == call(n_map=0) == call(B=0) == DBOA_ERR_SHAPE
+        assert call(null=i) == ERR_ARG
+    assert call(NJ=33) == call(n_map=0) == call(B=0) == ERR_SHAPE
 
 
 # ------------------------------------------------------------------ adapt's checks
-def pool(fused_eval, G=2):
-    from dynaboa_b200.multivideo import MultiVideoAdaptor
-    mv = MultiVideoAdaptor.__new__(MultiVideoAdaptor)          # no device: only the checks before any device work run
-    mv.G, mv.fused_eval = G, fused_eval
-    return mv
-
-
 @pytest.mark.parametrize('mode', ['final', 'all'])
 @pytest.mark.parametrize('key', ['pose', 'betas', 'gender'])
 def test_evaluation_needs_the_ground_truth(mode, key):
     full = dict(image=None, smpl_j2d=None, pose=None, betas=None, gender=None)
     part = {k: v for k, v in full.items() if k != key}
     with pytest.raises(ValueError, match=f'slot 1: .*{key}'):
-        pool(mode).adapt([full, part])
+        idle_pool(MultiVideoAdaptor, 2, fused_eval=mode).adapt([full, part])
     with pytest.raises(ValueError, match=key):
-        pool(mode).adapt([None, part])
+        idle_pool(MultiVideoAdaptor, 2, fused_eval=mode).adapt([None, part])
 
 
 def test_an_unknown_mode_is_refused():
     with pytest.raises(ValueError, match='fused_eval'):
-        pool('every').adapt([dict(image=None), None])
+        idle_pool(MultiVideoAdaptor, 2, fused_eval='every').adapt([dict(image=None), None])
 
 
 # ------------------------------------------------------------------ the shared writer

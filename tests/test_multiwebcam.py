@@ -1,25 +1,20 @@
-"""Webcam pool without a device: the bindings of dboa_crop_resize_normalize_groups / dboa_keypoint_transform_groups and their
-argument errors (returned on the host before any device access), the ctypes mirror of dboa_crop_desc against the compiled
-header, and the argument checks of MultiWebcamAdaptor.online_adaptation / adapt_processed."""
+"""Webcam pool without a device: the argument errors of dboa_crop_resize_normalize_groups / dboa_keypoint_transform_groups
+(returned on the host before any device access) and the argument checks of MultiWebcamAdaptor.online_adaptation /
+adapt_processed."""
 import ctypes
-import os
-import subprocess
 from types import SimpleNamespace
 
 import numpy as np
 import pytest
 
-from dynaboa_b200 import _lib, build
-
-DBOA_ERR_ARG, DBOA_ERR_SHAPE = -1, -2
-FAKE = 0x1000            # stand-in device pointers: every case below is rejected before one is dereferenced
-P, I, L, U = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_ulonglong
+from dynaboa_b200 import _lib
+from dynaboa_b200.webcam import MultiWebcamAdaptor
+from harness import ERR_ARG, ERR_SHAPE, FAKE, built_lib, idle_pool
 
 
 @pytest.fixture(scope='module')
 def lib():
-    build.build()
-    return _lib.load()
+    return built_lib()
 
 
 def descs(groups, **over):
@@ -35,106 +30,73 @@ def descs(groups, **over):
 
 def crop(lib, groups=2, active=0b11, res=224, tmp_floats=10 ** 9, frames=None, null=None):
     frames = descs(groups) if frames is None else frames
-    p = [frames, (ctypes.c_float * 3)(), (ctypes.c_float * 3)(), P(FAKE), P(FAKE)]
+    p = [frames, (ctypes.c_float * 3)(), (ctypes.c_float * 3)(), FAKE, FAKE]
     if null is not None:
         p[null] = None
     return lib.dboa_crop_resize_normalize_groups(p[0], groups, active, res, p[1], p[2], p[3], tmp_floats, p[4], None)
 
 
 def keypoints(lib, n=25, groups=2, active=0b11, res=224, null=None):
-    p = [P(FAKE), (ctypes.c_double * (4 * max(groups, 1)))(), P(FAKE)]
+    p = [FAKE, (ctypes.c_double * (4 * max(groups, 1)))(), FAKE]
     if null is not None:
         p[null] = None
     return lib.dboa_keypoint_transform_groups(p[0], n, p[1], res, p[2], groups, active, None)
 
 
-def test_bindings():
-    sig = _lib.SIGNATURES
-    assert sig['dboa_crop_resize_normalize_groups'] == (I, [ctypes.POINTER(_lib.CropDescStruct), I, U, I, P, P, P, L, P, P])
-    assert sig['dboa_keypoint_transform_groups'] == (I, [P, I, ctypes.POINTER(ctypes.c_double), I, P, I, U, P])
-    # the per-frame fields of the one-frame call, in its order
-    one = sig['dboa_crop_resize_normalize'][1]
-    assert one[:7] == [P, I, I, I, I, I, I] and [f[0] for f in _lib.CropDescStruct._fields_][5:] == ['is_u8', 'H', 'W', 'ul_x', 'ul_y',
-                                                                                                   'Hc', 'Tx', 'Ty']
-
-
-def test_descriptor_layout_matches_the_header(tmp_path):
-    """offsetof / sizeof of dboa_crop_desc compiled from the header against the ctypes mirror."""
-    fields = [f[0] for f in _lib.CropDescStruct._fields_]
-    repo = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    src = tmp_path / 'layout.c'
-    src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "dynaboa_b200.h"\nint main(void) {\n'
-                   + ''.join(f'  printf("%zu\\n", offsetof(dboa_crop_desc, {f}));\n' for f in fields)
-                   + '  printf("%zu\\n", sizeof(dboa_crop_desc));\n  return 0;\n}\n')
-    exe = tmp_path / 'layout'
-    subprocess.check_call(['gcc', '-I', os.path.join(repo, 'include'), str(src), '-o', str(exe)])
-    got = [int(x) for x in subprocess.check_output([str(exe)], text=True).split()]
-    want = [getattr(_lib.CropDescStruct, f).offset for f in fields] + [ctypes.sizeof(_lib.CropDescStruct)]
-    assert got == want
-    assert 64 * got[-1] < 32 * 1024                          # 64 descriptors fit the kernel parameter space
-
-
 @pytest.mark.parametrize('null', range(5))
 def test_crop_null_pointers(lib, null):
-    assert crop(lib, null=null) == DBOA_ERR_ARG
+    assert crop(lib, null=null) == ERR_ARG
 
 
 @pytest.mark.parametrize('field', ['img', 'wx', 'sx', 'wy', 'sy'])
 def test_crop_null_descriptor_pointers(lib, field):
-    assert crop(lib, frames=descs(2, **{field: None})) == DBOA_ERR_ARG
-    assert crop(lib, active=0b10, frames=descs(2, **{field: None}), tmp_floats=0) == DBOA_ERR_ARG       # idle: not read; tmp
+    assert crop(lib, frames=descs(2, **{field: None})) == ERR_ARG
+    assert crop(lib, active=0b10, frames=descs(2, **{field: None}), tmp_floats=0) == ERR_ARG       # idle: not read; tmp
 
 
 @pytest.mark.parametrize('kw', [dict(groups=0), dict(groups=65), dict(groups=-1), dict(res=0), dict(res=-224)])
 def test_crop_shape_errors(lib, kw):
-    assert crop(lib, **kw) == DBOA_ERR_SHAPE
-    assert crop(lib, active=0, **kw) == DBOA_ERR_SHAPE          # the shape is checked before the mask
+    assert crop(lib, **kw) == ERR_SHAPE
+    assert crop(lib, active=0, **kw) == ERR_SHAPE          # the shape is checked before the mask
 
 
 @pytest.mark.parametrize('field', ['H', 'W', 'Hc', 'Tx', 'Ty'])
 @pytest.mark.parametrize('value', [0, -3])
 def test_crop_descriptor_shape_errors(lib, field, value):
-    assert crop(lib, frames=descs(2, **{field: value})) == DBOA_ERR_SHAPE
+    assert crop(lib, frames=descs(2, **{field: value})) == ERR_SHAPE
     # an idle stream's descriptor is not looked at: the error left is the scratch size, which counts the active frame only
-    assert crop(lib, active=0b10, frames=descs(2, **{field: value}), tmp_floats=300 * 224 * 3 - 1) == DBOA_ERR_ARG
+    assert crop(lib, active=0b10, frames=descs(2, **{field: value}), tmp_floats=300 * 224 * 3 - 1) == ERR_ARG
 
 
 @pytest.mark.parametrize('groups,active', [(2, 0), (2, 0b100), (4, 0b10000), (4, 1 << 63), (1, 0b10), (1, 0), (8, 1 << 8)])
 def test_crop_mask_errors(lib, groups, active):
-    assert crop(lib, groups=groups, active=active) == DBOA_ERR_ARG
+    assert crop(lib, groups=groups, active=active) == ERR_ARG
 
 
 def test_crop_scratch_size(lib):
     need = 300 * 224 * 3
-    assert crop(lib, groups=3, active=0b101, tmp_floats=2 * need - 1) == DBOA_ERR_ARG
-    assert crop(lib, groups=1, active=1, tmp_floats=need - 1) == DBOA_ERR_ARG
-    assert crop(lib, groups=64, active=~0 & (2 ** 64 - 1), tmp_floats=64 * need - 1) == DBOA_ERR_ARG
+    assert crop(lib, groups=3, active=0b101, tmp_floats=2 * need - 1) == ERR_ARG
+    assert crop(lib, groups=1, active=1, tmp_floats=need - 1) == ERR_ARG
+    assert crop(lib, groups=64, active=~0 & (2 ** 64 - 1), tmp_floats=64 * need - 1) == ERR_ARG
 
 
 @pytest.mark.parametrize('null', range(3))
 def test_keypoint_null_pointers(lib, null):
-    assert keypoints(lib, null=null) == DBOA_ERR_ARG
+    assert keypoints(lib, null=null) == ERR_ARG
 
 
 @pytest.mark.parametrize('kw', [dict(groups=0), dict(groups=65), dict(n=-1), dict(n=50), dict(res=0)])
 def test_keypoint_shape_errors(lib, kw):
-    assert keypoints(lib, **kw) == DBOA_ERR_SHAPE
-    assert keypoints(lib, active=0, **kw) == DBOA_ERR_SHAPE
+    assert keypoints(lib, **kw) == ERR_SHAPE
+    assert keypoints(lib, active=0, **kw) == ERR_SHAPE
 
 
 @pytest.mark.parametrize('groups,active', [(2, 0), (2, 0b100), (1, 0b10), (8, 1 << 8), (63, 1 << 63)])
 def test_keypoint_mask_errors(lib, groups, active):
-    assert keypoints(lib, groups=groups, active=active) == DBOA_ERR_ARG
+    assert keypoints(lib, groups=groups, active=active) == ERR_ARG
 
 
 # ------------------------------------------------------------------ the pool's checks
-def pool(G=3):
-    from dynaboa_b200.webcam import MultiWebcamAdaptor
-    mv = MultiWebcamAdaptor.__new__(MultiWebcamAdaptor)        # no device: only the checks before any device work run
-    mv.G = G
-    return mv
-
-
 def frame():
     return np.zeros((48, 64, 3), np.uint8)
 
@@ -144,7 +106,7 @@ def det(shape=(1, 25, 3)):
 
 
 def test_online_adaptation_checks():
-    mv = pool(3)
+    mv = idle_pool(MultiWebcamAdaptor, 3)
     with pytest.raises(ValueError, match='3 frames'):
         mv.online_adaptation([frame()] * 2, [det()] * 3)
     with pytest.raises(ValueError, match='3 frames'):
@@ -161,7 +123,7 @@ def test_online_adaptation_checks():
 
 def test_adapt_processed_checks():
     import torch
-    mv = pool(2)
+    mv = idle_pool(MultiWebcamAdaptor, 2)
     img, kp = torch.zeros(1, 3, 224, 224), torch.zeros(1, 49, 3)
     with pytest.raises(ValueError, match='2 images'):
         mv.adapt_processed([img], [kp, kp])
@@ -185,7 +147,6 @@ def webcam_opts(**extra):
 
 def test_pool_options(lib):
     from dynaboa_b200.multivideo import check_options
-    from dynaboa_b200.webcam import MultiWebcamAdaptor
     assert MultiWebcamAdaptor.kp_range == (0, 25) and MultiWebcamAdaptor.motion_lead == 1
     o = webcam_opts(dynamic_boa=1)
     assert o.retrieval == 0 and o.teacher_dropout == 0 and o.batch_size == 1

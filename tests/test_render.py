@@ -6,7 +6,7 @@ import os
 import numpy as np
 import pytest
 
-from harness import CAM, px_verts, quad
+from harness import CAM, built_lib, px_verts, quad
 from oracle import render_ref
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -99,9 +99,7 @@ def test_wireframe_is_rejected():
 
 
 def test_abi_argument_errors_without_gpu():
-    from dynaboa_b200 import _lib, build
-    build.build()
-    lib = _lib.load()
+    lib = built_lib()
     assert lib.dboa_render_scratch_bytes(9000, 10, 6890, 13776, 4) == -2
     assert lib.dboa_render_scratch_bytes(640, 480, -1, 10, 4) == -2
     assert lib.dboa_render_scratch_bytes(640, 480, 10, 10, 2) == -1

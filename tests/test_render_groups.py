@@ -1,23 +1,19 @@
 """Grouped mesh overlay without a GPU: the error codes of dboa_render_overlay_groups and its size query (fake device pointers,
-every check happens before any device access), the scratch size against the one-mesh query, the dboa_render_desc layout
-against its ctypes mirror, and the Python argument checks of render.draw_groups and MultiWebcamAdaptor.render."""
+every check happens before any device access), the scratch size against the one-mesh query, and the Python argument checks of
+render.draw_groups and MultiWebcamAdaptor.render."""
 import ctypes
-import os
-import subprocess
 from types import SimpleNamespace
 
 import numpy as np
 import pytest
 import torch
 
-REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from harness import built_lib, idle_pool
 
 
 @pytest.fixture(scope='module')
 def lib():
-    from dynaboa_b200 import _lib, build
-    build.build()
-    return _lib.load()
+    return built_lib()
 
 
 def ints(*v):
@@ -89,27 +85,6 @@ def test_abi_argument_errors_without_gpu(lib):
     assert run(d, nbytes=16) == -1
 
 
-def test_render_desc_layout_matches_the_header(tmp_path):
-    from dynaboa_b200 import _lib
-    fields = [f[0] for f in _lib.RenderDescStruct._fields_]
-    src = tmp_path / 'layout.c'
-    src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "dynaboa_b200.h"\nint main(void) {\n'
-                   + ''.join(f'  printf("%zu\\n", offsetof(dboa_render_desc, {f}));\n' for f in fields)
-                   + '  printf("%zu\\n", sizeof(dboa_render_desc));\n  return 0;\n}\n')
-    exe = tmp_path / 'layout'
-    subprocess.check_call(['gcc', '-I', os.path.join(REPO, 'include'), str(src), '-o', str(exe)])
-    got = [int(x) for x in subprocess.check_output([str(exe)], text=True).split()]
-    want = [getattr(_lib.RenderDescStruct, f).offset for f in fields] + [ctypes.sizeof(_lib.RenderDescStruct)]
-    assert got == want
-
-
-def test_render_bindings():
-    from dynaboa_b200 import _lib
-    P, I, L = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong
-    assert _lib.SIGNATURES['dboa_render_scratch_bytes_groups'] == (L, [ctypes.POINTER(I), ctypes.POINTER(I), I, I, I, I])
-    assert _lib.SIGNATURES['dboa_render_overlay_groups'] == (I, [ctypes.POINTER(_lib.RenderDescStruct), I, P, P, P, I, I, I, P, L, P])
-
-
 FACES = np.array([[0, 1, 2]])
 
 
@@ -145,15 +120,9 @@ def test_render_groups_argument_checks():
         render.render_groups([None], [None, None], [None], [None], [None])
 
 
-def fake_pool(G, test_basemodel):
-    from dynaboa_b200.webcam import MultiWebcamAdaptor
-    mv = MultiWebcamAdaptor.__new__(MultiWebcamAdaptor)              # no device: only the argument checks run
-    mv.G, mv.options = G, SimpleNamespace(test_basemodel=test_basemodel)
-    return mv
-
-
 def test_pool_render_argument_checks():
-    mv = fake_pool(3, 1)
+    from dynaboa_b200.webcam import MultiWebcamAdaptor
+    mv = idle_pool(MultiWebcamAdaptor, 3, options=SimpleNamespace(test_basemodel=1))
     frame = np.zeros((48, 64, 3), np.uint8)
     res = {'vts': None, 'cam': None, 'bbox': None, 'vts_base': None, 'cam_base': None}
     with pytest.raises(ValueError, match='3 frames and 3 results'):
