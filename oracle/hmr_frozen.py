@@ -16,6 +16,10 @@ from its own values and is the network of ``hmr_ref`` (tests/test_hmr_frozen.py 
 The pattern is a dict: ``'relu'`` maps the name of each convolution that feeds a ReLU (``conv1``, ``layer1.0.conv1``, ...,
 ``layerL.B.conv3``; the shortcut joins conv3's ReLU) to an NCHW 0/1 mask, ``'pool'`` is the (B,64,56,56) integer window
 position of the max-pool, and ``'drop'`` is None or the (3,2,B,1024) scaled keep-masks.
+
+With ``need_feature`` the forward also returns the 15 feature tensors of ``hmr_ref.forward(need_feature=True)``, in the order of
+``dboa_hmr_feature_info``: the stem convolution's output, the outputs of layer1..4, the pooled 2048-vector and the nine rows of
+the regressor.
 """
 import torch
 import torch.nn.functional as F
@@ -63,23 +67,29 @@ def _bottleneck(x, p, pre, stride, has_ds, pattern, own):
     return _relu(out + res, pre + '.conv3', pattern, own)
 
 
-def forward(x, p, pattern=None, drop=None):
+def forward(x, p, pattern=None, drop=None, need_feature=False):
     """(rotmat, shape, cam, pattern) of the HMR forward (hmr_ref.forward with n_iter = 3) on ``pattern``, or on its own
     pattern when None (returned, with ``drop`` as its dropout keep-masks).  ``p`` holds the 169 parameters and the init_*
-    buffers by state_dict name."""
+    buffers by state_dict name.  ``need_feature``: the 15 feature tensors follow as a fifth element."""
     own = pattern is None
     if own:
         pattern = {'relu': {}, 'pool': None, 'drop': drop}
     B = x.shape[0]
-    y = _relu(hmr_ref._gn(F.conv2d(x, p['conv1.weight'], stride=2, padding=3), p, 'bn1'), 'conv1', pattern, own)
+    stem = F.conv2d(x, p['conv1.weight'], stride=2, padding=3)
+    feats = [stem]
+    y = _relu(hmr_ref._gn(stem, p, 'bn1'), 'conv1', pattern, own)
     y = _maxpool(y, pattern, own)
     for li, nblk in enumerate(hmr_ref.BLOCKS):
         for bi in range(nblk):
             y = _bottleneck(y, p, f'layer{li + 1}.{bi}', 2 if (li > 0 and bi == 0) else 1, bi == 0, pattern, own)
+        feats.append(y)
     xf = F.avg_pool2d(y, 7, stride=1).flatten(1)
+    feats.append(xf)
     drop = pattern['drop']
     masks = None if drop is None else [(drop[i, 0].to(xf), drop[i, 1].to(xf)) for i in range(3)]
-    pose, shape, cam, _ = hmr_ref.regressor(xf, p, p['init_pose'].expand(B, -1), p['init_shape'].expand(B, -1),
-                                            p['init_cam'].expand(B, -1), 3, masks)
+    pose, shape, cam, hfeats = hmr_ref.regressor(xf, p, p['init_pose'].expand(B, -1), p['init_shape'].expand(B, -1),
+                                                 p['init_cam'].expand(B, -1), 3, masks)
     rotmat = geometry_ref.rot6d_to_rotmat(pose).view(B, 24, 3, 3)
+    if need_feature:
+        return rotmat, shape, cam, pattern, feats + hfeats
     return rotmat, shape, cam, pattern

@@ -5,11 +5,15 @@ and no test module imports another.
 - The device-free ABI tests: ``built_lib``, the stand-in pointer ``FAKE``, the ``ERR_*`` codes, ``cpu_options`` and ``idle_pool``.
 - The per-video pool runs: ``video_masks`` / ``video_seed`` and the golden-aware ``masks_for`` / ``seed_for``, ``PoolRun`` (a
   MultiVideoAdaptor whose slots carry videos) and ``SingleRun`` (the same video through the single-video ``Adaptor.adapt``).
-- The grouped HMR plan tests: the ``model`` fixture body, ``stacked``, ``inputs`` and the fp64 bounds of the layer tests.
+- The grouped HMR plan tests: the ``model`` fixture body, ``stacked``, ``inputs``, the fp64 bounds of the layer tests and
+  ``tape_pattern``, the kink pattern of a GPU forward for oracle/hmr_frozen.py.
+- The exact references of the step's sweeps (``f32``, ``sgd_ref``, ``ema_ref``, ``adam_ref``) and the pose prior's near-tie rule
+  ``selected``.
 - Rendering: the analytic scene helpers, ``sphere``, ``posed_smpl_mesh``, ``check_against_oracle``, and the synthetic Internet
   video of the unchanged-driver tests."""
 import ast
 import ctypes
+import math
 import os
 import random
 from types import SimpleNamespace
@@ -273,6 +277,54 @@ def nchw(t):
 def rel(a, ref, scale=None):
     s = ref.abs().max() if scale is None else scale
     return float((a.double() - ref).abs().max() / s.clamp_min(1e-30))
+
+
+def tape_pattern(tape, B, rows=slice(None), masks=None):
+    """The kink pattern (oracle/hmr_frozen.py) of the samples ``rows`` of the GPU forward whose tape is ``tape`` (batch B):
+    each ReLU's ``a > 0``, the max-pool's window positions and the dropout keep-masks ``masks`` (None: no dropout)."""
+    from dynaboa_b200.hmr import tape_views
+    v = tape_views(tape, B)
+    geo, _ = structure()
+    return {'relu': {g[0]: nchw(v['a'][i][rows]) > 0 for i, g in enumerate(geo) if v['a'][i] is not None},
+            'pool': v['p0_idx'][rows].permute(0, 3, 1, 2).long(),
+            'drop': None if masks is None else masks[:, :, rows].double()}
+
+
+# ------------------------------------------------------------------ the step's sweeps and the pose prior's choice
+def f32(x):
+    """A Python double rounded once to fp32: the scalar torch hands its fp32 kernels."""
+    return float(np.float32(x))
+
+
+def sgd_ref(p, g, lr):
+    return torch.add(p, torch.mul(g, f32(-lr)))
+
+
+def ema_ref(t, p, alpha):
+    return torch.add(torch.mul(t, f32(alpha)), torch.mul(p, f32(1.0 - alpha)))
+
+
+def adam_ref(p, g, m, v, t, lr, betas, eps, step, alpha=0.1, gscale=1.0):
+    """torch's single-tensor Adam (lerp_, mul_ + addcmul_, sqrt / bias_correction2_sqrt + eps, addcdiv_) op by op in fp32,
+    then the EMA teacher on the new weights (t None: no teacher).  Returns (p, m, v, t)."""
+    beta1, beta2 = betas
+    bc1, bc2 = 1.0 - beta1 ** step, 1.0 - beta2 ** step
+    w1 = f32(1.0 - beta1)
+    g = torch.mul(g, f32(gscale))
+    diff = torch.sub(g, m)
+    # ATen's lerp: w < 0.5 ? a + w (b - a) : b - (b - a)(1 - w), with 1 - w formed in fp32
+    m = torch.add(m, torch.mul(diff, w1)) if w1 < 0.5 else torch.sub(g, torch.mul(diff, f32(1.0 - w1)))
+    v = torch.add(torch.mul(v, f32(beta2)), torch.mul(torch.mul(g, f32(1.0 - beta2)), g))
+    # ATen's vectorised CPU sqrt is not correctly rounded (a few elements in 10^3 are 1 ulp off); the fp64 square root of an
+    # fp32 value, rounded to fp32, is
+    denom = torch.add(torch.div(torch.sqrt(v.double()).float(), f32(math.sqrt(bc2))), f32(eps))
+    p = torch.add(p, torch.mul(torch.div(m, denom), f32(-(lr / bc1))))
+    return p, m, v, (None if t is None else ema_ref(t, p, alpha))
+
+
+def selected(ll, prior_b):
+    """The component each body's GPU prior value belongs to: the fp64 component value closest to it."""
+    return (ll.detach() - prior_b.double().cpu()[:, None]).abs().argmin(1)
 
 
 # ------------------------------------------------------------------ rendering

@@ -19,7 +19,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from harness import FWD_TOL, GRAD_L2, GRAD_TOL, nchw, rel, structure
+from harness import FWD_TOL, GRAD_L2, GRAD_TOL, nchw, rel, structure, tape_pattern
 
 pytestmark = pytest.mark.gpu
 
@@ -160,18 +160,14 @@ def test_forward_layer_by_layer(model, cfg):
 def frozen_gradient(m, x, masks, tape, B, d):
     """fp64 autograd gradient of hmr_frozen on the GPU's pattern, summed over chunks of samples (the network does not mix
     samples), as {parameter name: gradient}."""
-    from dynaboa_b200.hmr import layout, tape_views
+    from dynaboa_b200.hmr import layout
     from oracle import hmr_frozen
     lay = layout()
-    v = tape_views(tape, B)
-    geo, _ = structure()
     p = {n: w.detach().double().requires_grad_(True) for n, w in zip(lay.names, lay.views(m.arena))}
     bufs = {k: m._buffers[k].double() for k in ('init_pose', 'init_shape', 'init_cam')}
     for s0 in range(0, B, 16):
         s = slice(s0, min(B, s0 + 16))
-        pattern = {'relu': {g[0]: nchw(v['a'][i][s]) > 0 for i, g in enumerate(geo) if v['a'][i] is not None},
-                   'pool': v['p0_idx'][s].permute(0, 3, 1, 2).long(),
-                   'drop': None if masks is None else masks[:, :, s].double()}
+        pattern = tape_pattern(tape, B, s, masks)
         rot, shape, cam, _ = hmr_frozen.forward(x[s].double(), dict(p, **bufs), pattern)
         ((rot * d[0][s]).sum() + (shape * d[1][s]).sum() + (cam * d[2][s]).sum()).backward()
     return {n: t.grad for n, t in p.items()}

@@ -23,6 +23,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from harness import selected
+
 pytestmark = pytest.mark.gpu
 
 TOL = {                          # bound         worst measured
@@ -156,11 +158,6 @@ def gpu_prior(env, R, drot=None, scale=1.0):
     p = env.prior
     call('dboa_pose_prior', P(R), P(p.means), P(p.precisions), P(p.neg_log_weights), P(pb), P(drot), float(scale), B)
     return pb
-
-
-def selected(ll, prior_b):
-    """The component each body's GPU prior value belongs to: the fp64 component value closest to it."""
-    return (ll.detach() - prior_b.double().cpu()[:, None]).abs().argmin(1)
 
 
 def d64(t, grad=False):

@@ -21,6 +21,8 @@ import numpy as np
 import pytest
 import torch
 
+from harness import adam_ref, ema_ref, f32, sgd_ref
+
 GUARD = 64
 SENTINEL = {torch.float32: -1.2345678e33, torch.float64: -1.25e300, torch.int32: 0x5A5A5A5A}
 U32 = 2.0 ** -24                                   # unit roundoff of fp32
@@ -70,11 +72,6 @@ def same_bits(a, b):
     return torch.equal(a.view(view), b.view(view))
 
 
-def f32(x):
-    """A Python double rounded once to fp32: the scalar torch hands its fp32 kernels."""
-    return float(np.float32(x))
-
-
 def num_sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
@@ -88,32 +85,6 @@ def sweep_sizes(L):
 # ---------------------------------------------------------------------------------------------------------------------
 # fp32 restatements of the sweeps (CPU), the fp64 Adam they must mean
 # ---------------------------------------------------------------------------------------------------------------------
-def sgd_ref(p, g, lr):
-    return torch.add(p, torch.mul(g, f32(-lr)))
-
-
-def ema_ref(t, p, alpha):
-    return torch.add(torch.mul(t, f32(alpha)), torch.mul(p, f32(1.0 - alpha)))
-
-
-def adam_ref(p, g, m, v, t, lr, betas, eps, step, alpha=0.1, gscale=1.0):
-    """torch's single-tensor Adam (lerp_, mul_ + addcmul_, sqrt / bias_correction2_sqrt + eps, addcdiv_) op by op in fp32,
-    then the EMA teacher on the new weights (t None: no teacher).  Returns (p, m, v, t)."""
-    beta1, beta2 = betas
-    bc1, bc2 = 1.0 - beta1 ** step, 1.0 - beta2 ** step
-    w1 = f32(1.0 - beta1)
-    g = torch.mul(g, f32(gscale))
-    diff = torch.sub(g, m)
-    # ATen's lerp: w < 0.5 ? a + w (b - a) : b - (b - a)(1 - w), with 1 - w formed in fp32
-    m = torch.add(m, torch.mul(diff, w1)) if w1 < 0.5 else torch.sub(g, torch.mul(diff, f32(1.0 - w1)))
-    v = torch.add(torch.mul(v, f32(beta2)), torch.mul(torch.mul(g, f32(1.0 - beta2)), g))
-    # ATen's vectorised CPU sqrt is not correctly rounded (a few elements in 10^3 are 1 ulp off); the fp64 square root of an
-    # fp32 value, rounded to fp32, is
-    denom = torch.add(torch.div(torch.sqrt(v.double()).float(), f32(math.sqrt(bc2))), f32(eps))
-    p = torch.add(p, torch.mul(torch.div(m, denom), f32(-(lr / bc1))))
-    return p, m, v, (None if t is None else ema_ref(t, p, alpha))
-
-
 def adam_fp64(p, g, m, v, lr, betas, eps, step, gscale=1.0):
     """Adam in fp64 on the same fp32 inputs: (p, m, v, denom)."""
     beta1, beta2 = betas
