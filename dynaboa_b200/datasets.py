@@ -5,7 +5,10 @@ There are no licensed datasets on the build or GPU boxes, so these classes serve
 ``dynaboa_b200.synthetic`` -- and ONLY when the caller opts in: the unchanged reference driver run with ``--dataset 3dpw``
 would otherwise report MPJPE / PA-MPJPE / PVE on synthetic frames without saying so.  Opt in with
 ``options.synthetic_frames = N`` (tests, bench) or ``DBOA_SYNTHETIC_FRAMES=N`` in the environment (unchanged driver).
-Real crops go through ``dynaboa_b200.dataprocess`` (GPU crop / resize / normalise, the step before the hot path)."""
+Real crops go through ``dynaboa_b200.dataprocess`` (GPU crop / resize / normalise, the step before the hot path).
+
+``internet_videos(root)`` reads the same folder as one ``InternetVideo`` per sequence instead of one concatenated stream: the
+input of a pool that adapts the sequences side by side (``internet.MultiInternetAdaptor``)."""
 import os
 import warnings
 
@@ -93,3 +96,62 @@ class Internet_dataset(Dataset):
         kp = torch.from_numpy(np.asarray(self.smpl_j2ds[i], dtype=np.float32)).cuda()
         return {'image': dataprocess.crop(rgb, center, scale), 'imgname': name, 'smpl_j2d': dataprocess.j2d_processing(kp, center, scale),
                 'bbox': np.stack([center[0], center[1], scale * 200])}
+
+
+INTERNET_KEYS = ('imgname', 'center', 'scale', 'part')
+
+
+class InternetVideo:
+    """One Internet sequence on the host: ``name`` (its npz's file name without ``.npz``), the per-frame records of the npz
+    (``imgnames``, ``centers`` (n, 2), ``scales`` (n,), ``parts`` (n, 49, 3) pixel keypoints) and the directory ``imgdir`` of
+    its frames.  No frame is decoded here.  ``frame(t)`` gives frame t's record: the path, and the box and keypoints as
+    ``Internet_dataset.__getitem__`` reads them."""
+
+    def __init__(self, path, imgdir):
+        import os.path as osp
+
+        import numpy as np
+        self.path, self.imgdir = path, imgdir
+        self.name = osp.splitext(osp.basename(path))[0]
+        try:
+            with np.load(path) as d:
+                arrays = {k: np.asarray(d[k]) for k in INTERNET_KEYS if k in d.files}
+        except Exception as e:                              # not a zip, a pickled object, a truncated file
+            raise ValueError(f'{path}: not a readable npz ({type(e).__name__}: {e})') from e
+        missing = [k for k in INTERNET_KEYS if k not in arrays]
+        if missing:
+            raise ValueError(f'{path}: missing {", ".join(missing)} (expected {", ".join(INTERNET_KEYS)})')
+        self.imgnames, self.centers, self.scales, self.parts = (arrays[k] for k in INTERNET_KEYS)
+        if self.imgnames.ndim != 1:
+            raise ValueError(f'{path}: imgname of shape {tuple(self.imgnames.shape)}, expected one name per frame')
+        n = len(self.imgnames)
+        for k, v, shape in (('center', self.centers, (n, 2)), ('scale', self.scales, (n,)), ('part', self.parts, (n, 49, 3))):
+            if tuple(v.shape) != shape:
+                raise ValueError(f'{path}: {k} of shape {tuple(v.shape)}, expected {shape} for {n} frames')
+
+    def __len__(self):
+        return len(self.imgnames)
+
+    def frame(self, t):
+        """Frame t: (path, center [cx, cy], scale, (49, 3) float32 keypoints, (1, 3) float64 bbox), with the floats of
+        ``Internet_dataset.__getitem__``."""
+        import numpy as np
+        if not 0 <= t < len(self):
+            raise IndexError(f'{self.name}: frame {t} of {len(self)}')
+        center, scale = [float(self.centers[t][0]), float(self.centers[t][1])], float(self.scales[t])
+        return (os.path.join(self.imgdir, str(self.imgnames[t])), center, scale, np.asarray(self.parts[t], dtype=np.float32),
+                np.stack([center[0], center[1], scale * 200])[None])
+
+
+def internet_videos(root):
+    """One ``InternetVideo`` per ``root/*.npz`` (the layout ``Internet_dataset`` reads: the reference's npz, the frames under
+    ``root/images``), sorted by file name, so the videos come in ``Internet_dataset``'s order.  Raises FileNotFoundError when
+    ``root`` holds no npz and ValueError for a malformed one."""
+    import glob
+    import os.path as osp
+    if not osp.isdir(root):
+        raise FileNotFoundError(f'{root} is not a directory')
+    names = sorted(glob.glob(osp.join(root, '*.npz')))
+    if not names:
+        raise FileNotFoundError(f'no *.npz sequence under {root}')
+    return [InternetVideo(p, osp.join(root, 'images')) for p in names]

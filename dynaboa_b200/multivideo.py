@@ -46,6 +46,14 @@ def check_options(options, n_videos, dynamic_loop=False):
         raise ValueError(f'{G} videos x {rows} rows per grouped call exceed the 64 samples of the network tape')
 
 
+def video_names(videos, names, default):
+    """The directory names of ``videos`` for ``run``: ``names`` as strings (None: ``default``), one per video."""
+    names = list(default) if names is None else [str(x) for x in names]
+    if len(names) != len(videos):
+        raise ValueError(f'{len(names)} names for {len(videos)} videos')
+    return names
+
+
 def slot_records(frame, G, prev_upper_loss):
     """A pool's (``fit_losses``, ``kp2dlosses_lower``, ``last_upper_loss``) of the ``fused.Frame`` ``frame``: NaN for the slots
     outside the frame, except in ``last_upper_loss``, where they keep ``prev_upper_loss``."""
@@ -353,11 +361,26 @@ class MultiVideoAdaptor:
         video's index)."""
         from .adaptor import write_records
         videos = list(videos)
-        names = [str(i) for i in range(len(videos))] if names is None else [str(x) for x in names]
-        if len(names) != len(videos):
-            raise ValueError(f'{len(names)} names for {len(videos)} videos')
-        queue, its, nxt, out = list(range(len(videos))), [None] * self.G, [None] * self.G, [None] * len(videos)
+        names = video_names(videos, names, default=[str(i) for i in range(len(videos))])
         mean = lambda v: float(np.mean(v)) if len(v) else float('nan')
+
+        def finish(i, g):
+            if g is None:                                    # an empty video
+                return dict(name=names[i], frames=0, mpjpe=float('nan'), pampjpe=float('nan'), pve=float('nan'))
+            rec = self.records(g)
+            if exppath is not None:
+                d = os.path.join(exppath, names[i])
+                os.makedirs(d, exist_ok=True)
+                write_records(d, rec['frames'] - 1, rec)
+            return dict(name=names[i], frames=rec['frames'], mpjpe=mean(rec['mpjpe']), pampjpe=mean(rec['pampjpe']), pve=mean(rec['pve']))
+        return self._queue(videos, self.adapt, finish)
+
+    def _queue(self, videos, tick, finish):
+        """``run``'s queue: the slots are filled in order and refilled as soon as their video ends; video i starts with
+        ``start(g, seed=options.seed * 1000 + i)`` and ``slot_video[g] = i``.  ``tick(items)`` advances the pool by one frame,
+        ``items[g]`` being slot g's next item of its video (None: an idle slot); ``finish(i, g)`` returns video i's summary once
+        it ended in slot g (g None: video i was empty), before the slot is refilled.  Returns the summaries in order."""
+        queue, its, nxt, out = list(range(len(videos))), [None] * self.G, [None] * self.G, [None] * len(videos)
 
         def fill(g):
             self.slot_video[g] = None
@@ -365,31 +388,23 @@ class MultiVideoAdaptor:
                 i = queue.pop(0)
                 its[g] = iter(videos[i])
                 nxt[g] = next(its[g], None)
-                if nxt[g] is None:                           # an empty video
-                    out[i] = dict(name=names[i], frames=0, mpjpe=float('nan'), pampjpe=float('nan'), pve=float('nan'))
+                if nxt[g] is None:
+                    out[i] = finish(i, None)
                     continue
                 self.start(g, seed=self.options.seed * 1000 + i)
                 self.slot_video[g] = i
                 return
 
-        def finish(g):
-            i, rec = self.slot_video[g], self.records(g)
-            out[i] = dict(name=names[i], frames=rec['frames'], mpjpe=mean(rec['mpjpe']), pampjpe=mean(rec['pampjpe']), pve=mean(rec['pve']))
-            if exppath is not None:
-                d = os.path.join(exppath, names[i])
-                os.makedirs(d, exist_ok=True)
-                write_records(d, rec['frames'] - 1, rec)
-
         for g in range(self.G):
             fill(g)
         while any(i is not None for i in self.slot_video):
-            self.adapt([nxt[g] if self.slot_video[g] is not None else None for g in range(self.G)])
+            tick([nxt[g] if self.slot_video[g] is not None else None for g in range(self.G)])
             for g in range(self.G):
                 if self.slot_video[g] is None:
                     continue
                 nxt[g] = next(its[g], None)
                 if nxt[g] is None:
-                    finish(g)
+                    out[self.slot_video[g]] = finish(self.slot_video[g], g)
                     fill(g)
         return out
 
@@ -397,11 +412,16 @@ class MultiVideoAdaptor:
         """Every video's prediction for its rows of ``images`` with its current weights: a list of G dicts with rotmat, betas,
         cam, joints (49) and vertices.  ``active`` (bit mask; None: every slot): one grouped forward of only those slots
         (``dboa_hmr_forward_active``), then the SMPL decode; the entries of the other slots are None."""
-        with torch.no_grad():
-            image = images.to(self.thetas.device).contiguous().float()
-            rot, shape, cam, _, _ = hmr_mod.raw_forward(self.thetas, self.buffers, image, groups=self.G, active=active)
-            out = self.base.decode_smpl_params(rot, shape)
-        b = image.shape[0] // self.G
+        rot, shape, cam, out = self._outputs(images, active)
+        b = rot.shape[0] // self.G
         s = [slice(g * b, (g + 1) * b) for g in range(self.G)]
         return [dict(rotmat=rot[q], betas=shape[q], cam=cam[q], joints=out['s3d'][q], vertices=out['vts'][q])
                 if active is None or (active >> g) & 1 else None for g, q in enumerate(s)]
+
+    def _outputs(self, images, active=None):
+        """``predict``'s grouped forward and SMPL decode as whole (G b, ...) tensors: rotmat, betas, cam and the decode's dict
+        (rows of slots outside ``active`` hold no prediction)."""
+        with torch.no_grad():
+            image = images.to(self.thetas.device).contiguous().float()
+            rot, shape, cam, _, _ = hmr_mod.raw_forward(self.thetas, self.buffers, image, groups=self.G, active=active)
+            return rot, shape, cam, self.base.decode_smpl_params(rot, shape)
