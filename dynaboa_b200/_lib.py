@@ -53,6 +53,9 @@ SIGNATURES = {
     'dboa_version': (C.c_char_p, []),
     'dboa_last_cuda_error': (I, []),
     'dboa_launch_count': (L, []),
+    'dboa_launch_credit': (I, [L]),
+    'dboa_prepare_graph': (I, []),
+    'dboa_stream_wait_external': (I, [P, P]),
     'dboa_set_tensor_core_conv': (I, [I]),
     'dboa_set_fused_forward': (I, [I]),
     'dboa_get_fused_forward': (I, []),
@@ -110,6 +113,8 @@ SIGNATURES = {
     'dboa_adam_ema': (I, [P, P, P, P, P, L, D, D, D, D, I, D, P]),
     'dboa_ema_update': (I, [P, P, L, D, P]),
     'dboa_adam_ema_scaled': (I, [P, P, P, P, P, L, D, D, D, D, I, D, F, P]),
+    'dboa_adam_scalars': (I, [P, D, D, D, D, I, D, F]),
+    'dboa_adam_ema_dev': (I, [P, P, P, P, P, L, P, P]),
     'dboa_fill_zero': (I, [P, L, P]),
     'dboa_copy_async': (I, [P, P, L, P]),
     'dboa_hmr_backward_buckets': (I, [P, P, P]),
@@ -133,6 +138,7 @@ SIGNATURES = {
     'dboa_render_overlay_groups': (I, [C.POINTER(RenderDescStruct), I, P, P, P, I, I, I, P, L, P]),
 }
 
+ADAM_SCALARS = 9              # DBOA_ADAM_SCALARS: floats of dboa_adam_scalars' block
 _ERRORS = {-1: 'DBOA_ERR_ARG', -2: 'DBOA_ERR_SHAPE', -3: 'DBOA_ERR_CUDA', -4: 'DBOA_ERR_UNSUPPORTED'}
 _lib = None
 

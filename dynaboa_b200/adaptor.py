@@ -10,15 +10,19 @@ Two entry points per frame:
   arena, Adam and the teacher EMA fused in one sweep, no host syncs except the ``dynamic_boa`` decision
   (see fused.py).  This is what ``bench.py`` times.
 """
+import os
 import os.path as osp
 import random
 
 import numpy as np
 import torch
 
-from . import _lib, constants
+from . import _lib, constants, hmr as hmr_mod
 from .base_adaptor import BaseAdaptor
-from .fused import Step, _ArenaModel, fused_adapt
+from .fused import Frame, Step, _ArenaModel, fused_adapt
+
+# DBOA_STEP_GRAPH=0 in the environment runs every frame of ``adapt`` eagerly (A/B measurements, debugging)
+STEP_GRAPH = os.environ.get('DBOA_STEP_GRAPH', '1') != '0'
 
 
 RESULT_FILES = ('lowerlevel_kp2dloss.pt', 'upperlevel_kp2dloss.pt', 'res.pt', 'lower_res.pt', 'steps_statistic_res.pt', 'feat_sims.pt',
@@ -50,9 +54,35 @@ def write_records(exppath, step, rec):
             f.write(f'Lower-level  Step:{i} MPJPE:{lo_m}, PAMPJPE:{lo_p}\n')
 
 
+class _StepGraph:
+    """One single-video frame of ``fused_adapt`` captured as a CUDA graph: its static inputs (frame, keypoints, history frame),
+    the graph, its records packed into one (n,) tensor and the number of library kernels it holds.  ``key``: the
+    configuration it was captured in (``Adaptor._graph_key``)."""
+
+    def __init__(self, key, image, kp):
+        self.key, self.graph, self.launches = key, None, 0
+        new = lambda t: torch.empty(t.shape, dtype=torch.float32, device=t.device)
+        self.image, self.kp, self.hist_image, self.hist_kp = new(image), new(kp), new(image), new(kp)
+
+    def pack(self, f):
+        """Inside the capture: every record of the ``Frame`` f (one float each, G = 1) into ``packed``."""
+        self.names, self.n_lower = list(f.fit), len(f.lower)
+        self.packed = torch.cat([t.reshape(1) for t in [f.fit[k] for k in self.names] + list(f.lower) + [f.upper_loss]])
+
+    def frame(self):
+        """The ``Frame`` of the last replay, from a copy of ``packed``: the next replay does not change it."""
+        p, n = self.packed.clone(), len(self.names)
+        f = Frame(1)
+        f.fit = {k: p[i:i + 1] for i, k in enumerate(self.names)}
+        f.lower = [p[n + i:n + i + 1] for i in range(self.n_lower)]
+        f.upper_loss = p[-1:]
+        return f
+
+
 class Adaptor(BaseAdaptor):
     kp_range = (25, 24)          # joints of the 2D and motion terms (fused.Step)
     motion_lead = 0              # the motion term is live while global_step + motion_lead - interval > 0 (before save_hist)
+    step_graph = True            # adapt may replay its steady-state frame as a CUDA graph (see _graph_key)
 
     def __init__(self, options):
         super().__init__(options)
@@ -60,6 +90,8 @@ class Adaptor(BaseAdaptor):
         self.reset_records()
         self.fused_eval = 'final'                          # adapt's evaluations: 'none', 'final' or 'all'
         self.phase_events = None                           # a list: adapt records CUDA events at its phase boundaries
+        self._graph, self._graph_warm = None, None         # adapt's captured frame; the key of the last eager frame
+        self._weights_read = None                          # recorded by predict_async after its read of the weights
 
     def reset_records(self):
         n = len(self.dataloader)
@@ -171,6 +203,9 @@ class Adaptor(BaseAdaptor):
             out = self.predict(image)
             ev = torch.cuda.Event()
             ev.record(side)
+            if self._weights_read is None:
+                self._weights_read = torch.cuda.Event()
+            self._weights_read.record(side)                # what a captured optimiser step waits for (external wait)
         image.record_stream(side)
         for v in out.values():                             # allocated on the side stream, read by the caller's stream after the event
             v.record_stream(cur)
@@ -229,12 +264,25 @@ class Adaptor(BaseAdaptor):
 
     # ------------------------------------------------------------------ the same step without autograd (fused.py)
     def adapt(self, batch):
-        """One frame through ``fused.fused_adapt``, its records filed under the reference's names; returns ``inference``'s."""
+        """One frame through ``fused.fused_adapt``, its records filed under the reference's names; returns ``inference``'s.
+
+        In the steady state of a single video (``_graph_key``) the frame is captured once as a CUDA graph, after one eager
+        frame in the same configuration, and replayed from then on: same kernels, grids and order, so every result is the
+        eager frame's, bit for bit, without the host-side cost of enqueueing some 800 launches."""
         import torch.distributed as dist
+        key = self._graph_key(batch)
+        if key is not None and self._graph is not None and self._graph.key == key:
+            return self._file(self._replay(batch))
+        if key is not None and self._graph_warm == key:
+            return self._file(self._capture(batch, key))
         s, opt = self._step or self._make_step(), self.optimizer
         s.eval_mode, s.phase_events = self.fused_eval, self.phase_events
         s.grad_sync = opt.grad_sync if (opt.grad_sync is not None and dist.is_initialized() and dist.get_world_size() > 1) else None
         f = fused_adapt(s, batch, 1, [self.global_step])
+        self._graph_warm = key
+        return self._file(f)
+
+    def _file(self, f):
         self.fit_losses.update({k: v[0] for k, v in f.fit.items()})
         self.kp2dlosses_lower += [v[0] for v in f.lower]
         if 'ul/s2dloss' in f.fit:
@@ -246,6 +294,78 @@ class Adaptor(BaseAdaptor):
             self.feat_sims[self.global_step], self.optimized_step = f.sims[0], f.steps[0]
             self.optim_step_record.append(f.steps[0])
         return f.result
+
+    # ------------------------------------------------------------------ the frame as a CUDA graph
+    def _graph_key(self, batch):
+        """The configuration a captured frame of ``batch`` is valid in, or None when the frame runs eagerly.  A graph needs a
+        frame whose every host-side decision is fixed: one video on one GPU, no retrieval (its cluster index goes through the
+        host), no dynamic loop (its trip count does), no evaluation, the motion term live, the teacher's dropout from torch's
+        generator (a replay draws as an eager frame does), the default network plan; and the same tensors as at capture."""
+        o, opt = self.options, self.optimizer
+        if not (STEP_GRAPH and self.step_graph and o.use_boa) or o.retrieval or o.dynamic_boa or self.fused_eval != 'none':
+            return None
+        if self.phase_events is not None or opt.grad_sync is not None or opt.pre_step_hook is not None:
+            return None
+        if self.global_step + self.motion_lead - o.interval <= 0:
+            return None
+        masked = False
+        if o.use_meanteacher:
+            if self.teacher.mask_provider is not None or hmr_mod.DEFAULT_MASK_PROVIDER is not None:
+                return None
+            masked = self.teacher.training
+        lib = _lib.load()
+        if lib.dboa_get_fused_forward() or lib.dboa_get_fused_backward():
+            return None
+        s = self._step or self._make_step()
+        image, kp = batch['image'], batch['smpl_j2d']
+        arenas = (s.theta, s.grad, s.teacher, opt.m, opt.v)
+        return (id(s), tuple(None if t is None else t.data_ptr() for t in arenas), masked, tuple(image.shape), image.device,
+                tuple(kp.shape))
+
+    def _graph_prologue(self, g, batch):
+        """What a replayed frame takes from the host: the frame and its keypoints, the history (saved here, as ``fused_adapt``
+        saves it) and the step's Adam scalars.  The graph waits for ``predict_async``'s reads through ``_weights_read``."""
+        g.image.copy_(batch['image'])
+        g.kp.copy_(batch['smpl_j2d'])
+        self.save_hist(g.image, g.kp)
+        hist_image, hist_kp = self.get_hist()
+        g.hist_image.copy_(hist_image)
+        g.hist_kp.copy_(hist_kp)
+        self.optimizer.write_scalars(self.options.alpha)
+        self.optimizer.wait_before_write = []
+
+    def _capture(self, batch, key):
+        s, lib = self._step, _lib.load()
+        _lib.check(lib.dboa_prepare_graph(), 'dboa_prepare_graph')
+        if self._weights_read is None:                     # the captured wait needs an event; recorded once, it is a no-op
+            self._weights_read = torch.cuda.Event()
+            self._weights_read.record()
+        g = _StepGraph(key, batch['image'], batch['smpl_j2d'])
+        self._graph_prologue(g, batch)
+        s.eval_mode, s.phase_events, s.grad_sync = 'none', None, None
+        hooks = s.save_hist, s.get_hist, s.adam
+        s.save_hist = lambda image, kp, mask: None
+        s.get_hist = lambda live: (g.hist_image, g.hist_kp)
+        s.adam = lambda mask, teacher=None, alpha=0.0: self.optimizer.step_captured(
+            self._weights_read, teacher=None if teacher is None else self.teacher)
+        graph = torch.cuda.CUDAGraph()
+        n0 = lib.dboa_launch_count()
+        try:
+            with torch.cuda.graph(graph, capture_error_mode='thread_local'):
+                g.pack(fused_adapt(s, {'image': g.image, 'smpl_j2d': g.kp}, 1, [self.global_step]))
+        finally:
+            s.save_hist, s.get_hist, s.adam = hooks
+        g.graph, g.launches = graph, lib.dboa_launch_count() - n0
+        self._graph = g
+        graph.replay()                                     # this frame: its kernels were counted as they were captured
+        return g.frame()
+
+    def _replay(self, batch):
+        g = self._graph
+        self._graph_prologue(g, batch)
+        g.graph.replay()
+        _lib.call('dboa_launch_credit', g.launches)
+        return g.frame()
 
     def _make_step(self):
         o = self.options

@@ -18,6 +18,7 @@ int hmr_backward(const float* P, const float* T, int B, int masked, const float*
 void hmr_arm_bucket_events(cudaEvent_t e0, cudaEvent_t e1, cudaEvent_t e2);
 long long hmr_bucket_offset(int k);
 void hmr_set_fused_forward(bool on);
+int hmr_prepare();
 void hmr_set_fused_backward(bool on);
 bool hmr_fused_forward();
 bool hmr_fused_backward();
@@ -71,6 +72,18 @@ extern "C" {
 const char* dboa_version(void) { return "dynaboa_b200 0.1 (sm_90a)"; }
 int dboa_last_cuda_error(void) { return g_last_cuda_error; }
 long long dboa_launch_count(void) { return g_launch_count; }
+int dboa_launch_credit(long long n) {
+    if (n < 0) return DBOA_ERR_ARG;
+    g_launch_count += n;
+    return DBOA_OK;
+}
+int dboa_prepare_graph(void) { return hmr_prepare(); }
+int dboa_stream_wait_external(dboa_stream_t stream, void* event) {
+    if (!event) return DBOA_ERR_ARG;
+    cudaError_t e = cudaStreamWaitEvent(ST(stream), reinterpret_cast<cudaEvent_t>(event), cudaEventWaitExternal);
+    if (e != cudaSuccess) { g_last_cuda_error = (int)e; return DBOA_ERR_CUDA; }
+    return DBOA_OK;
+}
 int dboa_set_tensor_core_conv(int enable) { conv_tc_set_mode(enable); return DBOA_OK; }
 
 int dboa_set_fused_forward(int enable) { hmr_set_fused_forward(enable != 0); return DBOA_OK; }
@@ -324,6 +337,15 @@ int dboa_adam_ema_scaled(float* p, const float* g, float* m, float* v, float* te
                          double eps, int step, double alpha, float gscale, dboa_stream_t stream) {
     if (!p || !g || !m || !v || n < 0) return DBOA_ERR_ARG;
     return adam_ema(p, g, m, v, teacher, (size_t)n, lr, beta1, beta2, eps, step, alpha, gscale, ST(stream));
+}
+int dboa_adam_scalars(float* out, double lr, double beta1, double beta2, double eps, int step, double alpha, float gscale) {
+    if (!out || step < 1) return DBOA_ERR_ARG;
+    adam_scalars(lr, beta1, beta2, eps, step, alpha, gscale, out);
+    return DBOA_OK;
+}
+int dboa_adam_ema_dev(float* p, const float* g, float* m, float* v, float* teacher, long long n, const float* scalars, dboa_stream_t stream) {
+    if (!p || !g || !m || !v || !scalars || n < 0) return DBOA_ERR_ARG;
+    return adam_ema_dev(p, g, m, v, teacher, (size_t)n, scalars, ST(stream));
 }
 int dboa_fill_zero(void* dst, long long bytes, dboa_stream_t stream) {
     if (!dst || bytes < 0) return DBOA_ERR_ARG;

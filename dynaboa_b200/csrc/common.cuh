@@ -12,7 +12,7 @@
 namespace dboa {
 
 extern int g_last_cuda_error;      // set by check_launch (defined in hmr_plan.cu)
-extern int g_launch_count;         // number of kernels this library launched (bench "gpu_launches")
+extern long long g_launch_count;   // number of kernels this library launched (bench "gpu_launches"; replayed graphs credit theirs)
 
 inline int check_launch() {
     ++g_launch_count;
@@ -44,6 +44,14 @@ __device__ __forceinline__ float block_sum(float v, float* smem32) {
 __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
+
+// True while `st` is being captured into a CUDA graph (or its state cannot be read).  One-time set-up on the launch path
+// (allocations, stream / event creation, function attributes) is refused then with DBOA_ERR_UNSUPPORTED, before anything is
+// enqueued: dboa_prepare_graph does it ahead of a capture, as does the first eager call.
+inline bool stream_capturing(cudaStream_t st) {
+    cudaStreamCaptureStatus s = cudaStreamCaptureStatusNone;
+    return cudaStreamIsCapturing(st, &s) != cudaSuccess || s != cudaStreamCaptureStatusNone;
+}
 
 // SM count of the current device (queried once per process: one process drives one GPU)
 inline int num_sms() {
@@ -84,6 +92,7 @@ inline int launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t sme
         const unsigned have = slot >= 0 ? seen_bits[slot] : 0u;
         const unsigned want = (csize > 8 ? 1u : 0u) | (smem > 48 * 1024 ? 2u : 0u);
         if (want & ~have) {
+            if (stream_capturing(st)) return DBOA_ERR_UNSUPPORTED;
             cudaError_t e = cudaSuccess;
             if ((want & ~have) & 1u) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
             if (e == cudaSuccess && ((want & ~have) & 2u)) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);

@@ -65,6 +65,7 @@ static unsigned* sync_words() {
     }
     return g_sync_base;
 }
+int gn_prepare() { return sync_words() ? DBOA_OK : DBOA_ERR_CUDA; }
 
 // sums of two values over the CTA (fixed tree); valid in every thread.  `red` holds 64 floats and is used once.
 __device__ __forceinline__ float2 block_sum2(float a, float b, float* red) {
@@ -315,6 +316,7 @@ int gn_bwd_fused(const float* dout, const float* mask_src, const float* y, const
     if (bper <= 0) bper = B;
     if (!gn_plan(HW, C, &pl) || (C / 16) > 128 || B % bper != 0) return DBOA_ERR_SHAPE;
     if (bper < B && !defer) return DBOA_ERR_UNSUPPORTED;       // per-group affine gradients are reduced by gn_param_finish
+    if (g_sync_base == nullptr && stream_capturing(st)) return DBOA_ERR_UNSUPPORTED;
     unsigned* cnt = sync_words();
     if (!cnt) return DBOA_ERR_CUDA;
     return launch_ex(gn_bwd_fused_kernel, dim3(pl.chunks, GN_G, B), dim3(GN_NT), 0, st, dim3(pl.chunks, 1, 1), true, dout, mask_src, y, stats,

@@ -18,7 +18,7 @@
 namespace dboa {
 
 int g_last_cuda_error = 0;
-int g_launch_count = 0;
+long long g_launch_count = 0;
 bool pdl_enabled() {
     static const bool on = [] { const char* e = getenv("DBOA_PDL"); return !(e && e[0] == '0'); }();
     return on;
@@ -281,27 +281,47 @@ void hmr_set_fused_forward(bool on) { g_fused_fwd = on; }
 bool hmr_fused_forward() { return g_fused_fwd; }
 bool hmr_fused_backward() { return g_fused_bwd; }
 
-// table for gn_param_finish: where each GroupNorm's affine gradients live and where its per-sample rows start
-struct GnItems { std::vector<long long> cum; GnFinishItem* dev = nullptr; };
-static const GnItems& gn_items() {
+// table for gn_param_finish: where each GroupNorm's affine gradients live and where its per-sample rows start (the device copy
+// is made by hmr_prepare)
+struct GnItems { std::vector<long long> cum; std::vector<GnFinishItem> host; GnFinishItem* dev = nullptr; };
+static GnItems& gn_items() {
     static GnItems gi = [] {
         GnItems g;
-        const Net& n = net();
-        std::vector<GnFinishItem> host;
         long long cum = 0;
-        for (const ConvLayer& c : n.convs) {
+        for (const ConvLayer& c : net().convs) {
             g.cum.push_back(cum);
-            host.push_back(GnFinishItem{c.g_off, c.b_off, cum, c.cout});
+            g.host.push_back(GnFinishItem{c.g_off, c.b_off, cum, c.cout});
             cum += c.cout;
         }
-        void* p = nullptr;
-        if (cudaMalloc(&p, host.size() * sizeof(GnFinishItem)) == cudaSuccess &&
-            cudaMemcpy(p, host.data(), host.size() * sizeof(GnFinishItem), cudaMemcpyHostToDevice) == cudaSuccess)
-            g.dev = static_cast<GnFinishItem*>(p);
         return g;
     }();
     return gi;
 }
+
+// Everything the backward creates once: the weight-gradient side streams and events, the data-parallel join stream and events,
+// the GroupNorm item table on the device and the GroupNorm sync words.  Made by the first backward, or ahead of a CUDA graph
+// capture by dboa_prepare_graph (while a stream captures, none of it may be created: the capture would be invalidated).
+static bool g_prepared = false;
+int hmr_prepare() {
+    if (g_prepared) return DBOA_OK;
+    DBOA_TRY(device_guard());
+    if (!g_async.init()) return DBOA_ERR_CUDA;
+    if (g_join_stream == nullptr && cudaStreamCreateWithFlags(&g_join_stream, cudaStreamNonBlocking) != cudaSuccess) return DBOA_ERR_CUDA;
+    for (int i = 0; i < 4; ++i)
+        if (g_join_ev[i] == nullptr && cudaEventCreateWithFlags(&g_join_ev[i], cudaEventDisableTiming) != cudaSuccess) return DBOA_ERR_CUDA;
+    GnItems& gi = gn_items();
+    if (gi.dev == nullptr) {
+        void* p = nullptr;
+        const size_t bytes = gi.host.size() * sizeof(GnFinishItem);
+        if (cudaMalloc(&p, bytes) != cudaSuccess) return DBOA_ERR_CUDA;
+        if (cudaMemcpy(p, gi.host.data(), bytes, cudaMemcpyHostToDevice) != cudaSuccess) { cudaFree(p); return DBOA_ERR_CUDA; }
+        gi.dev = static_cast<GnFinishItem*>(p);
+    }
+    DBOA_TRY(gn_prepare());
+    g_prepared = true;
+    return DBOA_OK;
+}
+
 // backward convolutions: wgmma implicit GEMM when enabled and the shape is taken, else the fp32 CUDA-core kernels
 static int conv_backward_data(const ConvLayer& c, int B, int groups, unsigned long long active, const float* dy, const float* w, float* dx,
                               int accumulate, float* ws, cudaStream_t st);
@@ -563,10 +583,9 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
     const bool masked = masked_in != 0;     // the forward ran with dropout keep-masks (saved in the tape)
     BucketReq breq = g_bucket_req;
     g_bucket_req.armed = false;
-    if (breq.armed) {
-        if (g_join_stream == nullptr && cudaStreamCreateWithFlags(&g_join_stream, cudaStreamNonBlocking) != cudaSuccess) return DBOA_ERR_CUDA;
-        for (int i = 0; i < 4; ++i)
-            if (g_join_ev[i] == nullptr && cudaEventCreateWithFlags(&g_join_ev[i], cudaEventDisableTiming) != cudaSuccess) return DBOA_ERR_CUDA;
+    if (!g_prepared) {
+        if (stream_capturing(st)) return DBOA_ERR_UNSUPPORTED;
+        DBOA_TRY(hmr_prepare());
     }
 
     // ---- head
@@ -602,7 +621,7 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
     float* dIn = sc.g1;
     DBOA_TRY(avgpool_bwd(sc.dxf, 2048, dOut, B, 49, 2048, st));
     float* const tmp[6] = {sc.t1, sc.t2, sc.t3, sc.t4, sc.t5, sc.t6};
-    const bool async = g_async_enabled && g_async.init();
+    const bool async = g_async_enabled;
     BwdAsync& A = g_async;
     if (async) {                                   // the side stream starts after everything enqueued so far
         for (int i = 0; i < 8; ++i) A.pending[i] = false;
@@ -638,7 +657,6 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
     auto bucket_done = [&](int k, int first_conv) {
         if (B > 1 && first_conv < finished_from) {
             const GnItems& gi = gn_items();
-            if (gi.dev == nullptr) return DBOA_ERR_CUDA;
             DBOA_TRY(gn_param_finish(gi.dev + first_conv, finished_from - first_conv, sc.gnp, G, B, st, groups, PS, active));
             finished_from = first_conv;
         }
@@ -684,7 +702,6 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
         }
         auto finish_fixed = [&](int first_conv, int end_conv) {
             const GnItems& gi = gn_items();
-            if (gi.dev == nullptr) return DBOA_ERR_CUDA;
             return gn_dgb_finish(gi.dev + first_conv, end_conv - first_conv, sc.bdgb, G, st);
         };
         int fixed_from = (int)n.convs.size();

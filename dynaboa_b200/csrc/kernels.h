@@ -95,6 +95,7 @@ int gn_fwd_fused(const float* y, const float* gamma, const float* beta, const fl
 int gn_bwd_fused(const float* dout, const float* mask_src, const float* y, const float* stats, const float* gamma, float* dy,
                  float* dgamma, float* dbeta, float* partial, int B, int HW, int C, cudaStream_t st, int defer = 0, int bper = 0,
                  long long pstride = 0);
+int gn_prepare();                                   // the backward's cluster sync words (allocated once, before any capture)
 struct GnFinishItem { long long g_off, b_off, cum_channels; int C; };
 // rows of samples [g * B / groups, (g + 1) * B / groups) are added to G + g * pstride (groups whose `active` bit is set)
 int gn_param_finish(const GnFinishItem* items_dev, int n_items, const float* rows, float* G, int B, cudaStream_t st, int groups = 1,

@@ -44,10 +44,10 @@ __device__ __forceinline__ void adam_one(float& p, float g, float& m, float& v, 
     p = __fadd_rn(p, __fmul_rn(neg_step, __fdiv_rn(m, denom)));
 }
 
-__global__ void __launch_bounds__(256) adam_ema_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                                                       float* __restrict__ v, float* __restrict__ teacher, size_t n4, float w1, float b2,
-                                                       float one_m_b2, float bc2_sqrt, float eps, float neg_step, float alpha,
-                                                       float one_m_alpha, float gscale) {
+// one grid-stride Adam (+ EMA) sweep; the two kernels below differ only in where they read their scalars from
+__device__ __forceinline__ void adam_ema_sweep(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+                                               float* __restrict__ teacher, size_t n4, float w1, float b2, float one_m_b2, float bc2_sqrt,
+                                               float eps, float neg_step, float alpha, float one_m_alpha, float gscale) {
     for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n4; i += (size_t)gridDim.x * 256) {
         float4 pp = reinterpret_cast<float4*>(p)[i], gg = reinterpret_cast<const float4*>(g)[i];
         float4 mm = reinterpret_cast<float4*>(m)[i], vv = reinterpret_cast<float4*>(v)[i];
@@ -68,15 +68,36 @@ __global__ void __launch_bounds__(256) adam_ema_kernel(float* __restrict__ p, co
         }
     }
 }
-int adam_ema(float* p, const float* g, float* m, float* v, float* teacher, size_t n, double lr, double beta1, double beta2, double eps,
-             int step, double alpha, float gscale, cudaStream_t st) {
-    if (n % 4 || step < 1) return DBOA_ERR_ARG;
+__global__ void __launch_bounds__(256) adam_ema_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                                                       float* __restrict__ v, float* __restrict__ teacher, size_t n4, float w1, float b2,
+                                                       float one_m_b2, float bc2_sqrt, float eps, float neg_step, float alpha,
+                                                       float one_m_alpha, float gscale) {
+    adam_ema_sweep(p, g, m, v, teacher, n4, w1, b2, one_m_b2, bc2_sqrt, eps, neg_step, alpha, one_m_alpha, gscale);
+}
+// the scalars from a device block (adam_scalars' order): a replayed CUDA graph reads the bias correction of the current step
+__global__ void __launch_bounds__(256) adam_ema_dev_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                                                           float* __restrict__ v, float* __restrict__ teacher, size_t n4,
+                                                           const float* __restrict__ s) {
+    adam_ema_sweep(p, g, m, v, teacher, n4, s[0], s[1], s[2], s[3], s[4], s[5], s[6], s[7], s[8]);
+}
+void adam_scalars(double lr, double beta1, double beta2, double eps, int step, double alpha, float gscale, float out[ADAM_SCALARS]) {
     // torch.optim.Adam (single-tensor path) derives these from the hyperparameters in Python doubles, then casts each
     // scalar once to fp32: so does this, from the caller's doubles (1 - beta2 of a float-rounded beta2 is off by ulps)
     const double bc1 = 1.0 - pow(beta1, step), bc2 = 1.0 - pow(beta2, step);
-    adam_ema_kernel<<<sweep_grid(n / 4), 256, 0, st>>>(p, g, m, v, teacher, n / 4, (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2),
-                                                       (float)sqrt(bc2), (float)eps, (float)(-(lr / bc1)), (float)alpha,
-                                                       (float)(1.0 - alpha), gscale);
+    out[0] = (float)(1.0 - beta1); out[1] = (float)beta2; out[2] = (float)(1.0 - beta2); out[3] = (float)sqrt(bc2); out[4] = (float)eps;
+    out[5] = (float)(-(lr / bc1)); out[6] = (float)alpha; out[7] = (float)(1.0 - alpha); out[8] = gscale;
+}
+int adam_ema(float* p, const float* g, float* m, float* v, float* teacher, size_t n, double lr, double beta1, double beta2, double eps,
+             int step, double alpha, float gscale, cudaStream_t st) {
+    if (n % 4 || step < 1) return DBOA_ERR_ARG;
+    float s[ADAM_SCALARS];
+    adam_scalars(lr, beta1, beta2, eps, step, alpha, gscale, s);
+    adam_ema_kernel<<<sweep_grid(n / 4), 256, 0, st>>>(p, g, m, v, teacher, n / 4, s[0], s[1], s[2], s[3], s[4], s[5], s[6], s[7], s[8]);
+    return check_launch();
+}
+int adam_ema_dev(float* p, const float* g, float* m, float* v, float* teacher, size_t n, const float* scalars, cudaStream_t st) {
+    if (n % 4) return DBOA_ERR_ARG;
+    adam_ema_dev_kernel<<<sweep_grid(n / 4), 256, 0, st>>>(p, g, m, v, teacher, n / 4, scalars);
     return check_launch();
 }
 

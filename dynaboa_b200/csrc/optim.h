@@ -19,6 +19,12 @@ struct CosinePairs {
 int sgd_update(const float* p, const float* g, float* out, float lr, size_t n, cudaStream_t st);
 int adam_ema(float* p, const float* g, float* m, float* v, float* teacher, size_t n, double lr, double beta1, double beta2, double eps,
              int step, double alpha, float gscale, cudaStream_t st);
+// the fp32 scalars of one Adam (+ EMA) sweep, in this order: 1 - beta1, beta2, 1 - beta2, sqrt(bias correction 2), eps,
+// -(lr / bias correction 1), alpha, 1 - alpha, gscale
+constexpr int ADAM_SCALARS = 9;
+void adam_scalars(double lr, double beta1, double beta2, double eps, int step, double alpha, float gscale, float out[ADAM_SCALARS]);
+// adam_ema with the scalars read from the device block `scalars` (ADAM_SCALARS floats) when the kernel runs
+int adam_ema_dev(float* p, const float* g, float* m, float* v, float* teacher, size_t n, const float* scalars, cudaStream_t st);
 int ema_update(float* teacher, const float* p, size_t n, double alpha, cudaStream_t st);
 // out[i] = cos(a_i, b_i) (NULL to skip); terms[i] = (a.b, |a|^2, |b|^2) in double (NULL to skip): the data-parallel feature test all-reduces them.
 // Per video g whose bit is set in `active`: out[g][i], terms[g][i], each from video g's parts alone; the rows of other videos

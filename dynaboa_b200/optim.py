@@ -5,6 +5,8 @@ Drop-in for ``torch.optim.Adam(model.parameters(), lr, betas)`` as the reference
 Adam, but one kernel launch for all 169 tensors (``dboa_adam_ema``), optionally folding
 ``update_teacher`` (base_adaptor.py:193-201) into the same sweep.
 """
+import ctypes as C
+
 import torch
 
 from . import _lib
@@ -34,6 +36,7 @@ class FusedAdam(torch.optim.Optimizer):
         self.reduced = False                                   # the gradient of the coming step has already been all-reduced
         self.gscale = 1.0                                      # g * gscale inside the sweep (1 / world under data parallelism)
         self.wait_before_write = []                            # events of side-stream readers of the weights (Adaptor.predict_async)
+        self.scalars = None                                    # device block of step_captured's scalars (write_scalars)
 
     def _gather_grads(self):
         """Make sure every ``p.grad`` lives in the flat gradient arena (autograd may have re-created them)."""
@@ -81,6 +84,30 @@ class FusedAdam(torch.optim.Optimizer):
         _lib.call('dboa_adam_ema_scaled', ptr(self.model.arena), ptr(g), ptr(self.m), ptr(self.v), ptr(t), self.model.arena.numel(),
                   float(grp['lr']), float(grp['betas'][0]), float(grp['betas'][1]), float(grp['eps']), self.step_count, float(alpha),
                   float(self.gscale), stream())
+
+    # ---- the same step split for a CUDA graph: scalars written eagerly before each replay, the sweep captured once
+    def write_scalars(self, alpha):
+        """Advance ``step_count`` and write the fp32 scalars of its sweep (``dboa_adam_scalars``, the arithmetic of ``step``) to
+        the device block that ``step_captured`` reads; an asynchronous copy on the current stream."""
+        grp = self.param_groups[0]
+        self.step_count += 1
+        host = torch.empty(_lib.ADAM_SCALARS, dtype=torch.float32, pin_memory=True)
+        _lib.call('dboa_adam_scalars', ptr(host), float(grp['lr']), float(grp['betas'][0]), float(grp['betas'][1]), float(grp['eps']),
+                  self.step_count, float(alpha), float(self.gscale))
+        if self.scalars is None:
+            self.scalars = torch.empty(_lib.ADAM_SCALARS, dtype=torch.float32, device=self.m.device)
+        self.scalars.copy_(host, non_blocking=True)
+
+    @torch.no_grad()
+    def step_captured(self, read_event, teacher=None):
+        """``step`` for a graph capture: waits for the latest record of ``read_event`` (made outside the graph by the side-stream
+        readers of the weights) and sweeps with the scalars of the ``scalars`` block, both at replay time.  No gradient
+        all-reduce."""
+        g = self._gather_grads()
+        _lib.call('dboa_stream_wait_external', stream(), C.c_void_p(read_event.cuda_event))
+        t = None if teacher is None else teacher.arena
+        _lib.call('dboa_adam_ema_dev', ptr(self.model.arena), ptr(g), ptr(self.m), ptr(self.v), ptr(t), self.model.arena.numel(),
+                  ptr(self.scalars), stream())
 
 
 def ema_update(teacher, model, alpha):

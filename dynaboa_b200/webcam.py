@@ -49,6 +49,7 @@ def webcam_options(o):
 class WebcamAdaptor(Adaptor):
     kp_range = (0, 25)
     motion_lead = 1                                         # save_hist advances global_step before the levels
+    step_graph = False                                      # a replayed frame could not advance it
 
     def __init__(self, options):
         super().__init__(webcam_options(options))

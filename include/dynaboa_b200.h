@@ -30,6 +30,15 @@ typedef void* dboa_stream_t;
 const char* dboa_version(void);
 int dboa_last_cuda_error(void);            /* cudaError_t of the last failed launch */
 long long dboa_launch_count(void);         /* kernels launched by this library so far */
+/* add n >= 0 to dboa_launch_count: the kernels of a replayed CUDA graph, counted once when they were captured */
+int dboa_launch_credit(long long n);
+/* the one-time set-up of the network backward (side streams, events, device tables), made ahead of a CUDA graph capture; the
+ * first eager backward makes it otherwise.  A library call that would still need set-up while its stream is being captured
+ * returns DBOA_ERR_UNSUPPORTED and enqueues nothing. */
+int dboa_prepare_graph(void);
+/* cudaStreamWaitEvent(stream, event, cudaEventWaitExternal): captured into a graph, the wait applies on every replay to the
+ * event's latest record made outside the graph (event: a cudaEvent_t) */
+int dboa_stream_wait_external(dboa_stream_t stream, void* event);
 /* which convolution products of the HMR plan run on the wgmma TF32x3 kernel -- 0: none (fp32 CUDA cores); 1: forward;
  * 2: forward + dgrad + wgrad; 3 (default, faster on H100 at batch 1): forward + dgrad, weight gradients on CUDA cores */
 int dboa_set_tensor_core_conv(int mode);
@@ -291,6 +300,15 @@ int dboa_ema_update(float* teacher, const float* p, long long n, double alpha, d
 /* Adam(+EMA) on g * gscale: the data-parallel mean of an all-reduced (summed) gradient without a separate sweep */
 int dboa_adam_ema_scaled(float* p, const float* g, float* m, float* v, float* teacher /* or NULL */, long long n, double lr, double beta1,
                          double beta2, double eps, int step, double alpha, float gscale, dboa_stream_t stream);
+/* the DBOA_ADAM_SCALARS fp32 scalars of one dboa_adam_ema_scaled sweep, derived on the host as it derives them, into the host
+ * array out: 1 - beta1, beta2, 1 - beta2, sqrt(bias correction 2), eps, -(lr / bias correction 1), alpha, 1 - alpha, gscale */
+#define DBOA_ADAM_SCALARS 9
+int dboa_adam_scalars(float* out, double lr, double beta1, double beta2, double eps, int step, double alpha, float gscale);
+/* dboa_adam_ema_scaled with its scalars read from the device block `scalars` (dboa_adam_scalars' order) when the kernel runs:
+ * a sweep captured into a CUDA graph takes the step's bias correction from the block, written before each replay; same
+ * arithmetic, bit for bit */
+int dboa_adam_ema_dev(float* p, const float* g, float* m, float* v, float* teacher /* or NULL */, long long n, const float* scalars,
+                      dboa_stream_t stream);
 /* stream-ordered fill / device-to-device copy on the copy engine (gradient arenas, frame staging: no ATen kernels in a step) */
 int dboa_fill_zero(void* dst, long long bytes, dboa_stream_t stream);
 int dboa_copy_async(void* dst, const void* src, long long bytes, dboa_stream_t stream);
