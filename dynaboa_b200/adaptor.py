@@ -234,9 +234,9 @@ class Adaptor(BaseAdaptor):
         return mpjpe * 1000, pampjpe * 1000, pve * 1000
 
     def eval_metrics(self, pred_vertices, gt_vertices, gt_vertices_neutral, groups=1, active=None):
-        """(B,3) device tensor: MPJPE, PA-MPJPE, PVE (metres) of each sample -- ``dboa_eval_metrics``.  ``groups`` videos of
-        B / groups rows each, of which only those whose bit is set in ``active`` (an int; None: all) are evaluated
-        (``dboa_eval_metrics_active``): the rows of the others are left unwritten."""
+        """(B,3) device tensor: MPJPE, PA-MPJPE, PVE (metres) of each sample -- ``dboa_eval_metrics_active``.  ``groups``
+        videos of B / groups rows each, of which only those whose bit is set in ``active`` (an int; None: all) are evaluated:
+        the rows of the others are left unwritten."""
         B, dev = pred_vertices.shape[0], pred_vertices.device
         if getattr(self, '_eval_consts', None) is None or self._eval_consts[0].device != dev:
             self._eval_consts = (self.J_regressor.to(dev).contiguous().float(),
@@ -248,10 +248,7 @@ class Adaptor(BaseAdaptor):
         keep = [t.contiguous().float() for t in (pred_vertices, gt_vertices, gt_vertices_neutral)]
         args = (_lib.ptr(keep[0]), _lib.ptr(keep[1]), _lib.ptr(keep[2]), _lib.ptr(J), int(J.shape[0]), int(pred_vertices.shape[1]), _lib.ptr(jmap),
                 int(jmap.numel()), _lib.ptr(scratch), _lib.ptr(out), B)
-        if groups == 1 and active is None:
-            _lib.call('dboa_eval_metrics', *args, _lib.stream())
-        else:
-            _lib.call('dboa_eval_metrics_active', *args, int(groups), (1 << int(groups)) - 1 if active is None else int(active), _lib.stream())
+        _lib.call('dboa_eval_metrics_active', *args, int(groups), (1 << int(groups)) - 1 if active is None else int(active), _lib.stream())
         return out
 
     def _gt_meshes(self, batch):

@@ -15,8 +15,6 @@ CUDA_SOURCES = ['conv.cu', 'conv_tc.cu', 'stem_wgrad.cu', 'groupnorm.cu', 'gn_fu
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
               '--expt-relaxed-constexpr', '-Xptxas', '-v']
-if os.environ.get('DBOA_TIMELINE') == '1':          # diagnostic build: in-kernel phase timestamps (conv_tc.cu)
-    NVCC_FLAGS.append('-DDBOA_TIMELINE')
 
 
 def _stale(target, deps):

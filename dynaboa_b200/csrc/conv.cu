@@ -10,8 +10,6 @@
 // whose partial tiles are summed in a fixed order through distributed shared memory (cluster_reduce_store).
 #include <cooperative_groups.h>
 
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "kernels.h"
 
@@ -409,11 +407,9 @@ int conv_dgrad(const float* dy, const float* w, float* dx, const ConvDims& d, in
 }
 
 int conv_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, float* ws, size_t ws_floats, cudaStream_t st) {
-    static const bool use_stem = [] { const char* e = getenv("DBOA_STEM_WGRAD"); return !(e && e[0] == '0'); }();      // 0: generic kernel (A/B)
-    if (use_stem) {                                     // the stem has its own kernel (last on the critical path of every backward)
-        const int s = stem_wgrad(dy, x, dw, d, ws, ws_floats, st);
-        if (s != DBOA_ERR_UNSUPPORTED) return s;
-    }
+    // the stem has its own kernel (last on the critical path of every backward); the generic kernel below takes every other shape
+    const int s = stem_wgrad(dy, x, dw, d, ws, ws_floats, st);
+    if (s != DBOA_ERR_UNSUPPORTED) return s;
     if (d.Cout % BM != 0 || d.groups < 1) return DBOA_ERR_SHAPE;
     const int Mpix = d.B * d.Ho * d.Wo, K = d.kh * d.kw * d.Cin;
     const int piters = ceil_div(Mpix, BK);

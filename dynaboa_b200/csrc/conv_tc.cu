@@ -30,7 +30,6 @@
 //              loads in flight, then added in the fixed order z = 0..nz-1).
 #include <cooperative_groups.h>
 #include <stdint.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -47,33 +46,9 @@ static int g_tc_mode = 3;
 bool conv_tc_enabled() { return g_tc_mode != 0; }
 bool conv_tc_bwd_enabled() { return g_tc_mode >= 2; }
 bool conv_tc_wgrad_enabled() { return g_tc_mode == 2; }
-void conv_tc_set_enabled(bool on) { g_tc_mode = on ? 2 : 0; }
 void conv_tc_set_mode(int mode) { g_tc_mode = mode; }
 
 namespace tc {
-
-// Diagnostic build (-DDBOA_TIMELINE, buffer set by dboa_debug_set_timeline): thread 0 of every CTA stamps %globaltimer at the phase
-// boundaries of the kernel into a device buffer [cta][16]; compiled out of the product library.
-#ifdef DBOA_TIMELINE
-__device__ unsigned long long* g_timeline = nullptr;
-#define DBOA_TL(i)                                                                                        \
-    do {                                                                                                  \
-        if (threadIdx.x == 0 && g_timeline != nullptr) {                                                  \
-            unsigned long long t_;                                                                        \
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_));                                        \
-            g_timeline[((size_t)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 16 + (i)] = t_; \
-        }                                                                                                 \
-    } while (0)
-// per-iteration cycle stamps of CTA (0,0,0), thread 0: slot 40000 + it * 8 + j
-#define DBOA_TLC(it, j)                                                                                   \
-    do {                                                                                                  \
-        if (threadIdx.x == 0 && g_timeline != nullptr && (blockIdx.x | blockIdx.y | blockIdx.z) == 0 && (it) < 12)   \
-            g_timeline[40000 + (it) * 8 + (j)] = (unsigned long long)clock64();                           \
-    } while (0)
-#else
-#define DBOA_TL(i)
-#define DBOA_TLC(it, j)
-#endif
 
 enum { FWD = 0, DGRAD = 1, WGRAD = 2 };
 constexpr int BM = 128, BN = 64, BK = 32, STAGES = 2;
@@ -190,7 +165,6 @@ __global__ void __launch_bounds__(NT, 1) conv_tf32x3_kernel(const float* __restr
     float2 (&s_gn)[2][256] = sm.gn;
     constexpr bool XFWD = XF >= 1 && XF <= 3, XDG = XF == XD, XOP = XFWD || XDG;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    DBOA_TL(0);
     const int Ktaps = d.kh * d.kw, Kfull = Ktaps * d.Cin;
     // Grouped call: blockIdx.x = group * gx + tile, and group grp reads / writes only its own samples and weights (no tile
     // straddles two groups, since the weight operand differs per group).  groups == 1: grp = 0, bx = blockIdx.x.
@@ -248,7 +222,6 @@ __global__ void __launch_bounds__(NT, 1) conv_tf32x3_kernel(const float* __restr
         if (fill_x && fill_y) *reinterpret_cast<float4*>(O + (size_t)(orow + dyr + dxr) * ldo + col) = z;
     };
 
-    DBOA_TL(1);
     const int wg = warp >> 2;                              // warpgroup: tile rows 64 wg .. 64 wg + 63
     float acc[32], blk[32];                                // running total (round-to-nearest adds), accumulator of one k-block
 #pragma unroll
@@ -468,10 +441,8 @@ __global__ void __launch_bounds__(NT, 1) conv_tf32x3_kernel(const float* __restr
             for (int f = 0; f < STAGES; ++f)
                 if (f < nkb) fetch_b(rb[f]);
         }
-        DBOA_TL(2);
         pdl_wait();
         pdl_trigger();
-        DBOA_TL(3);
         if (XOP) {
             // per (sample, group) tables of the transform, from the producers' fixed-point sums
             const double n = (double)d.Ho * d.Wo * Cop / 4;        // XFWD: elements of one group of the operand (its producer's output)
@@ -506,13 +477,9 @@ __global__ void __launch_bounds__(NT, 1) conv_tf32x3_kernel(const float* __restr
                 const int it = it0 + f;
                 if (it < nkb) {
                     const int s = f;                                                              // stage == register set
-                    DBOA_TLC(it, 0);
                     stash(s, ra[f], rb[f], rx[f], roff[f], rch[f]);
-                    DBOA_TLC(it, 2);
                     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> async-proxy (wgmma) reads
                     __syncthreads();
-                    DBOA_TLC(it, 3);
-                    if (it == 0) DBOA_TL(4);
                     const uint64_t dah = make_desc(smem_u32(sm.a_hi[s])) + a_step, dal = make_desc(smem_u32(sm.a_lo[s])) + a_step;
                     const uint64_t dbh = make_desc(smem_u32(sm.b_hi[s])), dbl = make_desc(smem_u32(sm.b_lo[s]));
                     constexpr uint64_t KSTEP = (2 * CORE_BYTES) >> 4;      // 8 tf32 = two 16-byte chunks along K, in descriptor units
@@ -533,14 +500,11 @@ __global__ void __launch_bounds__(NT, 1) conv_tf32x3_kernel(const float* __restr
                     fence_operand(blk);
 #pragma unroll
                     for (int q = 0; q < 32; ++q) acc[q] += blk[q];
-                    DBOA_TLC(it, 4);
                 }
             }
         }
     }
-    DBOA_TL(5);
     __syncthreads();                                       // every MMA of this CTA has completed: the A tiles are free
-    DBOA_TL(6);
 
     // ---- epilogue: accumulator fragments -> shared memory (row-major tile) -> row-contiguous global stores
     const int nz = gridDim.z;
@@ -553,7 +517,6 @@ __global__ void __launch_bounds__(NT, 1) conv_tf32x3_kernel(const float* __restr
             *reinterpret_cast<float2*>(red + r * RED_LD + c) = make_float2(acc[i], acc[i + 1]);
         }
     }
-    DBOA_TL(7);
     // Fused epilogues.  A thread's columns are fixed (v & 15 does not change as v advances by NT) and its rows ascend, so the sums
     // are kept per thread and flushed as fixed-point atomics (exact integer addition: order independent) when the sample changes.
     constexpr bool FSTAT = XF >= 0 && XF <= 3;
@@ -626,7 +589,6 @@ __global__ void __launch_bounds__(NT, 1) conv_tf32x3_kernel(const float* __restr
     } else {
         cg::cluster_group cluster = cg::this_cluster();
         cluster.sync();
-        DBOA_TL(8);
         const int rank = (int)cluster.block_rank();
         const int rows_per = BM / nz;                                 // nz is a power of two <= 16
         for (int v = tid; v < rows_per * (BN / 4); v += NT) {
@@ -651,11 +613,9 @@ __global__ void __launch_bounds__(NT, 1) conv_tf32x3_kernel(const float* __restr
             }
             *dst = post(orow, n0 + c4, sacc);
         }
-        DBOA_TL(9);
         cluster.sync();                                               // peers may still be reading this CTA's tile
     }
     if (FSTAT || prep) flush_all();
-    DBOA_TL(10);
 }
 
 template <int MODE, int XF = -1>
@@ -672,7 +632,7 @@ static int launch(const float* p, const float* q, float* o, const ConvDims& d, i
     const int tiles = mtiles * (cols / BN);
     // K-slices per tile (cluster size): a power of two <= 8 (the portable cluster size) that keeps the grid within about one wave; a split must
     // leave at least `min_kb` k-blocks per CTA, since the cluster barrier and DSMEM reduction of a split tile cost several k-blocks.
-    static const int min_kb = [] { const char* e = getenv("DBOA_TC_MINKB"); int v = e ? atoi(e) : 2; return v < 1 ? 1 : v; }();
+    constexpr int min_kb = 2;
     int ns = 1;
     const int slots = num_sms();                          // one resident CTA per SM (~150-215 registers x 256 threads)
     while (ns < 8 && tiles * ns * 2 <= slots + tiles && nkb / (ns * 2) >= min_kb) ns *= 2;
@@ -689,12 +649,6 @@ static bool shape_ok(const ConvDims& d) {
 }
 
 }  // namespace tc
-
-#ifdef DBOA_TIMELINE
-extern "C" int dboa_debug_set_timeline(unsigned long long* buf) {
-    return cudaMemcpyToSymbol(tc::g_timeline, &buf, sizeof(buf)) == cudaSuccess ? 0 : -3;
-}
-#endif
 
 int conv_tc_fwd(const float* x, const float* w, float* y, const ConvDims& d, cudaStream_t st, bool pdl) {
     if (g_tc_mode == 0 || !tc::shape_ok(d)) return DBOA_ERR_UNSUPPORTED;

@@ -12,7 +12,7 @@
 namespace dboa {
 
 // tmp[yc][xo][c] = sum_j wx[xo][j] * crop(yc, sx[xo] + j, c);  crop(y, x) = img(ul_y + y, ul_x + x) or 0 outside the frame.
-// Element i = yc * res + xo of one frame: the body of crop_resize_rows_kernel and of the grouped rows pass.
+// Element i = yc * res + xo of one frame.
 template <typename T>
 __device__ __forceinline__ void crop_rows_elem(const T* __restrict__ img, int H, int W, int ul_x, int ul_y, const float* __restrict__ wx,
                                                const int* __restrict__ sx, int Tx, int res, int i, float* __restrict__ tmp) {
@@ -32,14 +32,6 @@ __device__ __forceinline__ void crop_rows_elem(const T* __restrict__ img, int H,
     }
     float* o = tmp + (size_t)i * 3;
     o[0] = a0; o[1] = a1; o[2] = a2;
-}
-template <typename T>
-__global__ void __launch_bounds__(256) crop_resize_rows_kernel(const T* __restrict__ img, int H, int W, int ul_x, int ul_y, int Hc,
-                                                               const float* __restrict__ wx, const int* __restrict__ sx, int Tx, int res,
-                                                               float* __restrict__ tmp) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;            // over Hc * res
-    if (i >= Hc * res) return;
-    crop_rows_elem(img, H, W, ul_x, ul_y, wx, sx, Tx, res, i, tmp);
 }
 // out[c][yo][xo] = ((sum_i wy[yo][i] * tmp[sy[yo] + i][xo][c]) / 255 - mean[c]) / std[c];  element i = yo * res + xo of one frame
 __device__ __forceinline__ void crop_cols_elem(const float* __restrict__ tmp, int Hc, const float* __restrict__ wy, const int* __restrict__ sy,
@@ -62,28 +54,6 @@ __device__ __forceinline__ void crop_cols_elem(const float* __restrict__ tmp, in
     out[plane + i] = __fdiv_rn(__fsub_rn(__fdiv_rn(a1, 255.0f), m1), s1);
     out[2 * plane + i] = __fdiv_rn(__fsub_rn(__fdiv_rn(a2, 255.0f), m2), s2);
 }
-__global__ void __launch_bounds__(256) crop_resize_cols_kernel(const float* __restrict__ tmp, int Hc, const float* __restrict__ wy,
-                                                               const int* __restrict__ sy, int Ty, int res, float m0, float m1, float m2,
-                                                               float s0, float s1, float s2, float* __restrict__ out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;            // over res * res
-    if (i >= res * res) return;
-    crop_cols_elem(tmp, Hc, wy, sy, Ty, res, m0, m1, m2, s0, s1, s2, i, out);
-}
-
-int crop_resize_normalize(const void* img, int is_u8, int H, int W, int ul_x, int ul_y, int Hc, const float* wx, const int* sx, int Tx,
-                          const float* wy, const int* sy, int Ty, int res, const float mean[3], const float stdv[3], float* tmp, float* out,
-                          cudaStream_t st) {
-    if (H < 1 || W < 1 || Hc < 1 || Tx < 1 || Ty < 1 || res < 1) return DBOA_ERR_SHAPE;
-    const int n1 = Hc * res;
-    if (is_u8)
-        crop_resize_rows_kernel<unsigned char><<<ceil_div(n1, 256), 256, 0, st>>>(static_cast<const unsigned char*>(img), H, W, ul_x, ul_y, Hc, wx, sx, Tx, res, tmp);
-    else
-        crop_resize_rows_kernel<float><<<ceil_div(n1, 256), 256, 0, st>>>(static_cast<const float*>(img), H, W, ul_x, ul_y, Hc, wx, sx, Tx, res, tmp);
-    DBOA_TRY(check_launch());
-    crop_resize_cols_kernel<<<ceil_div(res * res, 256), 256, 0, st>>>(tmp, Hc, wy, sy, Ty, res, mean[0], mean[1], mean[2], stdv[0], stdv[1], stdv[2], out);
-    return check_launch();
-}
-
 // utils/dataprocess.py:39-46 applied to kp + 1 (pw3d.py:155): p = t . (x, y, 1) in double, truncation toward zero, + 1, then
 // 2 p / res - 1 (double) -> float; the confidence column is copied.  One keypoint: the body of keypoint_transform_kernel and of
 // the grouped call.
@@ -110,7 +80,7 @@ int keypoint_transform(const float* kp, int n, double t00, double t02, double t1
 // ---- grouped input side: the frames of several streams in one launch per pass.  The descriptors of the active videos travel
 // compacted in the kernel parameter (__grid_constant__: read in place from parameter space, no host-to-device copy); entry k
 // describes video video[k].  Per element the arithmetic is crop_rows_elem / crop_cols_elem / keypoint_elem, so each active
-// row is bit-identical to the one-frame call.
+// row is bit-identical to the one-frame call (for the crop, this call with a single entry).
 struct CropGroups {
     dboa_crop_desc f[64];
     long long tmp_off[64];        // float offset of entry k's rows in tmp
@@ -120,7 +90,7 @@ struct CropGroups {
     float mean[3], stdv[3];
 };
 
-// one row of blocks per entry, back to back: entry k's blocks see exactly the indices of crop_resize_rows_kernel's grid
+// one row of blocks per entry, back to back: entry k's blocks see exactly the indices of a grid of its own
 __global__ void __launch_bounds__(256) crop_groups_rows_kernel(const __grid_constant__ CropGroups a, float* __restrict__ tmp) {
     int lo = 0, hi = a.n - 1;                                         // last entry whose first block is <= blockIdx.x
     while (lo < hi) {
@@ -177,6 +147,17 @@ int crop_resize_normalize_groups(const dboa_crop_desc* frames, int groups, unsig
     DBOA_TRY(check_launch());
     crop_groups_cols_kernel<<<dim3(ceil_div((long long)res * res, 256), a.n), 256, 0, st>>>(a, tmp, out);
     return check_launch();
+}
+
+// one frame: the grouped call with a single descriptor
+int crop_resize_normalize(const void* img, int is_u8, int H, int W, int ul_x, int ul_y, int Hc, const float* wx, const int* sx, int Tx,
+                          const float* wy, const int* sy, int Ty, int res, const float mean[3], const float stdv[3], float* tmp, float* out,
+                          cudaStream_t st) {
+    if (H < 1 || W < 1 || Hc < 1 || Tx < 1 || Ty < 1 || res < 1) return DBOA_ERR_SHAPE;
+    dboa_crop_desc d;
+    d.img = img; d.wx = wx; d.sx = sx; d.wy = wy; d.sy = sy;
+    d.is_u8 = is_u8; d.H = H; d.W = W; d.ul_x = ul_x; d.ul_y = ul_y; d.Hc = Hc; d.Tx = Tx; d.Ty = Ty;
+    return crop_resize_normalize_groups(&d, 1, 1ULL, res, mean, stdv, tmp, (long long)Hc * res * 3, out, st);
 }
 
 struct KeypointGroups {

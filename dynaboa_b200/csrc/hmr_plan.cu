@@ -262,10 +262,7 @@ long long hmr_bucket_offset(int k) {        // first float of bucket k's span; b
     return 0;
 }
 // DBOA_ASYNC_WGRAD=0 in the environment keeps everything on the caller's stream (A/B measurements, debugging)
-static bool g_async_enabled = [] { const char* e = getenv("DBOA_ASYNC_WGRAD"); return !(e && e[0] == '0'); }();
-void hmr_set_async_wgrad(bool on) { g_async_enabled = on; }
-// DBOA_WGRAD_STREAMS=1|2: how many side streams the weight gradients alternate over
-static const int g_wgrad_streams = [] { const char* e = getenv("DBOA_WGRAD_STREAMS"); return (e && e[0] == '1') ? 1 : BwdAsync::NSIDE; }();
+static const bool g_async_enabled = [] { const char* e = getenv("DBOA_ASYNC_WGRAD"); return !(e && e[0] == '0'); }();
 
 static ConvDims dims_of(const ConvLayer& c, int B, int groups = 1, unsigned long long active = ~0ULL);
 
@@ -643,7 +640,7 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
     auto wgrad = [&](const ConvLayer& c, int k, const float* xin_) {
         if (!async) return conv_backward_weight(c, B, groups, active, tmp[k], xin_, G + c.w_off, sc.ws, st);
         cudaStream_t ss = A.side[A.next_side];
-        A.next_side = (A.next_side + 1) % g_wgrad_streams;
+        A.next_side = (A.next_side + 1) % BwdAsync::NSIDE;
         cudaEventRecord(A.ev_ready[A.ring], st);
         cudaStreamWaitEvent(ss, A.ev_ready[A.ring], 0);
         A.ring = (A.ring + 1) & 7;

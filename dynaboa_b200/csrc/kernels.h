@@ -33,7 +33,6 @@ bool conv_tc_bwd_enabled();
 bool conv_tc_wgrad_enabled();
 int conv1x1_tc_fwd(const float* x, const float* w, float* y, int M, int Cin, int Cout, cudaStream_t st, bool pdl = true);
 bool conv_tc_enabled();
-void conv_tc_set_enabled(bool on);
 void conv_tc_set_mode(int mode);                      // 0 off, 1 forward, 2 forward + dgrad + wgrad, 3 forward + dgrad
 
 int conv_wgrad_tc(const float* dy, const float* x, float* dw, const ConvDims& d, cudaStream_t st);   // any mode; dw +=

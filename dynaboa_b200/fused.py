@@ -19,7 +19,6 @@ call) and callbacks for what stays with the adaptor.  A set of videos is an int 
 """
 import collections
 import ctypes as C
-import os
 
 import torch
 
@@ -28,7 +27,6 @@ from ._lib import ptr, stream
 
 
 _SIDE = {}
-_TEACHER_OVERLAP = os.environ.get('DBOA_TEACHER_STREAM', '1') != '0'     # 0: teacher forward on the caller's stream
 
 # retrieval's exemplars: cluster centres (K, 2048), each cluster's exemplars, their tensors by name, (K,) distance scratch
 Bank = collections.namedtuple('Bank', 'centers index exemplars dists')
@@ -103,11 +101,6 @@ def _mark(s, name):
         s.phase_events.append((name, ev))
 
 
-def _entry(mask, G):
-    """The ``active`` argument of a network pass over ``mask``: None (the ``_groups`` entry point) for every video."""
-    return None if mask == (1 << G) - 1 else mask
-
-
 def runs(mask, G, key=lambda g: 0):
     """[a, b) ranges of consecutive videos whose bit is set in ``mask`` and that share ``key(g)``."""
     out = []
@@ -142,7 +135,7 @@ def _smpl_fwd(smpl, betas, rot):
 def forward_graph(s, arena, buffers, image, mask, masks=None):
     p = _Pred()
     p.image, p.B, p.masked, p.groups, p.active = image, image.shape[0], masks is not None, s.G, mask
-    p.rot, p.shape, p.cam, _, p.tape = hmr_mod.raw_forward(arena, buffers, image, masks, groups=s.G, active=_entry(mask, s.G))
+    p.rot, p.shape, p.cam, _, p.tape = hmr_mod.raw_forward(arena, buffers, image, masks, groups=s.G, active=mask)
     p.verts, p.joints, p.smpl_tape = _smpl_fwd(s.smpl_neutral, p.shape, p.rot)
     p.p2d = torch.empty(p.B, 49, 2, dtype=torch.float32, device=image.device)
     _lib.call('dboa_project_fwd', ptr(p.cam), ptr(p.joints), ptr(p.p2d), p.B, 49, stream())
@@ -201,7 +194,7 @@ def backward_graph(s, arena, p, dp2d, dj3d, dR, dbeta, grad_arena, sync=None):
               ptr(dbeta), 1, stream())
     if sync is not None:
         sync.arm()
-    hmr_mod.raw_backward(arena, p.tape, B, p.masked, dR, dbeta, dcam, grad_arena, groups=p.groups, active=_entry(p.active, p.groups))
+    hmr_mod.raw_backward(arena, p.tape, B, p.masked, dR, dbeta, dcam, grad_arena, groups=p.groups, active=p.active)
     if sync is not None:
         sync.after_backward(grad_arena)
 
@@ -244,7 +237,7 @@ def level_backward(s, out, arena, image, kp, lower, grad_arena, mask, live, main
     # of small, latency-bound kernels overlap on the GPU (each one alone leaves most SMs idle at batch 1)
     tpred, side = None, None
     if use_temporal and o.use_meanteacher:
-        if _TEACHER_OVERLAP and G == 1:
+        if G == 1:
             side = _side_stream(image.device)
             side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):                           # None: the caller's stream
@@ -299,10 +292,7 @@ def level_backward(s, out, arena, image, kp, lower, grad_arena, mask, live, main
         kf, kn = s.kp_range
         margs = (ptr(main.p2d), ptr(p_hist), ptr(kp), ptr(hist_kp.contiguous()), float(o.motionloss_weight), ptr(mterm), ptr(dp2d), ptr(dph),
                  nb, 1, kf, kn, G)
-        if live == (1 << G) - 1:
-            _lib.call('dboa_loss_motion_groups', *margs, stream())
-        else:
-            _lib.call('dboa_loss_motion_active', *margs, live, stream())
+        _lib.call('dboa_loss_motion_active', *margs, live, stream())
         if not batched:
             backward_graph(s, arena, hist, dph, torch.zeros_like(hist.joints), torch.zeros_like(hist.rot), torch.zeros_like(hist.shape),
                            grad_arena)

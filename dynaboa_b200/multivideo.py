@@ -1,5 +1,5 @@
 """Several independent videos adapted in lockstep on one GPU: ``fused.fused_adapt`` over (G, P) stacks of weight arenas, with
-every network forward and backward one grouped call (``dboa_hmr_forward_groups`` / ``dboa_hmr_backward_groups``).  This module
+every network forward and backward one grouped call (``dboa_hmr_forward_active`` / ``dboa_hmr_backward_active``).  This module
 holds the per-video state, hands the step a ``fused.Step`` over it and files the records the step returns per slot.
 
 Each video keeps the reference's semantics: its own theta, Adam moments and step count, teacher, fast weights, gradient,
@@ -18,7 +18,7 @@ import torch
 
 from . import _lib, hmr as hmr_mod
 from ._lib import ptr, stream
-from .fused import Step, _entry, fused_adapt, pick, runs
+from .fused import Step, fused_adapt, pick, runs
 
 EVAL_MODES = ('none', 'final', 'all')
 GT_KEYS = ('pose', 'betas', 'gender')
@@ -294,7 +294,7 @@ class MultiVideoAdaptor:
         """One evaluation of ``arena`` (theta, or the fast weights of inner step ``inner``) for the slots in ``on``: a grouped
         forward, SMPL decode and ``dboa_eval_metrics_active`` (ground truth from the frame's first), kept on the device."""
         with torch.no_grad():
-            rot, shape, _, _, _ = hmr_mod.raw_forward(arena, self.buffers, batch['image'], groups=self.G, active=_entry(on, self.G))
+            rot, shape, _, _, _ = hmr_mod.raw_forward(arena, self.buffers, batch['image'], groups=self.G, active=on)
             pred = self.base.decode_smpl_params(rot, shape)['vts']
             if self._gt is None:                             # as Adaptor.inference, for every staged row
                 self._gt = self.base._gt_meshes(batch)

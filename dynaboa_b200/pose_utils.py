@@ -1,6 +1,6 @@
 """Evaluation metrics used by the driver (reference utils/pose_utils.py:9-64): Procrustes-aligned
 error.  Host-side numpy, as in the reference: PA-MPJPE is the parity metric, not a kernel target
-(SURVEY.md §2).  The driver itself evaluates on the device (`Adaptor.eval_metrics` -> `dboa_eval_metrics`, SURVEY §8f N1);
+(SURVEY.md §2).  The driver itself evaluates on the device (`Adaptor.eval_metrics` -> `dboa_eval_metrics_active`, SURVEY §8f N1);
 these numpy functions remain for API compatibility (`utils.pose_utils` of the drop-in tree)."""
 import numpy as np
 
