@@ -15,7 +15,10 @@ from its own values and is the network of ``hmr_ref`` (tests/test_hmr_frozen.py 
 
 The pattern is a dict: ``'relu'`` maps the name of each convolution that feeds a ReLU (``conv1``, ``layer1.0.conv1``, ...,
 ``layerL.B.conv3``; the shortcut joins conv3's ReLU) to an NCHW 0/1 mask, ``'pool'`` is the (B,64,56,56) integer window
-position of the max-pool, and ``'drop'`` is None or the (3,2,B,1024) scaled keep-masks.
+position of the max-pool, and ``'drop'`` is None or the (3,2,B,1024) scaled keep-masks.  An optional ``'pose6d'`` (B,144)
+(the GPU's final 6D pose) is the point at which the smooth 6D -> rotation map and its derivative are evaluated: its
+Gram-Schmidt derivative grows as the square of 1 / sin(a1, a2), so an fp32 forward's rounding of the 6D pose, small in
+itself, would otherwise move the derivative further than the backward's own rounding.
 
 With ``need_feature`` the forward also returns the 15 feature tensors of ``hmr_ref.forward(need_feature=True)``, in the order of
 ``dboa_hmr_feature_info``: the stem convolution's output, the outputs of layer1..4, the pooled 2048-vector and the nine rows of
@@ -89,6 +92,9 @@ def forward(x, p, pattern=None, drop=None, need_feature=False):
     masks = None if drop is None else [(drop[i, 0].to(xf), drop[i, 1].to(xf)) for i in range(3)]
     pose, shape, cam, hfeats = hmr_ref.regressor(xf, p, p['init_pose'].expand(B, -1), p['init_shape'].expand(B, -1),
                                                  p['init_cam'].expand(B, -1), 3, masks)
+    own6d = pattern.get('pose6d')
+    if own6d is not None:                          # the 6D -> rotation map taken at the given point, its derivative included
+        pose = own6d.to(pose) + (pose - pose.detach())
     rotmat = geometry_ref.rot6d_to_rotmat(pose).view(B, 24, 3, 3)
     if need_feature:
         return rotmat, shape, cam, pattern, feats + hfeats

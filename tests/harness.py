@@ -5,10 +5,11 @@ and no test module imports another.
 - The device-free ABI tests: ``built_lib``, the stand-in pointer ``FAKE``, the ``ERR_*`` codes, ``cpu_options`` and ``idle_pool``.
 - The per-video pool runs: ``video_masks`` / ``video_seed`` and the golden-aware ``masks_for`` / ``seed_for``, ``PoolRun`` (a
   MultiVideoAdaptor whose slots carry videos) and ``SingleRun`` (the same video through the single-video ``Adaptor.adapt``).
-- The grouped HMR plan tests: the ``model`` fixture body, ``stacked``, ``inputs``, the fp64 bounds of the layer tests and
-  ``tape_pattern``, the kink pattern of a GPU forward for oracle/hmr_frozen.py.
-- The exact references of the step's sweeps (``f32``, ``sgd_ref``, ``ema_ref``, ``adam_ref``) and the pose prior's near-tie rule
-  ``selected``.
+- The grouped HMR plan tests: the ``model`` fixture body, ``stacked``, ``inputs``, the fp64 bounds of the layer tests, the
+  fp64 GroupNorm ``gn_stats`` / ``gn_apply`` and ``tape_pattern``, the kink pattern of a GPU forward for oracle/hmr_frozen.py.
+- The grouped input side: the mixed frames and boxes of ``scene``, their ``crop_kind`` and the fp64 ``crop_oracle``.
+- The exact references of the step's sweeps (``f32``, ``sgd_ref``, ``ema_ref``, ``adam_ref``), the fp64 bounds of the cosine
+  feature test and the pose prior's near-tie rule ``selected``.
 - Rendering: the analytic scene helpers, ``sphere``, ``posed_smpl_mesh``, ``check_against_oracle``, and the synthetic Internet
   video of the unchanged-driver tests."""
 import ast
@@ -279,6 +280,18 @@ def rel(a, ref, scale=None):
     return float((a.double() - ref).abs().max() / s.clamp_min(1e-30))
 
 
+def gn_stats(y):
+    """fp64 GroupNorm (4 groups) statistics (mean, rstd) of an NCHW tensor, per sample and group."""
+    v = y.reshape(y.shape[0], 4, -1)
+    return v.mean(-1), (v.var(-1, unbiased=False) + 1e-5).rsqrt()
+
+
+def gn_apply(y, mean, rstd, gamma, beta):
+    B, C = y.shape[:2]
+    v = ((y.reshape(B, 4, -1) - mean[..., None]) * rstd[..., None]).reshape(y.shape)
+    return v * gamma.double().view(1, C, 1, 1) + beta.double().view(1, C, 1, 1)
+
+
 def tape_pattern(tape, B, rows=slice(None), masks=None):
     """The kink pattern (oracle/hmr_frozen.py) of the samples ``rows`` of the GPU forward whose tape is ``tape`` (batch B):
     each ReLU's ``a > 0``, the max-pool's window positions and the dropout keep-masks ``masks`` (None: no dropout)."""
@@ -322,6 +335,13 @@ def adam_ref(p, g, m, v, t, lr, betas, eps, step, alpha=0.1, gscale=1.0):
     return p, m, v, (None if t is None else ema_ref(t, p, alpha))
 
 
+# The cosine feature test's sums against fp64 sums of the same fp32 inputs: |terms - fp64| <= TERMS_TOL * scale (sum |a_k b_k|,
+# |a|^2, |b|^2).  Worst measured on an H100 80GB HBM3 (700 W) over test_gpu_step_kernels.py: 1.3e-7 (G = 8, b = 2).
+# |delta(1 - cos)| from the device sums: worst measured 1.4e-7 (G = 8, b = 1); the fp32 cosine the loop tests adds up to 3e-8.
+TERMS_TOL = 1e-6
+COS_TOL = 1e-6
+
+
 def selected(ll, prior_b):
     """The component each body's GPU prior value belongs to: the fp64 component value closest to it."""
     return (ll.detach() - prior_b.double().cpu()[:, None]).abs().argmin(1)
@@ -332,6 +352,59 @@ COLOR = (205 / 255, 129 / 255, 98 / 255)
 CAM = np.array([1.0, 1.0, 0.0, 0.0])
 # frame sizes (H, W) the grouped input side and the grouped overlay cycle through
 SIZES = [(240, 320), (1080, 1920), (720, 1280), (480, 640), (300, 400), (1080, 1920), (256, 256), (600, 800)]
+
+
+def scene(G, seed):
+    """G frames (sizes of SIZES, uint8 and float32 mixed) with boxes inside, partly outside and wholly outside the frame, and
+    scales that up-scale (box smaller than 224) and down-scale."""
+    rng = np.random.default_rng(seed)
+    frames, centers, scales = [], [], []
+    for g in range(G):
+        H, W = SIZES[(g + seed) % len(SIZES)]
+        img = rng.integers(0, 256, size=(H, W, 3), dtype=np.uint8)
+        t = torch.from_numpy(img).cuda()
+        frames.append(t if g % 2 == 0 else t.float())
+        kind = (g + seed) % 4
+        if kind == 0:
+            c, s = [W / 2 + rng.uniform(-20, 20), H / 2 + rng.uniform(-20, 20)], min(H, W) / 200 * rng.uniform(0.3, 0.9)
+        elif kind == 1:
+            c, s = [rng.uniform(0, 0.1) * W, rng.uniform(0.9, 1.0) * H], min(H, W) / 200 * 0.8
+        elif kind == 2:
+            c, s = [W + 300.0, -250.0], 1.2                                  # wholly outside: zeros
+        else:
+            c, s = [rng.uniform(0.3, 0.7) * W, rng.uniform(0.3, 0.7) * H], 0.5  # 100-pixel box: up-scales
+        centers.append(c)
+        scales.append(s)
+    return frames, centers, scales
+
+
+# |GPU crop - oracle| of a 1080p uint8 frame (test_dataprocess.py), the bound of every scene() frame
+CROP_TOL = 3e-5
+
+
+def crop_kind(frame, center, scale):
+    """How the box of ``center`` / ``scale`` meets the (H, W, 3) frame: 'outside' (no pixel of the frame), 'partial' or
+    'inside', and whether the crop is resized 'up' (smaller than 224 pixels) or 'down'."""
+    from dynaboa_b200 import dataprocess as D
+    H, W = frame.shape[:2]
+    ul_x, ul_y, Wc, Hc = D._box(center, scale, (224, 224))
+    if ul_x >= W or ul_y >= H or ul_x + Wc <= 0 or ul_y + Hc <= 0:
+        where = 'outside'
+    else:
+        where = 'inside' if ul_x >= 0 and ul_y >= 0 and ul_x + Wc <= W and ul_y + Hc <= H else 'partial'
+    return where, 'up' if Hc < 224 else ('down' if Hc > 224 else 'same')
+
+
+def crop_oracle(frame, center, scale):
+    """oracle/dataprocess_ref.py's normalised (3, 224, 224) crop of a device frame, in fp64 from its float32 values.  A box
+    that misses the frame crops zeros; the reference's slicing cannot express an empty overlap, so that crop is the oracle's
+    crop of a zero frame of the same size through a box inside it."""
+    from oracle import dataprocess_ref as R
+    img = frame.float().cpu().numpy()
+    if crop_kind(frame, center, scale)[0] == 'outside':
+        H, W = img.shape[:2]
+        return R.rgb_processing(np.zeros_like(img), [W / 2, H / 2], scale)
+    return R.rgb_processing(img, center, scale)
 
 
 def px_verts(pts, W, H):

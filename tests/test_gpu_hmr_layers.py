@@ -19,7 +19,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from harness import FWD_TOL, GRAD_L2, GRAD_TOL, nchw, rel, structure, tape_pattern
+from harness import FWD_TOL, GRAD_L2, GRAD_TOL, gn_apply, gn_stats, nchw, rel, structure, tape_pattern
 
 pytestmark = pytest.mark.gpu
 
@@ -63,17 +63,6 @@ def run_forward(m, cfg):
     rot, shape, cam, _, _ = raw_forward(m.arena, m._buffers, x, masks, tape)
     torch.cuda.synchronize()
     return x, masks, tape, (rot, shape, cam)
-
-
-def gn_stats(y):
-    v = y.reshape(y.shape[0], 4, -1)
-    return v.mean(-1), (v.var(-1, unbiased=False) + 1e-5).rsqrt()
-
-
-def gn_apply(y, mean, rstd, gamma, beta):
-    B, C = y.shape[:2]
-    v = ((y.reshape(B, 4, -1) - mean[..., None]) * rstd[..., None]).reshape(y.shape)
-    return v * gamma.double().view(1, C, 1, 1) + beta.double().view(1, C, 1, 1)
 
 
 @pytest.mark.parametrize('cfg', CONFIGS, ids=IDS)

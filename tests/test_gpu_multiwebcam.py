@@ -1,8 +1,9 @@
 """Webcam pool (MultiWebcamAdaptor) and its grouped input side on the GPU.
 
-- dboa_crop_resize_normalize_groups / dboa_keypoint_transform_groups: every active row bit-identical to the one-frame calls,
-  for frames of different sizes and dtypes, boxes partly and wholly outside the frame, up- and down-scaling crops; idle frames
-  (NaN-filled) not read and idle rows (a sentinel) not written; the dataprocess golden through the new entry.
+- dboa_crop_resize_normalize_groups: every frame against the fp64 oracle (oracle/dataprocess_ref.py), and every active frame of
+  a masked call bit-identical to the full call; dboa_keypoint_transform_groups: every active row bit-identical to the one-stream
+  transform.  Frames of different sizes and dtypes, boxes partly and wholly outside the frame, up- and down-scaling crops; idle
+  frames (NaN-filled) not read and idle rows (a sentinel) not written; the dataprocess golden through the new entry.
 - One stream is WebcamAdaptor, bit for bit, at adapt_webcam.npz's options.
 - G = 4 at the golden's options: stream 0 against the golden, streams 1..3 against their own WebcamAdaptor runs; the motion term
   goes live from frame `interval` on.
@@ -12,7 +13,7 @@ import pytest
 import torch
 
 from conftest import rel_err
-from harness import SIZES, bits, cam_options, state, webcam_pool
+from harness import CROP_TOL, bits, cam_options, crop_kind, crop_oracle, scene, state, webcam_pool
 
 pytestmark = pytest.mark.gpu
 SENTINEL = 0x7fc0dead                  # a NaN payload no kernel writes
@@ -21,42 +22,19 @@ SENTINEL = 0x7fc0dead                  # a NaN payload no kernel writes
 # ------------------------------------------------------------------ grouped input side
 
 
-def scene(G, seed):
-    """G frames (sizes of SIZES, uint8 and float32 mixed) with boxes inside, partly outside and wholly outside the frame, and
-    scales that up-scale (box smaller than 224) and down-scale."""
-    rng = np.random.default_rng(seed)
-    frames, centers, scales = [], [], []
-    for g in range(G):
-        H, W = SIZES[(g + seed) % len(SIZES)]
-        img = rng.integers(0, 256, size=(H, W, 3), dtype=np.uint8)
-        t = torch.from_numpy(img).cuda()
-        frames.append(t if g % 2 == 0 else t.float())
-        kind = (g + seed) % 4
-        if kind == 0:
-            c, s = [W / 2 + rng.uniform(-20, 20), H / 2 + rng.uniform(-20, 20)], min(H, W) / 200 * rng.uniform(0.3, 0.9)
-        elif kind == 1:
-            c, s = [rng.uniform(0, 0.1) * W, rng.uniform(0.9, 1.0) * H], min(H, W) / 200 * 0.8
-        elif kind == 2:
-            c, s = [W + 300.0, -250.0], 1.2                                  # wholly outside: zeros
-        else:
-            c, s = [rng.uniform(0.3, 0.7) * W, rng.uniform(0.3, 0.7) * H], 0.5  # 100-pixel box: up-scales
-        centers.append(c)
-        scales.append(s)
-    return frames, centers, scales
-
-
 @pytest.mark.parametrize('G', [1, 2, 4, 8])
 def test_grouped_crop_is_the_one_frame_crop(G):
+    """Every frame of the grouped call against the fp64 oracle; the frames of a masked call bit-identical to the full call's."""
     from dynaboa_b200 import dataprocess as D
     frames, centers, scales = scene(G, G)
-    ref = [D.crop(f, c, s) for f, c, s in zip(frames, centers, scales)]
     Ts = {D._tables(D._box(c, s, (224, 224))[3], 224, frames[0].device)[1].shape[1] for c, s in zip(centers, scales)}
     if G >= 4:
         assert len(Ts) > 1                                                   # the Ty of the videos differ
-    out = torch.full((G, 3, 224, 224), float('nan'), device='cuda')
-    D.crop_groups(frames, centers, scales, out)
+    ref = D.crop_groups(frames, centers, scales, torch.full((G, 3, 224, 224), float('nan'), device='cuda'))
+    out = ref.cpu().numpy()
     for g in range(G):
-        assert torch.equal(bits(out[g]), bits(ref[g])), g
+        err = np.abs(out[g] - crop_oracle(frames[g], centers[g], scales[g])).max()
+        assert err < CROP_TOL, (g, crop_kind(frames[g], centers[g], scales[g]), err)
     masks = [1] if G == 1 else [1 << (G - 1), ((1 << G) - 1) & ~0b10]        # one active; all but one
     for active in masks:
         idle = [g for g in range(G) if not (active >> g) & 1]

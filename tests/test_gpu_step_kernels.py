@@ -21,7 +21,7 @@ import numpy as np
 import pytest
 import torch
 
-from harness import adam_ref, ema_ref, f32, sgd_ref
+from harness import COS_TOL, TERMS_TOL, adam_ref, ema_ref, f32, sgd_ref
 
 GUARD = 64
 SENTINEL = {torch.float32: -1.2345678e33, torch.float64: -1.25e300, torch.int32: 0x5A5A5A5A}
@@ -369,14 +369,8 @@ def feature_pairs(lengths, G, seed):
     return A, B
 
 
-# fp64 sums of the same fp32 inputs: |terms - fp64| <= TERMS_TOL * scale (sum |a_k b_k|, |a|^2, |b|^2).  Worst measured
-# on an H100 80GB HBM3 (700 W) over this file: 1.3e-7 (G = 8, b = 2).  |delta(1 - cos)| from the device sums: worst
-# measured 1.4e-7 (G = 8, b = 1); the fp32 cosine the loop tests adds up to 3e-8.  dboa_cosine_terms equals the grouped
+# TERMS_TOL, COS_TOL (harness.py): the bounds against fp64 sums of the same fp32 inputs.  dboa_cosine_terms equals the grouped
 # call at G = 1 bit for bit.
-TERMS_TOL = 1e-6
-COS_TOL = 1e-6
-
-
 def check_cosine_case(L, A, B, G, active, record):
     st, terms, part = cosine_terms(L, A, B, G, active)
     assert st == OK and terms.intact() and part.intact()
