@@ -51,6 +51,27 @@ def test_world_size_2_gloo():
     assert shards == [(0, 6), (6, 11)]                      # contiguous, covering, first ranks take the remainder
 
 
+def test_gradient_buckets_partition_the_arena_into_whole_layers():
+    """The three spans ``BucketedGradSync`` all-reduces partition [0, arena_floats) and each holds whole parameters of the layers
+    whose gradients the backward has finished when it records that bucket's event: layer4 and the head (bucket 0), layer3
+    (bucket 1), then the stem, layer1 and layer2 (bucket 2)."""
+    from harness import built_lib
+    from dynaboa_b200.hmr import ArenaLayout
+    lib = built_lib()
+    lay = ArenaLayout()
+    bounds = [(lib.dboa_hmr_bucket_offset(k), lib.dboa_hmr_bucket_offset(k - 1)) for k in range(3)]
+    assert bounds[0][1] == lay.floats and bounds[2][0] == 0
+    assert all(lo < hi for lo, hi in bounds) and bounds[0][0] == bounds[1][1] and bounds[1][0] == bounds[2][1]
+    first = dict(zip(lay.names, lay.offsets))
+    assert bounds[0][0] == first['layer4.0.conv1.weight'] and bounds[1][0] == first['layer3.0.conv1.weight']
+    owner = lambda name: 0 if name.split('.')[0] in ('layer4', 'fc1', 'fc2', 'decpose', 'decshape', 'deccam') else (
+        1 if name.startswith('layer3.') else 2)
+    for name, off, shape, stride in zip(lay.names, lay.offsets, lay.shapes, lay.strides):
+        end = off + 1 + sum((s - 1) * st for s, st in zip(shape, stride))
+        lo, hi = bounds[owner(name)]
+        assert lo <= off and end <= hi, (name, off, end, owner(name), bounds)
+
+
 def test_shard_range_partitions():
     from dynaboa_b200.dist import shard_range
     for n in (0, 1, 7, 8, 64):
