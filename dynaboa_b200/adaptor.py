@@ -10,6 +10,7 @@ Two entry points per frame:
   arena, Adam and the teacher EMA fused in one sweep, no host syncs except the ``dynamic_boa`` decision
   (see fused.py).  This is what ``bench.py`` times.
 """
+import itertools
 import os
 import os.path as osp
 import random
@@ -17,7 +18,7 @@ import random
 import numpy as np
 import torch
 
-from . import _lib, constants, hmr as hmr_mod
+from . import _lib, constants, hmr as hmr_mod, layout, state
 from .base_adaptor import BaseAdaptor
 from .fused import Frame, Step, _ArenaModel, fused_adapt
 
@@ -83,6 +84,9 @@ class Adaptor(BaseAdaptor):
     kp_range = (25, 24)          # joints of the 2D and motion terms (fused.Step)
     motion_lead = 0              # the motion term is live while global_step + motion_lead - interval > 0 (before save_hist)
     step_graph = True            # adapt may replay its steady-state frame as a CUDA graph (see _graph_key)
+    # the records a saved state carries (save_state)
+    RECORDS = ('feat_sims', 'optim_step_record', 'mpjpe_statistics', 'pampjpe_statistics', 'mpjpe_all_lower', 'pampjpe_all_lower',
+               'kp2dlosses_lower', 'kp2dlosses_upper', 'last_upper_loss', 'last_retrieval', 'optimized_step')
 
     def __init__(self, options):
         super().__init__(options)
@@ -102,10 +106,17 @@ class Adaptor(BaseAdaptor):
         self.history, self.kp2dlosses_lower, self.kp2dlosses_upper = {}, [], {}
 
     # ------------------------------------------------------------------ frame loop (reference :71-123)
-    def excute(self, max_frames=None, fused=False):
+    def excute(self, max_frames=None, fused=False, checkpoint=None, every=0):
+        """The frame loop.  ``checkpoint``: a video-state file (``save_state``); when it exists the run resumes from it, skipping
+        the frames it already adapted, and with ``every`` > 0 it is written after every ``every`` frames.  A resumed run
+        writes the same eight result files, byte for byte, as one that was never interrupted."""
         self.reset_records()
         mpjpe_all, pampjpe_all, pve_all = [], [], []
-        for step, batch in enumerate(self.dataloader):
+        start = 0
+        if checkpoint is not None and osp.exists(checkpoint):
+            run = self.load_state(checkpoint)
+            start, mpjpe_all, pampjpe_all, pve_all = run['next_frame'], run['mpjpe'], run['pampjpe'], run['pve']
+        for step, batch in enumerate(self._batches_from(start), start):
             if max_frames is not None and step >= max_frames:
                 break
             self.global_step, self.fit_losses = step, {}
@@ -115,9 +126,24 @@ class Adaptor(BaseAdaptor):
             self.fit_losses.update({'metrics/mpjpe': mpjpe, 'metrics/pampjpe': pampjpe, 'metrics/pve': pve})
             self.write_summaries(self.fit_losses)
             mpjpe_all.append(mpjpe); pampjpe_all.append(pampjpe); pve_all.append(pve)
+            if checkpoint is not None and every and (step + 1) % every == 0:
+                self.save_state(checkpoint, run=dict(next_frame=step + 1, mpjpe=mpjpe_all, pampjpe=pampjpe_all, pve=pve_all))
         summary = dict(mpjpe=float(np.mean(mpjpe_all)), pampjpe=float(np.mean(pampjpe_all)), pve=float(np.mean(pve_all)))
         self.save_records(mpjpe_all, pampjpe_all, pve_all)
         return summary
+
+    def _batches_from(self, start):
+        """The batches of ``dataloader`` from batch ``start`` on: a ``DataLoader`` over an indexable dataset skips the first
+        ``start`` batches without loading them; any other iterable is advanced with ``itertools.islice``."""
+        dl = self.dataloader
+        if start == 0:
+            return dl
+        ds = getattr(dl, 'dataset', None)
+        if isinstance(dl, torch.utils.data.DataLoader) and hasattr(ds, '__len__') and dl.batch_size is not None:
+            rest = torch.utils.data.Subset(ds, range(min(start * dl.batch_size, len(ds)), len(ds)))
+            return torch.utils.data.DataLoader(rest, batch_size=dl.batch_size, shuffle=False, num_workers=0, collate_fn=dl.collate_fn,
+                                               drop_last=dl.drop_last)
+        return itertools.islice(dl, start, None)
 
     def save_records(self, mpjpe_all, pampjpe_all, pve_all):
         """The eight result files of the reference driver (``write_records``)."""
@@ -179,6 +205,63 @@ class Adaptor(BaseAdaptor):
                 mpjpe, pampjpe, pve = self.inference(batch, self.model)
             self.optim_step_record.append(self.optimized_step)
         return mpjpe, pampjpe, pve
+
+    # ------------------------------------------------------------------ saved state (state.py, DESIGN.md section 11)
+    def _check_state_support(self):
+        opt = self.optimizer
+        if opt.grad_sync is not None or opt.pre_step_hook is not None:
+            raise ValueError('the state of a data-parallel (dist.attach) optimizer cannot be saved or loaded: its ranks would have '
+                             'to be resumed together')
+
+    def save_state(self, path, run=None):
+        """Write this video's state to ``path`` (``state.video_state``, atomically): theta, teacher, Adam moments and step count,
+        ``global_step``, the history ring, the ``random``, torch CPU and torch CUDA generator states and every record
+        (``run``: ``excute``'s own, kept with them).  Call it between frames: the copies to the host wait for the frame's last
+        write to the arenas on the current stream."""
+        self._check_state_support()
+        model, opt = getattr(self.model, 'module', self.model), self.optimizer
+        records = {k: getattr(self, k, None) for k in self.RECORDS}
+        records['run'] = run
+        st = state.video_state(self.options, 'adaptor', 1, model.arena, self.teacher.arena if self.options.use_meanteacher else None,
+                               opt.m, opt.v, opt.step_count, self.global_step,
+                               [(k, h['image'], h['s2d']) for k, h in sorted(self.history.items())],
+                               dict(random=random.getstate(), torch=torch.get_rng_state(), cuda=torch.cuda.get_rng_state(self.device)),
+                               records)
+        state.write(path, st)
+
+    def load_state(self, path):
+        """Continue from the state ``save_state`` wrote to ``path``: every check runs before any device work (ValueError), then
+        the arenas, moments and generator states are restored in place and the records replaced.  The next frame of ``adapt``
+        runs eagerly and the one after is captured again.  Returns the ``run`` the state was saved with."""
+        self._check_state_support()
+        st = state.read_video(path, self.options, 'adaptor')
+        model, opt = getattr(self.model, 'module', self.model), self.optimizer
+        torch.cuda.synchronize(self.device)                # no reader of the weights (predict_async) is still in flight
+        model.arena.copy_(st['theta'])
+        if self.options.use_meanteacher:
+            self.teacher.arena.copy_(st['teacher'])
+        opt.m.copy_(st['m'])
+        opt.v.copy_(st['v'])
+        opt.step_count, opt.wait_before_write = st['step_count'], []
+        self.global_step = st['frames']
+        self.history = {k: {'image': a.to(self.device), 's2d': b.to(self.device)} for k, (a, b) in st['history'].items()}
+        rng = st['rng']
+        random.setstate(rng['random'])
+        torch.set_rng_state(rng['torch'])
+        torch.cuda.set_rng_state(rng['cuda'], self.device)
+        rec = st['records']
+        for k in self.RECORDS:
+            v = rec.get(k)
+            setattr(self, k, v.to(self.device) if isinstance(v, torch.Tensor) and k == 'last_upper_loss' else v)
+        self._graph, self._graph_warm = None, None
+        torch.cuda.synchronize(self.device)
+        return rec.get('run')
+
+    def export_model(self, path):
+        """Write the adapted weights as a checkpoint in the reference's format, ``{'model': {'module.' + name: tensor}}`` with
+        the ``init_*`` buffers: it loads as ``model_file`` (and into the reference's ``hmr()``)."""
+        model = getattr(self.model, 'module', self.model)
+        state.write(path, {'model': layout.state_dict(model.arena, model._buffers, prefix='module.')})
 
     # ------------------------------------------------------------------ evaluation (reference :204-262)
     def predict(self, image, model=None):

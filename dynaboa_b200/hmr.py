@@ -20,40 +20,11 @@ from torch import nn
 
 from . import _lib
 from ._lib import ptr, stream
+from .layout import ArenaLayout, arena_layout as layout  # noqa: F401  (the arena's parameter table)
 
-_LAYOUT = None
 # callable(B, device) -> (3,2,B,1024) scaled keep-masks used by every HMR in train mode that has no mask_provider of its own
 # (parity tests replay the reference's recorded teacher dropout masks through the UNCHANGED driver this way)
 DEFAULT_MASK_PROVIDER = None
-
-
-class ArenaLayout:
-    """Parameter table queried from the library (names, offsets, logical shapes, strides)."""
-
-    def __init__(self):
-        lib = _lib.load()
-        self.n = lib.dboa_hmr_num_params()
-        self.floats = lib.dboa_hmr_arena_floats()
-        self.names, self.offsets, self.shapes, self.strides = [], [], [], []
-        name = C.create_string_buffer(128)
-        off, nd = C.c_longlong(), C.c_int()
-        shp, strd = (C.c_longlong * 4)(), (C.c_longlong * 4)()
-        for i in range(self.n):
-            _lib.check(lib.dboa_hmr_param_info(i, name, 128, C.byref(off), C.byref(nd), shp, strd), 'dboa_hmr_param_info')
-            self.names.append(name.value.decode())
-            self.offsets.append(off.value)
-            self.shapes.append(tuple(shp[k] for k in range(nd.value)))
-            self.strides.append(tuple(strd[k] for k in range(nd.value)))
-
-    def views(self, flat):
-        return [flat.as_strided(s, st, o) for s, st, o in zip(self.shapes, self.strides, self.offsets)]
-
-
-def layout():
-    global _LAYOUT
-    if _LAYOUT is None:
-        _LAYOUT = ArenaLayout()
-    return _LAYOUT
 
 
 _FEATURE_INFO = {}

@@ -189,14 +189,18 @@ class MultiInternetAdaptor(MultiVideoAdaptor):
                 self.writer.image(png_path, image)
 
     # ------------------------------------------------------------------ videos
-    def run(self, videos, exppath, names=None):
+    def run(self, videos, exppath, names=None, checkpoint=None, every=0):
         """Adapt every video of ``videos`` (``datasets.InternetVideo``s) through the G slots with ``MultiVideoAdaptor.run``'s
         queue (slots filled in order and refilled as soon as their video ends; video i starts with seed ``options.seed * 1000 +
         i``) and write each video's files under ``exppath/<name>/`` (``names``: default the videos' names).  The frames of
         the next tick are decoded, and the files written, on ``workers`` threads; a tick enqueues its device work before it
         waits for the previous tick's files, and the files of one video are written in frame order.  Returns once every file
         is on disk (an exception of a writer is raised here) with one summary per video: name, frames and, with the dynamic
-        loop, ``optim_step_record`` (the trip count of each frame)."""
+        loop, ``optim_step_record`` (the trip count of each frame).
+
+        ``checkpoint`` / ``every``: ``MultiVideoAdaptor.run``'s pool checkpoints.  A checkpoint is complete only once every
+        ``Pred_<t>`` file of the frames it covers is written; a resumed video is advanced to its frame by index, without
+        decoding the frames before it."""
         videos = list(videos)
         for i, v in enumerate(videos):
             if not callable(getattr(v, 'frame', None)) or not hasattr(v, '__len__') or not hasattr(v, 'name'):
@@ -212,13 +216,14 @@ class MultiInternetAdaptor(MultiVideoAdaptor):
         with ThreadPoolExecutor(max_workers=self.workers, thread_name_prefix='dboa-io') as io:
             pending = []                                     # the previous tick's writes
 
-            def frames_of(i):
-                """Video i's frames as (video, t, Future of the decoded frame), frame t + 1 submitted when frame t is taken."""
+            def frames_of(i, k=0):
+                """Video i's frames from frame k on as (video, t, Future of the decoded frame), frame t + 1 submitted when frame t
+                is taken."""
                 v = videos[i]
-                if len(v) == 0:
+                if len(v) <= k:
                     return
-                nxt = io.submit(decode, v.frame(0)[0])
-                for t in range(len(v)):
+                nxt = io.submit(decode, v.frame(k)[0])
+                for t in range(k, len(v)):
                     cur, nxt = nxt, (io.submit(decode, v.frame(t + 1)[0]) if t + 1 < len(v) else None)
                     yield (v, t, cur)
 
@@ -236,7 +241,8 @@ class MultiInternetAdaptor(MultiVideoAdaptor):
                     out['optim_step_record'] = [] if g is None else list(self.optim_step_record[g])
                 return out
 
-            out = self._queue([_Frames(frames_of, i) for i in range(len(videos))], tick, finish)
+            out = self._queue([_Frames(frames_of, i) for i in range(len(videos))], tick, finish, checkpoint=checkpoint, every=every,
+                              items_from=frames_of, barrier=lambda: pending)
             for f in pending:
                 f.result()
         return out

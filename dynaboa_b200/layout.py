@@ -5,7 +5,13 @@ model/hmr.py:67-124 (``HMR.__init__`` / ``_make_layer``) and SURVEY.md §8(a1):
 169 parameter tensors, 26 977 501 scalars, in module-registration order, plus
 the three ``init_*`` buffers.  The CUDA library holds the same table
 (csrc/hmr_plan.cu) and ``tests/test_layout.py`` checks they agree.
+
+``ArenaLayout`` is that table as the library stores it (offset, logical shape and strides of every
+parameter inside the one flat fp32 arena); ``state_dict`` maps an arena to named tensors with it, the
+mapping ``HMR``'s parameters use, and ``digest`` fingerprints it for saved states (state.py).
 """
+import ctypes as C
+import hashlib
 from collections import OrderedDict
 
 BLOCKS = (3, 4, 6, 3)            # reference model/hmr.py:322  hmr() -> HMR(Bottleneck, [3, 4, 6, 3])
@@ -84,3 +90,60 @@ def num_params():
 FEATURE_NAMES = ['stem_conv', 'layer1', 'layer2', 'layer3', 'layer4', 'pooled',
                  'fc1_it0', 'drop1_it0', 'fc2_it0', 'fc1_it1', 'drop1_it1', 'fc2_it1',
                  'fc1_it2', 'drop1_it2', 'fc2_it2']
+
+
+class ArenaLayout:
+    """Parameter table queried from the library (names, offsets, logical shapes, strides)."""
+
+    def __init__(self):
+        from . import _lib
+        lib = _lib.load()
+        self.n = lib.dboa_hmr_num_params()
+        self.floats = lib.dboa_hmr_arena_floats()
+        self.names, self.offsets, self.shapes, self.strides = [], [], [], []
+        name = C.create_string_buffer(128)
+        off, nd = C.c_longlong(), C.c_int()
+        shp, strd = (C.c_longlong * 4)(), (C.c_longlong * 4)()
+        for i in range(self.n):
+            _lib.check(lib.dboa_hmr_param_info(i, name, 128, C.byref(off), C.byref(nd), shp, strd), 'dboa_hmr_param_info')
+            self.names.append(name.value.decode())
+            self.offsets.append(off.value)
+            self.shapes.append(tuple(shp[k] for k in range(nd.value)))
+            self.strides.append(tuple(strd[k] for k in range(nd.value)))
+
+    def views(self, flat):
+        return [flat.as_strided(s, st, o) for s, st, o in zip(self.shapes, self.strides, self.offsets)]
+
+
+_LAYOUT = None
+
+
+def arena_layout():
+    """The library's ``ArenaLayout``, queried once."""
+    global _LAYOUT
+    if _LAYOUT is None:
+        _LAYOUT = ArenaLayout()
+    return _LAYOUT
+
+
+def digest():
+    """sha256 of the arena's parameter table (name, shape, offset and strides of every parameter, the arena size) and of the
+    buffer shapes: two arenas with the same digest hold the same parameter at the same place."""
+    lay = arena_layout()
+    rows = [lay.floats] + list(zip(lay.names, lay.shapes, lay.offsets, lay.strides)) + list(buffer_shapes().items())
+    return hashlib.sha256(repr(rows).encode()).hexdigest()
+
+
+def state_dict(arena, buffers, prefix=''):
+    """The reference's state_dict of the weights in the flat ``arena``: ``prefix + name`` -> a contiguous copy of each of the
+    169 parameters (the ``HMR`` parameter views of the arena), then the ``init_*`` buffers of ``buffers``, on the host."""
+    lay = arena_layout()
+    if arena.dim() != 1 or arena.numel() != lay.floats:
+        raise ValueError(f'expected a flat arena of {lay.floats} floats, got shape {tuple(arena.shape)}')
+    def own(t):                       # a host tensor with a storage of its own (a saved view would carry the whole arena)
+        t = t.detach().contiguous()
+        return t.cpu() if t.is_cuda else t.clone()
+    out = OrderedDict((prefix + n, own(v)) for n, v in zip(lay.names, lay.views(arena)))
+    for k in buffer_shapes():
+        out[prefix + k] = own(buffers[k])
+    return out

@@ -10,19 +10,23 @@ G slots are a pool: a slot whose batch is None sits the frame out (its CTAs retu
 'final' or 'all' every video gets the records and result files of the single-video driver.  DESIGN.md section 10.
 """
 import ctypes as C
+import itertools
 import os
 import random
 
 import numpy as np
 import torch
 
-from . import _lib, hmr as hmr_mod
+from . import _lib, hmr as hmr_mod, layout, state as state_mod
 from ._lib import ptr, stream
 from .fused import Step, fused_adapt, pick, runs
 
 EVAL_MODES = ('none', 'final', 'all')
 GT_KEYS = ('pose', 'betas', 'gender')
 PENDING_FRAMES = 256        # device records kept before adapt forms them on the host (one synchronisation)
+# a slot's host records, one entry per slot, as a slot state holds them
+SLOT_RECORDS = ('mpjpe_all', 'pampjpe_all', 'pve_all', 'mpjpe_all_lower', 'pampjpe_all_lower', 'mpjpe_statistics', 'pampjpe_statistics',
+                'kp2dloss_lower_all', 'kp2dloss_upper_all', 'optim_step_record', 'feat_sims', 'optimized_step', 'last_retrieval')
 
 
 def check_options(options, n_videos, dynamic_loop=False):
@@ -60,6 +64,14 @@ def slot_records(frame, G, prev_upper_loss):
     on = frame.mask
     return ({k: pick(on, G, v) for k, v in frame.fit.items()}, [pick(on, G, v) for v in frame.lower],
             pick(on, G, frame.upper_loss, prev_upper_loss))
+
+
+def _items_from(video, k):
+    """An iterator over ``video``'s items from item k on: by index for a video with ``len`` and indexing (nothing before k is
+    read), with ``itertools.islice`` for any other iterable."""
+    if k and hasattr(video, '__len__') and hasattr(video, '__getitem__'):
+        return (video[t] for t in range(k, len(video)))
+    return itertools.islice(iter(video), k, None)
 
 
 class MultiVideoAdaptor:
@@ -119,6 +131,7 @@ class MultiVideoAdaptor:
         self.mpjpe_all_lower, self.pampjpe_all_lower = [None] * G, [None] * G
         self.mpjpe_statistics, self.pampjpe_statistics = [{} for _ in range(G)], [{} for _ in range(G)]
         self.kp2dloss_lower_all, self.kp2dloss_upper_all = [[] for _ in range(G)], [{} for _ in range(G)]
+        self._writer, self._pinned = state_mod.Writer(), state_mod.Pinned()     # checkpoints written in the background (save)
         self._step = Step(o, G, self.thetas, self.grad, self.buffers, base.smpl_neutral, base.gmm_f, teacher=self.teachers,
                           teacher_buffers=self.buffers, teacher_masks=self._teacher_masks, kp_range=self.kp_range,
                           motion_lead=self.motion_lead, bank=base.bank if o.retrieval else None, rngs=self.rngs,
@@ -131,10 +144,17 @@ class MultiVideoAdaptor:
         from .adaptor import Adaptor
         return Adaptor(options)
 
-    def start(self, g, seed=None):
+    def start(self, g, seed=None, state=None):
         """Put a new video into slot g: theta and teacher from the checkpoint, zero Adam moments, step and frame counts, an empty
         history, empty records, and ``rngs[g] = random.Random(seed)`` (default ``options.seed * 1000 + g``).  The records of
-        the frames adapted so far are formed on the host first (one synchronisation, if any are pending)."""
+        the frames adapted so far are formed on the host first (one synchronisation, if any are pending).
+
+        ``state``: a video state written by ``save_slot`` (its path, or the dict ``state.read_video`` returned) of a pool with
+        the same G and compatible options, from any slot: slot g continues that video instead -- theta, teacher, moments, step
+        count, ``video_steps[g]``, history ring, ``rngs[g]`` and records.  It is checked before any device work (ValueError)."""
+        if state is not None and not isinstance(state, dict):
+            self._check_slot(g)
+            state = state_mod.read_video(state, self.options, 'slot', self.G)
         self._reset_weights(g)
         self._form_records()
         self.video_steps[g] = 0
@@ -146,11 +166,16 @@ class MultiVideoAdaptor:
         self.mpjpe_all_lower[g], self.pampjpe_all_lower[g] = [[] for _ in range(n)], [[] for _ in range(n)]
         self.mpjpe_statistics[g], self.pampjpe_statistics[g] = {}, {}
         self.kp2dloss_lower_all[g], self.kp2dloss_upper_all[g] = [], {}
+        if state is not None:
+            self._restore_slot(g, state)
+
+    def _check_slot(self, g):
+        if not isinstance(g, int) or not 0 <= g < self.G:
+            raise ValueError(f'slot {g!r} is not one of the {self.G} slots')
 
     def _reset_weights(self, g):
         """Slot g's theta and teacher back to the checkpoint and a fresh Adam (zero moments, step count 0)."""
-        if not isinstance(g, int) or not 0 <= g < self.G:
-            raise ValueError(f'slot {g!r} is not one of the {self.G} slots')
+        self._check_slot(g)
         self.thetas[g].copy_(self.base.model.module.arena.detach())
         if self.teachers is not None:
             self.teachers[g].copy_(self.base.teacher.arena.detach())
@@ -351,14 +376,19 @@ class MultiVideoAdaptor:
                     feat_sims=dict(self.feat_sims[g]), optim_step_record=list(self.optim_step_record[g]),
                     kp2dlosses_lower=list(self.kp2dloss_lower_all[g]), kp2dlosses_upper=dict(self.kp2dloss_upper_all[g]))
 
-    def run(self, videos, exppath=None, names=None):
+    def run(self, videos, exppath=None, names=None, checkpoint=None, every=0):
         """Adapt every video of ``videos`` (a list of iterables of batch dicts with batch size 1: a ``DataLoader`` over a
         sequence, a ``SyntheticStream``) through the G slots.  Slots are filled in order and refilled from the queue as soon as
         their video ends; video i starts with ``start(g, seed=options.seed * 1000 + i)``, so its seed follows the video, and
         ``slot_video[g]`` is the index of the video slot g holds (for a ``mask_provider``).  Returns one summary per video, in
         order: name, frames, and the mean MPJPE, PA-MPJPE and PVE of its frames (``res.txt``'s; NaN without evaluation).  With
         ``exppath``, each video's eight result files go to ``exppath/<name>/`` when it finishes (``names``: default the
-        video's index)."""
+        video's index).
+
+        ``checkpoint``: a directory of pool checkpoints (``save``), written every ``every`` ticks and once more at the end.  When it
+        holds a complete checkpoint the run resumes from it: the finished videos' summaries are returned as recorded (their
+        result files are left alone), every video in flight continues in its slot from its own frame, and the queue goes on
+        from there.  The summaries and result files are those of a run that was never interrupted."""
         from .adaptor import write_records
         videos = list(videos)
         names = video_names(videos, names, default=[str(i) for i in range(len(videos))])
@@ -373,20 +403,37 @@ class MultiVideoAdaptor:
                 os.makedirs(d, exist_ok=True)
                 write_records(d, rec['frames'] - 1, rec)
             return dict(name=names[i], frames=rec['frames'], mpjpe=mean(rec['mpjpe']), pampjpe=mean(rec['pampjpe']), pve=mean(rec['pve']))
-        return self._queue(videos, self.adapt, finish)
+        return self._queue(videos, self.adapt, finish, checkpoint=checkpoint, every=every)
 
-    def _queue(self, videos, tick, finish):
+    def _queue(self, videos, tick, finish, checkpoint=None, every=0, items_from=None, barrier=None):
         """``run``'s queue: the slots are filled in order and refilled as soon as their video ends; video i starts with
         ``start(g, seed=options.seed * 1000 + i)`` and ``slot_video[g] = i``.  ``tick(items)`` advances the pool by one frame,
         ``items[g]`` being slot g's next item of its video (None: an idle slot); ``finish(i, g)`` returns video i's summary once
-        it ended in slot g (g None: video i was empty), before the slot is refilled.  Returns the summaries in order."""
-        queue, its, nxt, out = list(range(len(videos))), [None] * self.G, [None] * self.G, [None] * len(videos)
+        it ended in slot g (g None: video i was empty), before the slot is refilled.  Returns the summaries in order.
+
+        ``checkpoint`` / ``every``: ``run``'s.  ``items_from(i, k)``: an iterator over video i's items from item k on (default
+        ``items_from``); ``barrier()``: futures of files a checkpoint taken now covers (``save``)."""
+        n = len(videos)
+        queue, its, nxt, out = list(range(n)), [None] * self.G, [None] * self.G, [None] * n
+        items_from = items_from or (lambda i, k: _items_from(videos[i], k))
+        run = self.load(checkpoint) if checkpoint is not None else None
+        if run is not None:
+            if run['videos'] != n:
+                raise ValueError(f'{checkpoint}: the checkpoint is of a queue of {run["videos"]} videos, not {n}')
+            queue, out = list(run['queue']), list(run['out'])
+            for g in range(self.G):
+                if self.slot_video[g] is not None:
+                    its[g] = items_from(self.slot_video[g], self.video_steps[g])
+                    nxt[g] = next(its[g], None)
+
+        def save():
+            self.save(checkpoint, run=dict(videos=n, queue=queue, out=out), barrier=barrier, wait=False)
 
         def fill(g):
             self.slot_video[g] = None
             while queue:
                 i = queue.pop(0)
-                its[g] = iter(videos[i])
+                its[g] = items_from(i, 0)
                 nxt[g] = next(its[g], None)
                 if nxt[g] is None:
                     out[i] = finish(i, None)
@@ -395,18 +442,134 @@ class MultiVideoAdaptor:
                 self.slot_video[g] = i
                 return
 
-        for g in range(self.G):
-            fill(g)
-        while any(i is not None for i in self.slot_video):
-            tick([nxt[g] if self.slot_video[g] is not None else None for g in range(self.G)])
-            for g in range(self.G):
-                if self.slot_video[g] is None:
-                    continue
-                nxt[g] = next(its[g], None)
-                if nxt[g] is None:
-                    out[self.slot_video[g]] = finish(self.slot_video[g], g)
+        try:
+            if run is None:
+                for g in range(self.G):
                     fill(g)
+            while any(i is not None for i in self.slot_video):
+                tick([nxt[g] if self.slot_video[g] is not None else None for g in range(self.G)])
+                for g in range(self.G):
+                    if self.slot_video[g] is None:
+                        continue
+                    nxt[g] = next(its[g], None)
+                    if nxt[g] is None:
+                        out[self.slot_video[g]] = finish(self.slot_video[g], g)
+                        fill(g)
+                if checkpoint is not None and every and self.global_step % every == 0:
+                    save()
+            if checkpoint is not None:
+                save()
+        finally:
+            self._writer.wait()                              # no checkpoint is still being written when run returns or raises
         return out
+
+    # ------------------------------------------------------------------ saved state (state.py, DESIGN.md section 11)
+    def _slot_state(self, g, copy):
+        """Slot g's video state, its arenas brought to the host by ``copy(key, device tensor)`` and its history frames by
+        ``state.host_copy``, both on the current stream (the records must have been formed)."""
+        G, small = self.G, state_mod.host_copy
+        hist = []
+        for k, (image, kp) in sorted(self.histories[g].items()):
+            b = image.shape[0] // G
+            hist.append((k, small(image[g * b:(g + 1) * b]), small(kp[g * b:(g + 1) * b])))
+        records = {name: getattr(self, name)[g] for name in SLOT_RECORDS}
+        records['last_upper_loss'] = small(self.last_upper_loss[g:g + 1])
+        return state_mod.video_state(self.options, 'slot', G, copy(('theta', g), self.thetas[g]),
+                                     None if self.teachers is None else copy(('teacher', g), self.teachers[g]),
+                                     copy(('m', g), self.m[g]), copy(('v', g), self.v[g]), self.step_counts[g], self.video_steps[g], hist,
+                                     dict(random=self.rngs[g].getstate()), records)
+
+    def _restore_slot(self, g, st):
+        G, dev = self.G, self.thetas.device
+        self.thetas[g].copy_(st['theta'])
+        if self.teachers is not None:
+            self.teachers[g].copy_(st['teacher'])
+        self.m[g].copy_(st['m'])
+        self.v[g].copy_(st['v'])
+        self.step_counts[g], self.video_steps[g] = st['step_count'], st['frames']
+        h = self.histories[g]
+        for k, rows in st['history'].items():                 # the pool's history frames hold every slot's rows: slot g's filled
+            full = []
+            for t in rows:
+                b = t.shape[0]
+                f = torch.zeros((G * b,) + tuple(t.shape[1:]), dtype=t.dtype, device=dev)
+                f[g * b:(g + 1) * b].copy_(t)
+                full.append(f)
+            h[k] = tuple(full)
+        self.rngs[g].setstate(st['rng']['random'])
+        rec = st['records']
+        for name in SLOT_RECORDS:
+            getattr(self, name)[g] = rec[name]
+        self.last_upper_loss[g] = rec['last_upper_loss'].to(dev)[0]
+
+    def save_slot(self, g, path):
+        """Write slot g's video as a video state to ``path`` (durably and atomically): what ``start(g', state=path)`` continues
+        from in any slot of a pool with the same G.  Between frames: the copies wait for the slot's last write."""
+        self._check_slot(g)
+        self._check_runtime()
+        self._form_records()
+        st = self._slot_state(g, lambda key, t: state_mod.host_copy(t))
+        torch.cuda.current_stream().synchronize()
+        state_mod.write(path, st)
+
+    def save(self, root, slots=None, run=None, barrier=None, wait=True):
+        """Write a pool checkpoint under the directory ``root``: one video state per slot of ``slots`` (default: every slot that
+        holds a video of ``run``, or all G slots of a pool driven by ``adapt``), a pool file (``global_step``, torch's CUDA
+        generator state -- the teacher masks of every slot are drawn from it in slot order --, ``slot_video`` and ``run``) and
+        the manifest, written last.  The arenas come to the host through pinned buffers on the current stream and the files are
+        written on a background thread, after the futures of ``barrier()`` (files the checkpoint covers) are done; a new save
+        waits for the previous one.  ``wait``: return once the checkpoint is durable."""
+        self._check_runtime()
+        self._writer.wait()                                  # the pinned buffers are free again
+        if slots is None:
+            slots = [g for g in range(self.G) if self.slot_video[g] is not None] if run is not None else list(range(self.G))
+        self._form_records()
+        states = {g: self._slot_state(g, self._pinned.copy) for g in slots}
+        pool = state_mod.header(state_mod.POOL, self.options)
+        pool.update(G=self.G, global_step=self.global_step, cuda_rng=torch.cuda.get_rng_state(self.thetas.device),
+                    slot_video=list(self.slot_video), run=state_mod.plain(run))
+        done = torch.cuda.Event()
+        done.record()
+        waits = list(barrier()) if barrier is not None else []
+
+        def job():
+            for f in waits:
+                f.result()
+            path = state_mod.new_checkpoint(root)
+            for g, st in states.items():
+                state_mod.write(os.path.join(path, f'slot{g}.pt'), st)
+            state_mod.write(os.path.join(path, 'pool.pt'), pool)
+            state_mod.commit(root, path, {g: f'slot{g}.pt' for g in states})
+        self._writer.submit(job, done)
+        if wait:
+            self._writer.wait()
+
+    def load(self, root):
+        """Continue from the newest complete checkpoint ``save`` wrote under ``root``: every file is checked first (ValueError),
+        then the saved slots are restored with ``start(g, state=...)``, the others marked empty in ``slot_video``, and
+        ``global_step`` and torch's CUDA generator set.  Returns the checkpoint's ``run`` (None without a checkpoint)."""
+        found = state_mod.latest(root)
+        if found is None:
+            return None
+        path, man = found
+        self._check_runtime()
+        pool = state_mod.read(os.path.join(path, man['pool']), state_mod.POOL, self.options)
+        if pool.get('G') != self.G:
+            raise ValueError(f'{path}: a checkpoint of a {pool.get("G")}-slot pool cannot be loaded into {self.G} slots')
+        states = {g: state_mod.read_video(os.path.join(path, f), self.options, 'slot', self.G) for g, f in man['slots'].items()}
+        for g in range(self.G):
+            self.slot_video[g] = pool['slot_video'][g] if g in states else None
+            if g in states:
+                self.start(g, state=states[g])
+        self.global_step = pool['global_step']
+        torch.cuda.set_rng_state(pool['cuda_rng'], self.thetas.device)
+        torch.cuda.synchronize(self.thetas.device)
+        return state_mod.unplain(pool['run'])
+
+    def export_model(self, g, path):
+        """Write video g's adapted weights as a checkpoint in the reference's format (``Adaptor.export_model``)."""
+        self._check_slot(g)
+        state_mod.write(path, {'model': layout.state_dict(self.thetas[g], self.buffers, prefix='module.')})
 
     def predict(self, images, active=None):
         """Every video's prediction for its rows of ``images`` with its current weights: a list of G dicts with rotmat, betas,
