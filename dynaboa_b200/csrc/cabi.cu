@@ -22,6 +22,8 @@ int hmr_prepare();
 void hmr_set_fused_backward(bool on);
 bool hmr_fused_forward();
 bool hmr_fused_backward();
+void hmr_set_tc_mode(int mode);
+int hmr_tc_mode();
 int hmr_num_params();
 long long hmr_arena_floats();
 int hmr_param_info(int i, char* name, int cap, long long* off, int* ndim, long long shape[4], long long stride[4]);
@@ -84,7 +86,7 @@ int dboa_stream_wait_external(dboa_stream_t stream, void* event) {
     if (e != cudaSuccess) { g_last_cuda_error = (int)e; return DBOA_ERR_CUDA; }
     return DBOA_OK;
 }
-int dboa_set_tensor_core_conv(int enable) { conv_tc_set_mode(enable); return DBOA_OK; }
+int dboa_set_tensor_core_conv(int enable) { hmr_set_tc_mode(enable); return DBOA_OK; }
 
 int dboa_set_fused_forward(int enable) { hmr_set_fused_forward(enable != 0); return DBOA_OK; }
 int dboa_get_fused_forward(void) { return hmr_fused_forward() ? 1 : 0; }
@@ -143,43 +145,52 @@ int dboa_hmr_backward_active(const float* arena, const float* tape, int B, int m
 int dboa_conv2d_fwd(const float* x, const float* w, float* y, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad, int Kpitch,
                     float* ws, long long ws_floats, dboa_stream_t stream) {
     if (!x || !w || !y) return DBOA_ERR_ARG;
-    return conv_fwd(x, w, y, make_dims(B, Hi, Wi, Cin, Cout, k, stride, pad, Kpitch), ws, ws ? (size_t)ws_floats : 0, ST(stream));
+    (void)ws; (void)ws_floats;
+    return conv_fwd(x, w, y, make_dims(B, Hi, Wi, Cin, Cout, k, stride, pad, Kpitch), ST(stream));
 }
 int dboa_conv2d_dgrad(const float* dy, const float* w, float* dx, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad,
                       int Kpitch, int accumulate, float* ws, long long ws_floats, dboa_stream_t stream) {
     if (!dy || !w || !dx) return DBOA_ERR_ARG;
-    return conv_dgrad(dy, w, dx, make_dims(B, Hi, Wi, Cin, Cout, k, stride, pad, Kpitch), accumulate, ws, ws ? (size_t)ws_floats : 0, ST(stream));
+    (void)ws; (void)ws_floats;
+    return conv_dgrad(dy, w, dx, make_dims(B, Hi, Wi, Cin, Cout, k, stride, pad, Kpitch), accumulate, ST(stream));
 }
 int dboa_conv2d_wgrad(const float* dy, const float* x, float* dw, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad,
                       int Kpitch, float* ws, long long ws_floats, dboa_stream_t stream) {
     if (!dy || !x || !dw) return DBOA_ERR_ARG;
-    return conv_wgrad(dy, x, dw, make_dims(B, Hi, Wi, Cin, Cout, k, stride, pad, Kpitch), ws, ws ? (size_t)ws_floats : 0, ST(stream));
+    const ConvDims d = make_dims(B, Hi, Wi, Cin, Cout, k, stride, pad, Kpitch);
+    const int s = stem_wgrad(dy, x, dw, d, ws, ws ? (size_t)ws_floats : 0, ST(stream));     // the stem shape, given a workspace
+    if (s != DBOA_ERR_UNSUPPORTED) return s;
+    return conv_wgrad(dy, x, dw, d, ST(stream));
 }
 int dboa_conv1x1_tc_fwd(const float* x, const float* w, float* y, int M, int Cin, int Cout, float* ws, long long ws_floats,
                         dboa_stream_t stream) {
     if (!x || !w || !y) return DBOA_ERR_ARG;
     (void)ws; (void)ws_floats;                 /* kept in the signature: the split-K reduction lives in shared memory (DSMEM) now */
+    if (hmr_tc_mode() == 0) return DBOA_ERR_UNSUPPORTED;
     return conv1x1_tc_fwd(x, w, y, M, Cin, Cout, ST(stream), cabi_pdl());
 }
 int dboa_conv2d_tc_fwd(const float* x, const float* w, float* y, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad,
                        int Kpitch, dboa_stream_t stream) {
     if (!x || !w || !y) return DBOA_ERR_ARG;
+    if (hmr_tc_mode() == 0) return DBOA_ERR_UNSUPPORTED;
     return conv_tc_fwd(x, w, y, make_dims(B, Hi, Wi, Cin, Cout, k, stride, pad, Kpitch), ST(stream), cabi_pdl());
 }
 int dboa_conv2d_tc_dgrad(const float* dy, const float* w, float* dx, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad,
                          int Kpitch, int accumulate, dboa_stream_t stream) {
     if (!dy || !w || !dx) return DBOA_ERR_ARG;
+    if (hmr_tc_mode() < 2) return DBOA_ERR_UNSUPPORTED;
     return conv_tc_dgrad(dy, w, dx, make_dims(B, Hi, Wi, Cin, Cout, k, stride, pad, Kpitch), accumulate, ST(stream), cabi_pdl());
 }
 int dboa_conv2d_tc_wgrad(const float* dy, const float* x, float* dw, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad,
                          int Kpitch, dboa_stream_t stream) {
     if (!dy || !x || !dw) return DBOA_ERR_ARG;
+    if (hmr_tc_mode() < 2) return DBOA_ERR_UNSUPPORTED;
     return conv_tc_wgrad(dy, x, dw, make_dims(B, Hi, Wi, Cin, Cout, k, stride, pad, Kpitch), ST(stream), cabi_pdl());
 }
 int dboa_conv2d_wgrad_tma(const float* dy, const float* x, float* dw, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad,
                           int Kpitch, dboa_stream_t stream) {
     if (!dy || !x || !dw) return DBOA_ERR_ARG;
-    return conv_wgrad_tc(dy, x, dw, make_dims(B, Hi, Wi, Cin, Cout, k, stride, pad, Kpitch), ST(stream));
+    return conv_tc_wgrad(dy, x, dw, make_dims(B, Hi, Wi, Cin, Cout, k, stride, pad, Kpitch), ST(stream), false);
 }
 int dboa_dgrad_fused(const dboa_dgrad_args* f, int B, int H, int Cin, int Cout, int k, dboa_stream_t stream) {
     if (!f || !f->dz || !f->y_c || !f->w || !f->stats_c || !f->sums_c || !f->gamma_c || !f->out) return DBOA_ERR_ARG;

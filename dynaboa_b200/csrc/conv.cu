@@ -376,8 +376,7 @@ static int launch_z_cluster(K kernel, dim3 grid, cudaStream_t st, Args... args) 
     return launch_ex(kernel, grid, dim3(NT), 0, st, dim3(1, 1, grid.z), true, args...);
 }
 
-int conv_fwd(const float* x, const float* w, float* y, const ConvDims& d, float* ws, size_t ws_floats, cudaStream_t st) {
-    (void)ws; (void)ws_floats;
+int conv_fwd(const float* x, const float* w, float* y, const ConvDims& d, cudaStream_t st) {
     if (d.groups < 1) return DBOA_ERR_SHAPE;
     if (d.Cout % BN != 0 || d.Kpitch % 4 != 0) return DBOA_ERR_SHAPE;
     const int M = d.B * d.Ho * d.Wo, K = d.kh * d.kw * d.Cin;
@@ -392,9 +391,7 @@ int conv_fwd(const float* x, const float* w, float* y, const ConvDims& d, float*
     return launch_z_cluster(g ? conv_fwd_kernel<1, true> : conv_fwd_kernel<1, false>, grid, st, x, w, y, d, klen);
 }
 
-int conv_dgrad(const float* dy, const float* w, float* dx, const ConvDims& d, int accumulate, float* ws, size_t ws_floats,
-               cudaStream_t st) {
-    (void)ws; (void)ws_floats;
+int conv_dgrad(const float* dy, const float* w, float* dx, const ConvDims& d, int accumulate, cudaStream_t st) {
     if (d.groups < 1) return DBOA_ERR_SHAPE;
     if (d.Cin % BN != 0 || d.Cout % BK != 0) return DBOA_ERR_SHAPE;
     const int M = d.B * d.Hi * d.Wi, K = d.kh * d.kw * d.Cout;
@@ -406,10 +403,7 @@ int conv_dgrad(const float* dy, const float* w, float* dx, const ConvDims& d, in
     return launch_z_cluster(d.groups > 1 ? conv_dgrad_kernel<true> : conv_dgrad_kernel<false>, grid, st, dy, w, dx, d, klen, accumulate);
 }
 
-int conv_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, float* ws, size_t ws_floats, cudaStream_t st) {
-    // the stem has its own kernel (last on the critical path of every backward); the generic kernel below takes every other shape
-    const int s = stem_wgrad(dy, x, dw, d, ws, ws_floats, st);
-    if (s != DBOA_ERR_UNSUPPORTED) return s;
+int conv_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, cudaStream_t st) {
     if (d.Cout % BM != 0 || d.groups < 1) return DBOA_ERR_SHAPE;
     const int Mpix = d.B * d.Ho * d.Wo, K = d.kh * d.kw * d.Cin;
     const int piters = ceil_div(Mpix, BK);

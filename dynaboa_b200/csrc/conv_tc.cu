@@ -38,15 +38,9 @@ namespace cg = cooperative_groups;
 
 namespace dboa {
 
-// 0 = fp32 CUDA cores; 1 = forward on tensor cores; 2 = forward, data and weight gradient on tensor cores;
-// 3 = forward and data gradient on tensor cores, weight gradient on CUDA cores (default: C2 at batch 1 on an H100 SXM, 700 W,
-// runs alternated in one session: 129.0-129.1 adapted frames/s against 116.3-116.6 with mode 2; a batch-1 weight gradient
-// reduces over few pixels into many outputs, which the CUDA-core kernel's cluster split serves better)
-static int g_tc_mode = 3;
-bool conv_tc_enabled() { return g_tc_mode != 0; }
-bool conv_tc_bwd_enabled() { return g_tc_mode >= 2; }
-bool conv_tc_wgrad_enabled() { return g_tc_mode == 2; }
-void conv_tc_set_mode(int mode) { g_tc_mode = mode; }
+// The launchers below refuse only shapes they do not take.  Which convolution products run here is the network plan's choice
+// (hmr_plan.cu, the tensor-core mode of dboa_set_tensor_core_conv); the stand-alone C-ABI entry points apply the same mode in
+// their wrappers (cabi.cu).
 
 namespace tc {
 
@@ -651,23 +645,17 @@ static bool shape_ok(const ConvDims& d) {
 }  // namespace tc
 
 int conv_tc_fwd(const float* x, const float* w, float* y, const ConvDims& d, cudaStream_t st, bool pdl) {
-    if (g_tc_mode == 0 || !tc::shape_ok(d)) return DBOA_ERR_UNSUPPORTED;
+    if (!tc::shape_ok(d)) return DBOA_ERR_UNSUPPORTED;
     return tc::launch<tc::FWD>(x, w, y, d, d.B * d.Ho * d.Wo, d.Cout, d.kh * d.kw * d.Cin, 0, st, pdl);
 }
 int conv_tc_dgrad(const float* dy, const float* w, float* dx, const ConvDims& d, int accumulate, cudaStream_t st, bool pdl) {
-    if (g_tc_mode < 2 || !tc::shape_ok(d)) return DBOA_ERR_UNSUPPORTED;
+    if (!tc::shape_ok(d)) return DBOA_ERR_UNSUPPORTED;
     if (d.stride == 2 && ((d.Hi | d.Wi) & 1)) return DBOA_ERR_UNSUPPORTED;       // the parity-class enumeration needs even extents
     return tc::launch<tc::DGRAD>(dy, w, dx, d, d.B * d.Hi * d.Wi, d.Cin, d.kh * d.kw * d.Cout, accumulate, st, pdl);
 }
 int conv_tc_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, cudaStream_t st, bool pdl) {
-    if (g_tc_mode < 2 || !tc::shape_ok(d)) return DBOA_ERR_UNSUPPORTED;
-    return tc::launch<tc::WGRAD>(dy, x, dw, d, d.Cout, d.kh * d.kw * d.Cin, d.B * d.Ho * d.Wo, 1, st, pdl);
-}
-
-// weight gradient on the tensor cores whatever the plan's mode (C ABI dboa_conv2d_wgrad_tma); dw is accumulated
-int conv_wgrad_tc(const float* dy, const float* x, float* dw, const ConvDims& d, cudaStream_t st) {
     if (!tc::shape_ok(d)) return DBOA_ERR_UNSUPPORTED;
-    return tc::launch<tc::WGRAD>(dy, x, dw, d, d.Cout, d.kh * d.kw * d.Cin, d.B * d.Ho * d.Wo, 1, st, false);
+    return tc::launch<tc::WGRAD>(dy, x, dw, d, d.Cout, d.kh * d.kw * d.Cin, d.B * d.Ho * d.Wo, 1, st, pdl);
 }
 
 bool conv_fused_ok(const FusedConv& f) {

@@ -164,7 +164,7 @@ static const Tape& tape_for(int B) {
     return cache[B];
 }
 
-static const long long kConvWs = 8LL << 20;    // split-K workspace (floats)
+static const long long kConvWs = 8LL << 20;    // workspace of the stem weight gradient's partials (floats)
 
 struct Scratch {
     float *ws, *g0, *g1, *t1, *t2, *t3, *t4, *t5, *t6, *gnp, *dP, *dy_dec, *d_h2, *d_h1, *dxc, *dxf, *tmp1024, *lin_ws;
@@ -264,8 +264,6 @@ long long hmr_bucket_offset(int k) {        // first float of bucket k's span; b
 // DBOA_ASYNC_WGRAD=0 in the environment keeps everything on the caller's stream (A/B measurements, debugging)
 static const bool g_async_enabled = [] { const char* e = getenv("DBOA_ASYNC_WGRAD"); return !(e && e[0] == '0'); }();
 
-static ConvDims dims_of(const ConvLayer& c, int B, int groups = 1, unsigned long long active = ~0ULL);
-
 // Fused plan (conv_tc.cu with an operand transform): every convolution applies the GroupNorm (+ residual, ReLU) of its operand on
 // load and leaves the statistics of its output as fixed-point sums; the fused data gradient applies GroupNorm backward on load
 // and produces the sums of the next GroupNorm backward in its epilogue.  Both plans fill the same tape.  The default is one
@@ -277,6 +275,16 @@ static bool g_fused_fwd = [] { const char* e = getenv("DBOA_FUSED_FWD"); return 
 void hmr_set_fused_forward(bool on) { g_fused_fwd = on; }
 bool hmr_fused_forward() { return g_fused_fwd; }
 bool hmr_fused_backward() { return g_fused_bwd; }
+
+// Tensor-core mode (dboa_set_tensor_core_conv): which convolution products run on the wgmma kernel (conv_tc.cu) when it takes the
+// shape.  0 = none (fp32 CUDA cores); 1 = forward; 2 = forward, data and weight gradient; 3 = forward and data gradient, weight
+// gradient on CUDA cores (default: C2 at batch 1 on an H100 SXM, 700 W, runs alternated in one session: 129.0-129.1 adapted
+// frames/s against 116.3-116.6 with mode 2; a batch-1 weight gradient reduces over few pixels into many outputs, which the
+// CUDA-core kernel's cluster split serves better).  The fused plans need the tensor cores: the fused forward runs when the mode is
+// not 0, the fused backward when it is 2 or more.
+static int g_tc_mode = 3;
+void hmr_set_tc_mode(int mode) { g_tc_mode = mode; }
+int hmr_tc_mode() { return g_tc_mode; }
 
 // table for gn_param_finish: where each GroupNorm's affine gradients live and where its per-sample rows start (the device copy
 // is made by hmr_prepare)
@@ -319,15 +327,9 @@ int hmr_prepare() {
     return DBOA_OK;
 }
 
-// backward convolutions: wgmma implicit GEMM when enabled and the shape is taken, else the fp32 CUDA-core kernels
-static int conv_backward_data(const ConvLayer& c, int B, int groups, unsigned long long active, const float* dy, const float* w, float* dx,
-                              int accumulate, float* ws, cudaStream_t st);
-static int conv_backward_weight(const ConvLayer& c, int B, int groups, unsigned long long active, const float* dy, const float* x, float* dw,
-                                float* ws, cudaStream_t st);
-
 // B samples in `groups` videos of B / groups consecutive samples; video g's weights (and weight gradients) are one arena further on;
 // the videos whose `active` bit is clear are skipped
-static ConvDims dims_of(const ConvLayer& c, int B, int groups, unsigned long long active) {
+static ConvDims dims_of(const ConvLayer& c, int B, int groups = 1, unsigned long long active = ~0ULL) {
     ConvDims d;
     d.B = B / groups; d.groups = groups; d.wstride = net().arena_floats; d.active = active;
     d.Hi = c.hin; d.Wi = c.hin; d.Cin = c.cin; d.Ho = c.hout; d.Wo = c.hout; d.Cout = c.cout;
@@ -335,34 +337,37 @@ static ConvDims dims_of(const ConvLayer& c, int B, int groups, unsigned long lon
     return d;
 }
 
-// conv forward: wgmma implicit GEMM when enabled and the shape is taken (Cin % 64 == 0, Cout % 64 == 0), else the fp32 CUDA-core kernel
-static int conv_forward(const ConvLayer& c, int B, int groups, unsigned long long active, const float* x, const float* w, float* y, float* ws,
+// The choice of kernel for every convolution of the plan: the wgmma kernel when the tensor-core mode selects the product and the
+// kernel takes the shape, else the fp32 CUDA-core kernel (for the stem's weight gradient, its own kernel first).
+static int conv_forward(const ConvLayer& c, int B, int groups, unsigned long long active, const float* x, const float* w, float* y,
                         cudaStream_t st) {
     const ConvDims d = dims_of(c, B, groups, active);
-    if (conv_tc_enabled()) {
+    if (g_tc_mode != 0) {
         int s = conv_tc_fwd(x, w, y, d, st);
         if (s != DBOA_ERR_UNSUPPORTED) return s;
     }
-    return conv_fwd(x, w, y, d, ws, (size_t)kConvWs, st);
+    return conv_fwd(x, w, y, d, st);
 }
-
 static int conv_backward_data(const ConvLayer& c, int B, int groups, unsigned long long active, const float* dy, const float* w, float* dx,
-                              int accumulate, float* ws, cudaStream_t st) {
+                              int accumulate, cudaStream_t st) {
     const ConvDims d = dims_of(c, B, groups, active);
-    if (conv_tc_bwd_enabled()) {
+    if (g_tc_mode >= 2) {
         int s = conv_tc_dgrad(dy, w, dx, d, accumulate, st);
         if (s != DBOA_ERR_UNSUPPORTED) return s;
     }
-    return conv_dgrad(dy, w, dx, d, accumulate, ws, (size_t)kConvWs, st);
+    return conv_dgrad(dy, w, dx, d, accumulate, st);
 }
+// `ws`: the scratch's kConvWs floats, the stem kernel's partials
 static int conv_backward_weight(const ConvLayer& c, int B, int groups, unsigned long long active, const float* dy, const float* x, float* dw,
                                 float* ws, cudaStream_t st) {
     const ConvDims d = dims_of(c, B, groups, active);
-    if (conv_tc_wgrad_enabled()) {
+    if (g_tc_mode == 2) {
         int s = conv_tc_wgrad(dy, x, dw, d, st);
         if (s != DBOA_ERR_UNSUPPORTED) return s;
     }
-    return conv_wgrad(dy, x, dw, d, ws, (size_t)kConvWs, st);
+    const int s = stem_wgrad(dy, x, dw, d, ws, (size_t)kConvWs, st);     // last on the critical path of every backward
+    if (s != DBOA_ERR_UNSUPPORTED) return s;
+    return conv_wgrad(dy, x, dw, d, st);
 }
 
 // Argument checks of a grouped call (host only, before any device access).  Video g owns samples [g * B / groups, (g + 1) * B /
@@ -460,14 +465,14 @@ int hmr_forward(const float* P, const float* init_pose, const float* init_shape,
         return gn_fwd_fused(T + t.conv[ci].y, P + c.g_off, P + c.b_off, res, out, T + t.conv[ci].stats, T + t.conv[ci].part, B, HW,
                             c.cout, relu, st, B / groups, PS);
     };
-    if (g_fused_fwd && conv_tc_enabled())
+    if (g_fused_fwd && g_tc_mode != 0)
         cudaMemsetAsync(T + t.acc, 0, n.convs.size() * (size_t)B * 16 * sizeof(float), st);      // statistics accumulators of this forward
     DBOA_TRY(nchw_to_nhwc(image, T + t.x0, B, 3, 224, 224, st));
-    DBOA_TRY(conv_forward(n.convs[0], B, groups, active, T + t.x0, P + n.convs[0].w_off, T + t.conv[0].y, sc.ws, st));
+    DBOA_TRY(conv_forward(n.convs[0], B, groups, active, T + t.x0, P + n.convs[0].w_off, T + t.conv[0].y, st));
     DBOA_TRY(gn_plain(0, T + t.conv[0].a, 1, nullptr));
     DBOA_TRY(maxpool3x3s2_fwd(T + t.conv[0].a, T + t.p0, reinterpret_cast<unsigned char*>(T + t.p0_idx), B, 112, 112, 64, st));
     const float* x = T + t.p0;
-    if (g_fused_fwd && conv_tc_enabled()) {
+    if (g_fused_fwd && g_tc_mode != 0) {
         // ---- fused plan (conv_tc.cu operand transform): every convolution applies the GroupNorm (+ residual, ReLU) of its operand on
         // load and leaves the statistics of its output as fixed-point sums; one launch per convolution.
         auto acc_of = [&](int ci) { return T + t.acc + (long long)ci * B * 16; };
@@ -521,15 +526,15 @@ int hmr_forward(const float* P, const float* init_pose, const float* init_shape,
     } else {
     for (const Block& b : n.blocks) {
         const ConvLayer &c1 = n.convs[b.c1], &c2 = n.convs[b.c2], &c3 = n.convs[b.c3];
-        DBOA_TRY(conv_forward(c1, B, groups, active, x, P + c1.w_off, T + t.conv[b.c1].y, sc.ws, st));
+        DBOA_TRY(conv_forward(c1, B, groups, active, x, P + c1.w_off, T + t.conv[b.c1].y, st));
         DBOA_TRY(gn_plain(b.c1, T + t.conv[b.c1].a, 1, nullptr));
-        DBOA_TRY(conv_forward(c2, B, groups, active, T + t.conv[b.c1].a, P + c2.w_off, T + t.conv[b.c2].y, sc.ws, st));
+        DBOA_TRY(conv_forward(c2, B, groups, active, T + t.conv[b.c1].a, P + c2.w_off, T + t.conv[b.c2].y, st));
         DBOA_TRY(gn_plain(b.c2, T + t.conv[b.c2].a, 1, nullptr));
-        DBOA_TRY(conv_forward(c3, B, groups, active, T + t.conv[b.c2].a, P + c3.w_off, T + t.conv[b.c3].y, sc.ws, st));
+        DBOA_TRY(conv_forward(c3, B, groups, active, T + t.conv[b.c2].a, P + c3.w_off, T + t.conv[b.c3].y, st));
         const int HW = c3.hout * c3.hout;
         if (b.cd >= 0) {
             const ConvLayer& cd = n.convs[b.cd];
-            DBOA_TRY(conv_forward(cd, B, groups, active, x, P + cd.w_off, T + t.conv[b.cd].y, sc.ws, st));
+            DBOA_TRY(conv_forward(cd, B, groups, active, x, P + cd.w_off, T + t.conv[b.cd].y, st));
             (void)HW;
             DBOA_TRY(gn_plain(b.cd, sc.t1, 0, nullptr));                 // normalised shortcut -> scratch
             DBOA_TRY(gn_plain(b.c3, T + t.conv[b.c3].a, 1, sc.t1));      // relu(gn(y3) + shortcut)
@@ -668,7 +673,7 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
         cudaEventRecord(breq.ev[k], g_join_stream);
         return DBOA_OK;
     };
-    const bool fused = g_fused_bwd && conv_tc_bwd_enabled();
+    const bool fused = g_fused_bwd && g_tc_mode >= 2;
     if (fused) {
         // ---- fused chain (conv_tc.cu, GroupNorm backward on load): per stride-1 layer ONE launch does GroupNorm backward (on load), the data gradient, the
         // shortcut add, the ReLU mask of the producing layer and the sums of ITS GroupNorm backward; the stride-2 layers (conv2
@@ -740,13 +745,13 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
                 const ConvLayer& cd = n.convs[b.cd];
                 DBOA_TRY(gnb(b.cd, dzo, a3, claim(1)));
                 DBOA_TRY(wgrad(cd, 1, xin));
-                DBOA_TRY(conv_backward_data(cd, B, groups, active, tmp[1], P + cd.w_off, dIn, 0, sc.ws, st));
+                DBOA_TRY(conv_backward_data(cd, B, groups, active, tmp[1], P + cd.w_off, dIn, 0, st));
                 DBOA_TRY(gnb(b.c2, tmp[2], T + t.conv[b.c2].a, claim(3)));
                 DBOA_TRY(wgrad(c2, 3, T + t.conv[b.c1].a));
-                DBOA_TRY(conv_backward_data(c2, B, groups, active, tmp[3], P + c2.w_off, claim(4), 0, sc.ws, st));
+                DBOA_TRY(conv_backward_data(c2, B, groups, active, tmp[3], P + c2.w_off, claim(4), 0, st));
                 DBOA_TRY(gnb(b.c1, tmp[4], T + t.conv[b.c1].a, claim(5)));
                 DBOA_TRY(wgrad(c1, 5, xin));
-                DBOA_TRY(conv_backward_data(c1, B, groups, active, tmp[5], P + c1.w_off, dIn, 1, sc.ws, st));
+                DBOA_TRY(conv_backward_data(c1, B, groups, active, tmp[5], P + c1.w_off, dIn, 1, st));
                 const Block& pb = n.blocks[bi - 1];             // seam: the previous block (last of its layer) has an identity shortcut
                 const ConvLayer& p3 = n.convs[pb.c3];
                 DBOA_TRY(gn_bwd_prep(dIn, T + t.conv[pb.c3].a, dIn, prep_of(pb.c3), B, p3.hout * p3.hout, p3.cout, st));
@@ -769,24 +774,24 @@ int hmr_backward(const float* P, const float* T, int B, int masked_in, const flo
             const ConvLayer& cd = n.convs[b.cd];
             DBOA_TRY(gnb(b.cd, dOut, a3, claim(1)));
             DBOA_TRY(wgrad(cd, 1, xin));
-            DBOA_TRY(conv_backward_data(cd, B, groups, active, tmp[1], P + cd.w_off, dIn, 0, sc.ws, st));
+            DBOA_TRY(conv_backward_data(cd, B, groups, active, tmp[1], P + cd.w_off, dIn, 0, st));
         } else {
             DBOA_TRY(relu_mask(dOut, a3, dIn, (size_t)B * c3.hout * c3.hout * c3.cout, st));
         }
-        DBOA_TRY(conv_backward_data(c3, B, groups, active, tmp[0], P + c3.w_off, claim(2), 0, sc.ws, st));
+        DBOA_TRY(conv_backward_data(c3, B, groups, active, tmp[0], P + c3.w_off, claim(2), 0, st));
         DBOA_TRY(gnb(b.c2, tmp[2], T + t.conv[b.c2].a, claim(3)));
         DBOA_TRY(wgrad(c2, 3, T + t.conv[b.c1].a));
-        DBOA_TRY(conv_backward_data(c2, B, groups, active, tmp[3], P + c2.w_off, claim(4), 0, sc.ws, st));
+        DBOA_TRY(conv_backward_data(c2, B, groups, active, tmp[3], P + c2.w_off, claim(4), 0, st));
         DBOA_TRY(gnb(b.c1, tmp[4], T + t.conv[b.c1].a, claim(5)));
         DBOA_TRY(wgrad(c1, 5, xin));
-        DBOA_TRY(conv_backward_data(c1, B, groups, active, tmp[5], P + c1.w_off, dIn, 1, sc.ws, st));
+        DBOA_TRY(conv_backward_data(c1, B, groups, active, tmp[5], P + c1.w_off, dIn, 1, st));
         float* sw = dOut; dOut = dIn; dIn = sw;
     }
     }
     // ---- stem: maxpool, GroupNorm+ReLU, conv (weight gradient only; the image needs none)
     DBOA_TRY(maxpool3x3s2_bwd(dOut, reinterpret_cast<const unsigned char*>(T + t.p0_idx), dIn, B, 112, 112, 64, st));
     DBOA_TRY(gnb(0, dIn, T + t.conv[0].a, claim(0)));
-    int rc = conv_wgrad(tmp[0], T + t.x0, G + n.convs[0].w_off, dims_of(n.convs[0], B, groups, active), sc.ws, (size_t)kConvWs, st);
+    int rc = conv_backward_weight(n.convs[0], B, groups, active, tmp[0], T + t.x0, G + n.convs[0].w_off, sc.ws, st);
     if (rc == DBOA_OK) rc = bucket_done(2, 0);               // stem, layer1, layer2 (and, for B > 1, their GroupNorm affine rows)
     if (async) {                                   // join: nothing of this call is left running when the caller's stream continues
         for (int i = 0; i < BwdAsync::NSIDE; ++i) {

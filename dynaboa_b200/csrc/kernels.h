@@ -17,25 +17,23 @@ struct ConvDims {
     unsigned long long active = ~0ULL;
 };
 
-// ---- conv.cu (fp32 CUDA-core implicit GEMM)
-int conv_fwd(const float* x, const float* w, float* y, const ConvDims& d, float* ws, size_t ws_floats, cudaStream_t st);
-int conv_dgrad(const float* dy, const float* w, float* dx, const ConvDims& d, int accumulate, float* ws, size_t ws_floats, cudaStream_t st);
-int conv_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, float* ws, size_t ws_floats, cudaStream_t st);
+// Which of these kernels computes a convolution product is chosen by the network plan (hmr_plan.cu: conv_forward,
+// conv_backward_data, conv_backward_weight) from the tensor-core mode and the shape; every launcher checks only shapes.
 
-// ---- conv_tc.cu (wgmma TF32x3 implicit GEMM); returns DBOA_ERR_UNSUPPORTED when the shape is not taken
+// ---- conv.cu (fp32 CUDA-core implicit GEMM)
+int conv_fwd(const float* x, const float* w, float* y, const ConvDims& d, cudaStream_t st);
+int conv_dgrad(const float* dy, const float* w, float* dx, const ConvDims& d, int accumulate, cudaStream_t st);
+int conv_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, cudaStream_t st);
+
+// ---- conv_tc.cu (wgmma TF32x3 implicit GEMM); returns DBOA_ERR_UNSUPPORTED when the shape is not taken (Cin % 64, Cout % 64,
+// Kpitch != kh*kw*Cin; data gradient: stride 2 with an odd input extent).  The weight gradient is accumulated (dw +=).
 // `pdl`: launch with programmatic stream serialization.  The forward / data-gradient kernels prefetch WEIGHT tiles before
 // their dependency wait, which is only safe when the preceding kernel in the stream does not write the weights (true inside
 // the network plan; the stand-alone C-ABI wrappers pass false).
 int conv_tc_fwd(const float* x, const float* w, float* y, const ConvDims& d, cudaStream_t st, bool pdl = true);
 int conv_tc_dgrad(const float* dy, const float* w, float* dx, const ConvDims& d, int accumulate, cudaStream_t st, bool pdl = true);
 int conv_tc_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, cudaStream_t st, bool pdl = true);
-bool conv_tc_bwd_enabled();
-bool conv_tc_wgrad_enabled();
 int conv1x1_tc_fwd(const float* x, const float* w, float* y, int M, int Cin, int Cout, cudaStream_t st, bool pdl = true);
-bool conv_tc_enabled();
-void conv_tc_set_mode(int mode);                      // 0 off, 1 forward, 2 forward + dgrad + wgrad, 3 forward + dgrad
-
-int conv_wgrad_tc(const float* dy, const float* x, float* dw, const ConvDims& d, cudaStream_t st);   // any mode; dw +=
 
 // ---- fused convolutions (conv_tc.cu, same kernel with an operand transform on load and sums in the epilogue)
 struct FusedConv {
