@@ -239,11 +239,11 @@ int dboa_groupnorm_bwd(const float* dout, const float* mask_src, const float* y,
     return gn_bwd_fused(dout, mask_src, y, stats, gamma, dy, dgamma, dbeta, partial, B, HW, C, ST(stream));
 }
 int dboa_maxpool_fwd(const float* x, float* y, unsigned char* idx, int B, int H, int W, int C, dboa_stream_t stream) {
-    if (!x || !y || !idx || (H & 1) || (W & 1) || (C & 3)) return DBOA_ERR_ARG;
+    if (!x || !y || !idx) return DBOA_ERR_ARG;
     return maxpool3x3s2_fwd(x, y, idx, B, H, W, C, ST(stream));
 }
 int dboa_maxpool_bwd(const float* dy, const unsigned char* idx, float* dx, int B, int H, int W, int C, dboa_stream_t stream) {
-    if (!dy || !idx || !dx || (H & 1) || (W & 1) || (C & 3)) return DBOA_ERR_ARG;
+    if (!dy || !idx || !dx) return DBOA_ERR_ARG;
     return maxpool3x3s2_bwd(dy, idx, dx, B, H, W, C, ST(stream));
 }
 

@@ -376,11 +376,17 @@ static int launch_z_cluster(K kernel, dim3 grid, cudaStream_t st, Args... args) 
     return launch_ex(kernel, grid, dim3(NT), 0, st, dim3(1, 1, grid.z), true, args...);
 }
 
+// The weight rows of all three products are read or written as float4 at co * Kpitch and padded up to the next k-slab:
+// Kpitch % 4 == 0 and Kpitch >= roundup16(kh * kw * Cin), else DBOA_ERR_SHAPE.
+static bool pitch_ok(const ConvDims& d) {
+    const int K = d.kh * d.kw * d.Cin;
+    return d.Kpitch % 4 == 0 && d.Kpitch >= (K + BK - 1) / BK * BK;
+}
+
 int conv_fwd(const float* x, const float* w, float* y, const ConvDims& d, cudaStream_t st) {
     if (d.groups < 1) return DBOA_ERR_SHAPE;
-    if (d.Cout % BN != 0 || d.Kpitch % 4 != 0) return DBOA_ERR_SHAPE;
+    if (d.Cout % BN != 0 || !pitch_ok(d)) return DBOA_ERR_SHAPE;
     const int M = d.B * d.Ho * d.Wo, K = d.kh * d.kw * d.Cin;
-    if (d.Kpitch < (K + BK - 1) / BK * BK) return DBOA_ERR_SHAPE;
     const int kiters = (K + BK - 1) / BK;
     const int tiles = d.groups * ceil_div(M, BM) * (d.Cout / BN);
     const int ns = pick_split(tiles, kiters);
@@ -393,7 +399,7 @@ int conv_fwd(const float* x, const float* w, float* y, const ConvDims& d, cudaSt
 
 int conv_dgrad(const float* dy, const float* w, float* dx, const ConvDims& d, int accumulate, cudaStream_t st) {
     if (d.groups < 1) return DBOA_ERR_SHAPE;
-    if (d.Cin % BN != 0 || d.Cout % BK != 0) return DBOA_ERR_SHAPE;
+    if (d.Cin % BN != 0 || d.Cout % BK != 0 || !pitch_ok(d)) return DBOA_ERR_SHAPE;
     const int M = d.B * d.Hi * d.Wi, K = d.kh * d.kw * d.Cout;
     const int kiters = K / BK;
     const int tiles = d.groups * ceil_div(M, BM) * (d.Cin / BN);
@@ -404,7 +410,7 @@ int conv_dgrad(const float* dy, const float* w, float* dx, const ConvDims& d, in
 }
 
 int conv_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, cudaStream_t st) {
-    if (d.Cout % BM != 0 || d.groups < 1) return DBOA_ERR_SHAPE;
+    if (d.Cout % BM != 0 || d.groups < 1 || !pitch_ok(d)) return DBOA_ERR_SHAPE;
     const int Mpix = d.B * d.Ho * d.Wo, K = d.kh * d.kw * d.Cin;
     const int piters = ceil_div(Mpix, BK);
     const int tiles = d.groups * (d.Cout / BM) * ceil_div(K, BN);

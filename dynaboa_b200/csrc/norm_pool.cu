@@ -66,7 +66,12 @@ __global__ void maxpool_fwd_kernel(const float* __restrict__ x, float* __restric
     *reinterpret_cast<float4*>(y + o) = make_float4(best[0], best[1], best[2], best[3]);
     *reinterpret_cast<uchar4*>(idx + o) = make_uchar4(bi[0], bi[1], bi[2], bi[3]);
 }
+// The kernels take even H and W (output H/2 x W/2, which is MaxPool2d(3, 2, 1)'s (H + 1) / 2 only for even extents) and whole
+// float4 channel vectors (C % 4 == 0); any other shape is refused rather than computed with a row, a column or channels missing.
+static bool maxpool_shape_ok(int H, int W, int C) { return ((H | W) & 1) == 0 && C % 4 == 0; }
+
 int maxpool3x3s2_fwd(const float* x, float* y, unsigned char* idx, int B, int H, int W, int C, cudaStream_t st) {
+    if (!maxpool_shape_ok(H, W, C)) return DBOA_ERR_SHAPE;
     size_t total = (size_t)B * (H / 2) * (W / 2) * (C / 4);
     return launch_ex(maxpool_fwd_kernel, dim3(ceil_div(total, 256)), dim3(256), 0, st, dim3(1, 1, 1), true, x, y, idx, B, H, W, C);
 }
@@ -106,6 +111,7 @@ __global__ void maxpool_bwd_kernel(const float* __restrict__ dy, const unsigned 
     *reinterpret_cast<float4*>(dx + (((size_t)b * H + hi) * W + wi) * C + cv * 4) = make_float4(acc[0], acc[1], acc[2], acc[3]);
 }
 int maxpool3x3s2_bwd(const float* dy, const unsigned char* idx, float* dx, int B, int H, int W, int C, cudaStream_t st) {
+    if (!maxpool_shape_ok(H, W, C)) return DBOA_ERR_SHAPE;
     size_t total = (size_t)B * H * W * (C / 4);
     return launch_ex(maxpool_bwd_kernel, dim3(ceil_div(total, 256)), dim3(256), 0, st, dim3(1, 1, 1), true, dy, idx, dx, B, H, W, C);
 }

@@ -109,9 +109,12 @@ __global__ void __launch_bounds__(256) stem_wgrad_reduce_kernel(const float* __r
 
 }  // namespace stem
 
+// The reduction's scalar stores would take any Kpitch >= 147; the stem shape is held to the pitch rule of the general weight
+// gradient (conv.cu: Kpitch % 4 == 0, Kpitch >= roundup16(K) = 160), so the weight-gradient entry point has one rule whichever
+// kernel serves it.
 bool stem_wgrad_ok(const ConvDims& d) {
     return d.Cin == 3 && d.Cout == stem::CO && d.kh == 7 && d.kw == 7 && d.stride == 2 && d.pad == 3 && d.Hi == stem::HI && d.Wi == stem::HI &&
-           d.Ho == stem::HO && d.Wo == stem::HO && d.Kpitch >= stem::KK;
+           d.Ho == stem::HO && d.Wo == stem::HO && d.Kpitch % 4 == 0 && d.Kpitch >= (stem::KK + 15) / 16 * 16;
 }
 
 int stem_wgrad(const float* dy, const float* x, float* dw, const ConvDims& d, float* ws, size_t ws_floats, cudaStream_t st) {

@@ -136,7 +136,11 @@ int dboa_hmr_backward_buckets(void* ev0, void* ev1, void* ev2);
 long long dboa_hmr_bucket_offset(int k);
 
 /* ---- single operators (unit-parity surface; same kernels the plan above launches) ----------- */
-/* replaces: nn.Conv2d forward / backward (model/hmr.py:29-34,72,113); NHWC activations, weights [Cout][Kpitch] */
+/* replaces: nn.Conv2d forward / backward (model/hmr.py:29-34,72,113); NHWC activations, weights [Cout][Kpitch].
+ * All three take Kpitch % 4 == 0 and Kpitch >= roundup16(k*k*Cin) (the weight rows are read / written as float4 up to the
+ * next 16-element slab; the columns past k*k*Cin are zero padding the weight gradient leaves untouched), else DBOA_ERR_SHAPE;
+ * the weight gradient of the 7x7 stem given a workspace (a kernel of its own) is held to the same rule.
+ * forward: Cout % 64 == 0; data gradient: Cin % 64 == 0, Cout % 16 == 0; weight gradient: Cout % 64 == 0, dw accumulated (+=). */
 int dboa_conv2d_fwd(const float* x, const float* w, float* y, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad,
                     int Kpitch, float* ws, long long ws_floats, dboa_stream_t stream);
 int dboa_conv2d_dgrad(const float* dy, const float* w, float* dx, int B, int Hi, int Wi, int Cin, int Cout, int k, int stride, int pad,
@@ -210,8 +214,13 @@ long long dboa_gn_partial_floats(int B, int HW, int C);
 long long dboa_gn_bwd_partial_floats(int B, int HW, int C);
 int dboa_groupnorm_fwd(const float* y, const float* gamma, const float* beta, const float* residual, float* out, float* stats,
                        float* partial, int B, int HW, int C, int relu, dboa_stream_t stream);
+/* dgamma / dbeta are accumulated (+=).  With B > 1 the last cluster to finish sums the per-sample rows in sample order; it
+ * is found through ticket counters the library holds once per process, so two such calls must not run concurrently (on
+ * two streams): calls ordered on one stream are fine. */
 int dboa_groupnorm_bwd(const float* dout, const float* mask_src, const float* y, const float* stats, const float* gamma, float* dy,
                        float* dgamma, float* dbeta, float* partial, int B, int HW, int C, dboa_stream_t stream);
+/* replaces: nn.MaxPool2d(3, 2, 1) (model/hmr.py:75) on NHWC; idx holds each output's window position r * 3 + s (first maximum
+ * in scan order, NaN propagates).  H and W even (output H/2 x W/2) and C % 4 == 0, else DBOA_ERR_SHAPE. */
 int dboa_maxpool_fwd(const float* x, float* y, unsigned char* idx, int B, int H, int W, int C, dboa_stream_t stream);
 int dboa_maxpool_bwd(const float* dy, const unsigned char* idx, float* dx, int B, int H, int W, int C, dboa_stream_t stream);
 

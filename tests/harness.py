@@ -1,7 +1,8 @@
 """Scaffolding shared by the test modules and the timing scripts.  A plain module, not a test module: pytest does not collect it,
 and no test module imports another.
 
-- Helpers: ``bits``, ``fetch``, ``stream``, ``golden_options`` and its presets, ``state``.
+- Helpers: ``bits``, ``same_bits``, ``fetch``, ``stream``, ``golden_options`` and its presets, ``state``.
+- Guard-banded device buffers: ``Buf`` (an output starts as NaN, its tail of ``GUARD`` ``SENTINEL`` elements must survive).
 - The device-free ABI tests: ``built_lib``, the stand-in pointer ``FAKE``, the ``ERR_*`` codes, ``cpu_options`` and ``idle_pool``.
 - The per-video pool runs: ``video_masks`` / ``video_seed`` and the golden-aware ``masks_for`` / ``seed_for``, ``PoolRun`` (a
   MultiVideoAdaptor whose slots carry videos) and ``SingleRun`` (the same video through the single-video ``Adaptor.adapt``).
@@ -32,6 +33,47 @@ def bits(t):
     if t.dtype == torch.float64:
         return t.view(torch.int64)
     return t.view(torch.int32) if t.dtype == torch.float32 else t
+
+
+def same_bits(a, b):
+    """a and b have the same dtype, shape and bits (NaN payloads included); b may live on another device."""
+    a, b = a.contiguous(), b.to(a.device).contiguous()
+    if a.dtype != b.dtype or a.shape != b.shape:
+        return False
+    return torch.equal(bits(a), bits(b))
+
+
+# ------------------------------------------------------------------ guard-banded device buffers
+GUARD = 64
+SENTINEL = {torch.float32: -1.2345678e33, torch.float64: -1.25e300, torch.int32: 0x5A5A5A5A, torch.uint8: 0xA5}
+UNSET = {torch.int32: -7, torch.uint8: 0xEE}            # the fill of an output buffer of an integer type (floats: NaN)
+
+
+class Buf:
+    """A device buffer of n elements (``x``'s values, else NaN / UNSET) followed by GUARD sentinel elements."""
+
+    def __init__(self, x=None, n=None, dtype=torch.float32):
+        if x is not None:
+            dtype, n = x.dtype, x.numel()
+        self.n, self.dtype = n, dtype
+        self.whole = torch.empty(n + GUARD, dtype=dtype, device='cuda')
+        self.whole[n:] = SENTINEL[dtype]
+        self.t = self.whole[:n]
+        if x is not None:
+            self.t.copy_(x.reshape(-1))
+        else:
+            self.t.fill_(UNSET.get(dtype, float('nan')))
+
+    @property
+    def ptr(self):
+        return ctypes.c_void_p(self.t.data_ptr())
+
+    def cpu(self):
+        return self.t.cpu()
+
+    def intact(self):
+        tail = self.whole[self.n:].cpu()
+        return same_bits(tail, torch.full_like(tail, SENTINEL[self.dtype]))
 
 
 def fetch(batch):

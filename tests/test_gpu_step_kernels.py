@@ -21,10 +21,8 @@ import numpy as np
 import pytest
 import torch
 
-from harness import COS_TOL, TERMS_TOL, adam_ref, ema_ref, f32, sgd_ref
+from harness import COS_TOL, TERMS_TOL, Buf, adam_ref, ema_ref, f32, same_bits, sgd_ref
 
-GUARD = 64
-SENTINEL = {torch.float32: -1.2345678e33, torch.float64: -1.25e300, torch.int32: 0x5A5A5A5A}
 U32 = 2.0 ** -24                                   # unit roundoff of fp32
 OK, ERR_ARG, ERR_SHAPE = 0, -1, -2
 THRESHOLD = 3.1e-4                                 # bench.py's cos_sim_threshold
@@ -35,41 +33,6 @@ def L():
     from dynaboa_b200 import _lib
     _lib.load()
     return _lib
-
-
-class Buf:
-    """A device buffer of n elements (``x``'s values, else NaN / -7) followed by GUARD sentinel elements."""
-
-    def __init__(self, x=None, n=None, dtype=torch.float32):
-        if x is not None:
-            dtype, n = x.dtype, x.numel()
-        self.n, self.dtype = n, dtype
-        self.whole = torch.empty(n + GUARD, dtype=dtype, device='cuda')
-        self.whole[n:] = SENTINEL[dtype]
-        self.t = self.whole[:n]
-        if x is not None:
-            self.t.copy_(x.reshape(-1))
-        else:
-            self.t.fill_(-7 if dtype == torch.int32 else float('nan'))
-
-    @property
-    def ptr(self):
-        return C.c_void_p(self.t.data_ptr())
-
-    def cpu(self):
-        return self.t.cpu()
-
-    def intact(self):
-        tail = self.whole[self.n:].cpu()
-        return same_bits(tail, torch.full_like(tail, SENTINEL[self.dtype]))
-
-
-def same_bits(a, b):
-    a, b = a.contiguous(), b.to(a.device).contiguous()
-    if a.dtype != b.dtype or a.shape != b.shape:
-        return False
-    view = {torch.float32: torch.int32, torch.float64: torch.int64}.get(a.dtype, a.dtype)
-    return torch.equal(a.view(view), b.view(view))
 
 
 def num_sms():
