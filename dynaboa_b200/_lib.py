@@ -109,7 +109,12 @@ SIGNATURES = {
     'dboa_loss_motion_joints': (I, [P, P, P, P, F, P, P, P, I, I, I, I, P]),
     'dboa_loss_motion_groups': (I, [P, P, P, P, F, P, P, P, I, I, I, I, I, P]),
     'dboa_loss_motion_active': (I, [P, P, P, P, F, P, P, P, I, I, I, I, I, C.c_ulonglong, P]),
+    'dboa_pose_prior_groups': (I, [P, P, P, P, P, P, C.POINTER(F), I, I, P]),
+    'dboa_loss_multi_weights': (I, [C.POINTER(LossArgsStruct), C.POINTER(F), P]),
+    'dboa_loss_motion_weights': (I, [P, P, P, P, C.POINTER(F), P, P, P, I, I, I, I, I, C.c_ulonglong, P]),
     'dboa_sgd_update': (I, [P, P, P, F, L, P]),
+    'dboa_sgd_update_groups': (I, [P, P, P, C.POINTER(F), L, I, C.c_ulonglong, P]),
+    'dboa_adam_ema_groups': (I, [P, P, P, P, P, L, C.POINTER(F), I, C.c_ulonglong, P]),
     'dboa_adam_ema': (I, [P, P, P, P, P, L, D, D, D, D, I, D, P]),
     'dboa_ema_update': (I, [P, P, L, D, P]),
     'dboa_adam_ema_scaled': (I, [P, P, P, P, P, L, D, D, D, D, I, D, F, P]),

@@ -334,6 +334,28 @@ int dboa_loss_motion_active(const float* p_cur, const float* p_hist, const float
     return loss_motion_launch(p_cur, p_hist, kp_cur, kp_hist, weight, term, dp_cur, dp_hist, B, accumulate_cur, first, count, ST(stream),
                               groups, active);
 }
+// the checks every per-video entry point makes on its `active` mask: none empty, no bit at position >= groups
+static bool bad_mask(int groups, unsigned long long active) { return active == 0 || (groups < 64 && (active >> groups) != 0); }
+int dboa_pose_prior_groups(const float* rotmat, const float* means, const float* precisions, const float* neg_log_w, float* prior_b,
+                           float* d_rotmat, const float* scale, int B, int groups, dboa_stream_t stream) {
+    if (!rotmat || !means || !precisions || !neg_log_w || !prior_b || !scale) return DBOA_ERR_ARG;
+    if (groups < 1 || groups > MAX_VIDEOS || B < 1 || B % groups != 0) return DBOA_ERR_SHAPE;
+    return pose_prior_groups_launch(rotmat, means, precisions, neg_log_w, prior_b, d_rotmat, scale, B, groups, ST(stream));
+}
+int dboa_loss_multi_weights(const dboa_loss_args* a, const float* w, dboa_stream_t stream) {
+    if (!a || !w || !a->p2d || !a->j3d || !a->R || !a->beta || !a->terms) return DBOA_ERR_ARG;
+    if (a->gt_s3d && !a->kp) return DBOA_ERR_ARG;
+    return loss_multi_weights_launch(*a, w, ST(stream));
+}
+int dboa_loss_motion_weights(const float* p_cur, const float* p_hist, const float* kp_cur, const float* kp_hist, const float* weight,
+                             float* term, float* dp_cur, float* dp_hist, int B, int accumulate_cur, int first, int count, int groups,
+                             unsigned long long active, dboa_stream_t stream) {
+    if (!p_cur || !p_hist || !kp_cur || !kp_hist || !weight || !term || !dp_cur || !dp_hist || B < 1) return DBOA_ERR_ARG;
+    if (groups < 1 || groups > MAX_VIDEOS || B % groups != 0) return DBOA_ERR_SHAPE;
+    if (bad_mask(groups, active)) return DBOA_ERR_ARG;
+    return loss_motion_weights_launch(p_cur, p_hist, kp_cur, kp_hist, weight, term, dp_cur, dp_hist, B, accumulate_cur, first, count,
+                                      ST(stream), groups, active);
+}
 
 int dboa_sgd_update(const float* p, const float* g, float* out, float lr, long long n, dboa_stream_t stream) {
     if (!p || !g || !out || n < 0) return DBOA_ERR_ARG;
@@ -357,6 +379,20 @@ int dboa_adam_scalars(float* out, double lr, double beta1, double beta2, double 
 int dboa_adam_ema_dev(float* p, const float* g, float* m, float* v, float* teacher, long long n, const float* scalars, dboa_stream_t stream) {
     if (!p || !g || !m || !v || !scalars || n < 0) return DBOA_ERR_ARG;
     return adam_ema_dev(p, g, m, v, teacher, (size_t)n, scalars, ST(stream));
+}
+int dboa_sgd_update_groups(const float* p, const float* g, float* out, const float* lr, long long n, int groups, unsigned long long active,
+                           dboa_stream_t stream) {
+    if (!p || !g || !out || !lr || n < 0) return DBOA_ERR_ARG;
+    if (groups < 1 || groups > MAX_VIDEOS || n % 4 != 0) return DBOA_ERR_SHAPE;
+    if (bad_mask(groups, active)) return DBOA_ERR_ARG;
+    return sgd_update_groups(p, g, out, lr, (size_t)n, groups, active, ST(stream));
+}
+int dboa_adam_ema_groups(float* p, const float* g, float* m, float* v, float* teacher, long long n, const float* scalars, int groups,
+                         unsigned long long active, dboa_stream_t stream) {
+    if (!p || !g || !m || !v || !scalars || n < 0) return DBOA_ERR_ARG;
+    if (groups < 1 || groups > MAX_VIDEOS || n % 4 != 0) return DBOA_ERR_SHAPE;
+    if (bad_mask(groups, active)) return DBOA_ERR_ARG;
+    return adam_ema_groups(p, g, m, v, teacher, (size_t)n, scalars, groups, active, ST(stream));
 }
 int dboa_fill_zero(void* dst, long long bytes, dboa_stream_t stream) {
     if (!dst || bytes < 0) return DBOA_ERR_ARG;

@@ -22,6 +22,8 @@ inline int check_launch() {
 }
 
 #define DBOA_TRY(expr) do { int _s = (expr); if (_s != DBOA_OK) return _s; } while (0)
+// the most videos one grouped call takes (the bits of an `active` mask)
+constexpr int MAX_VIDEOS = 64;
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -58,9 +58,9 @@ int project_bwd_launch(const float* cam, const float* j3d, const float* dp2d, fl
 // FROM_ROT: input is the (24,3,3) rotation stack, gradient goes to d_rot (B,24,3,3)
 // otherwise : input is the 69-d axis-angle body pose, gradient goes to d_in (B,69)
 template <bool FROM_ROT>
-__global__ void __launch_bounds__(256) pose_prior_kernel(const float* __restrict__ in, const float* __restrict__ means,
-                                                         const float* __restrict__ prec, const float* __restrict__ neg_log_w,
-                                                         float* __restrict__ prior_b, float* __restrict__ d_in, float scale) {
+__device__ __forceinline__ void pose_prior_body(const float* __restrict__ in, const float* __restrict__ means, const float* __restrict__ prec,
+                                                const float* __restrict__ neg_log_w, float* __restrict__ prior_b, float* __restrict__ d_in,
+                                                float scale) {
     pdl_wait();
     pdl_trigger();
     __shared__ float sx[69], sd[8][69], sPd[8][69], sg[8][69], sll[8];
@@ -139,9 +139,30 @@ __global__ void __launch_bounds__(256) pose_prior_kernel(const float* __restrict
         }
     }
 }
+template <bool FROM_ROT>
+__global__ void __launch_bounds__(256) pose_prior_kernel(const float* __restrict__ in, const float* __restrict__ means,
+                                                         const float* __restrict__ prec, const float* __restrict__ neg_log_w,
+                                                         float* __restrict__ prior_b, float* __restrict__ d_in, float scale) {
+    pose_prior_body<FROM_ROT>(in, means, prec, neg_log_w, prior_b, d_in, scale);
+}
+// per-video scale: body b belongs to video b / rows and scales its gradient by t.scale[video]
+struct VideoScales { float scale[MAX_VIDEOS]; };
+__global__ void __launch_bounds__(256) pose_prior_groups_kernel(const float* __restrict__ in, const float* __restrict__ means,
+                                                                const float* __restrict__ prec, const float* __restrict__ neg_log_w,
+                                                                float* __restrict__ prior_b, float* __restrict__ d_in, int rows,
+                                                                const VideoScales t) {
+    pose_prior_body<true>(in, means, prec, neg_log_w, prior_b, d_in, t.scale[blockIdx.x / rows]);
+}
 int pose_prior_launch(const float* rot, const float* means, const float* prec, const float* neg_log_w, float* prior_b, float* drot,
                       float scale, int B, cudaStream_t st) {
     return launch_ex(pose_prior_kernel<true>, dim3(B), dim3(256), 0, st, dim3(1, 1, 1), true, rot, means, prec, neg_log_w, prior_b, drot, scale);
+}
+int pose_prior_groups_launch(const float* rot, const float* means, const float* prec, const float* neg_log_w, float* prior_b, float* drot,
+                             const float* scale, int B, int groups, cudaStream_t st) {
+    VideoScales t;
+    for (int g = 0; g < groups; ++g) t.scale[g] = scale[g];
+    return launch_ex(pose_prior_groups_kernel, dim3(B), dim3(256), 0, st, dim3(1, 1, 1), true, rot, means, prec, neg_log_w, prior_b, drot,
+                     B / groups, t);
 }
 int gmm_prior_launch(const float* pose69, const float* means, const float* prec, const float* neg_log_w, float* prior_b, float* dpose,
                      float scale, int B, cudaStream_t st) {
@@ -154,7 +175,9 @@ int gmm_prior_launch(const float* pose69, const float* means, const float* prec,
 //        3 target p2d MSE  4 target j3d MSE  5 target beta MSE  6 target R MSE  7 hip-centred 3D
 // ---------------------------------------------------------------------------------------------
 // grouped (a.groups > 1): block g computes video g's terms on its own rows
-__global__ void __launch_bounds__(256) loss_multi_kernel(LossArgs a) {
+// w(k): weight k of the block's video
+template <class W>
+__device__ __forceinline__ void loss_multi_body(LossArgs& a, const W& w) {
     pdl_wait();
     pdl_trigger();
     __shared__ float red[32];
@@ -182,12 +205,12 @@ __global__ void __launch_bounds__(256) loss_multi_kernel(LossArgs a) {
             const float k = a.kp[(size_t)(b * 49 + j) * 3 + (i & 1)];
             const float d = p - k;
             acc[0] += d * d * conf;
-            g += a.w[0] * 2.0f * conf * d / (float)(B * kn * 2);
+            g += w(0) * 2.0f * conf * d / (float)(B * kn * 2);
         }
         if (a.t_p2d != nullptr) {
             const float d = p - a.t_p2d[i];
             acc[3] += d * d;
-            g += a.w[3] * 2.0f * d / (float)(B * 98);
+            g += w(3) * 2.0f * d / (float)(B * 98);
         }
         if (a.dp2d != nullptr) a.dp2d[i] = g;
     }
@@ -197,7 +220,7 @@ __global__ void __launch_bounds__(256) loss_multi_kernel(LossArgs a) {
         if (a.t_j3d != nullptr) {
             const float d = a.j3d[i] - a.t_j3d[i];
             acc[4] += d * d;
-            g = a.w[4] * 2.0f * d / (float)(B * 147);
+            g = w(4) * 2.0f * d / (float)(B * 147);
         }
         if (a.dj3d != nullptr) a.dj3d[i] = g;
     }
@@ -205,11 +228,11 @@ __global__ void __launch_bounds__(256) loss_multi_kernel(LossArgs a) {
     for (int i = t; i < B * 10; i += 256) {
         const float be = a.beta[i];
         acc[1] += be * be;
-        float g = a.w[1] * 2.0f * be / (float)B;
+        float g = w(1) * 2.0f * be / (float)B;
         if (a.t_beta != nullptr) {
             const float d = be - a.t_beta[i];
             acc[5] += d * d;
-            g += a.w[5] * 2.0f * d / (float)(B * 10);
+            g += w(5) * 2.0f * d / (float)(B * 10);
         }
         if (a.dbeta != nullptr) a.dbeta[i] = g;
     }
@@ -219,7 +242,7 @@ __global__ void __launch_bounds__(256) loss_multi_kernel(LossArgs a) {
         if (a.t_R != nullptr) {
             const float d = a.R[i] - a.t_R[i];
             acc[6] += d * d;
-            g = a.w[6] * 2.0f * d / (float)(B * 216);
+            g = w(6) * 2.0f * d / (float)(B * 216);
         }
         if (a.dR != nullptr) a.dR[i] = a.dR_accumulate ? a.dR[i] + g : g;
     }
@@ -231,7 +254,7 @@ __global__ void __launch_bounds__(256) loss_multi_kernel(LossArgs a) {
         const float* gj = a.gt_s3d + (size_t)b * 96;
         float ph[3], gh[3], sum_e[3] = {0.f, 0.f, 0.f};
         for (int k = 0; k < 3; ++k) { ph[k] = (pj[2 * 3 + k] + pj[3 * 3 + k]) / 2.0f; gh[k] = (gj[2 * 4 + k] + gj[3 * 4 + k]) / 2.0f; }
-        const float gs = a.w[7] * 2.0f / (float)(B * 72);
+        const float gs = w(7) * 2.0f / (float)(B * 72);
         for (int j = 0; j < 24; ++j) {
             const float conf = a.kp[(size_t)(b * 49 + 25 + j) * 3 + 2];
             for (int k = 0; k < 3; ++k) {
@@ -262,15 +285,38 @@ __global__ void __launch_bounds__(256) loss_multi_kernel(LossArgs a) {
             sterm[2] = s / (float)B;
         } else sterm[2] = 0.f;
         float total = 0.f;
-        for (int k = 0; k < 8; ++k) { a.terms[k] = sterm[k]; total += a.w[k] * sterm[k]; }
+        for (int k = 0; k < 8; ++k) { a.terms[k] = sterm[k]; total += w(k) * sterm[k]; }
         a.terms[8] = total;
     }
 }
-int loss_multi_launch(const LossArgs& a, cudaStream_t st) {
+__global__ void __launch_bounds__(256) loss_multi_kernel(LossArgs a) {
+    loss_multi_body(a, [&](int k) { return a.w[k]; });
+}
+// per-video weights: block g reads t.w[g] in place of a.w.  With __launch_bounds__(256) alone ptxas spills here (sm_90a, CUDA
+// 12.9: 79 registers, 8 bytes stack frame, 8 bytes spill stores); with a minimum of one block per SM it keeps every value in
+// registers (84 registers, no stack frame).  One block per video never needs more residency than that.
+struct VideoWeights { float w[MAX_VIDEOS][8]; };
+__global__ void __launch_bounds__(256, 1) loss_multi_weights_kernel(LossArgs a, const VideoWeights t) {
+    loss_multi_body(a, [&](int k) { return t.w[blockIdx.x][k]; });
+}
+static int loss_multi_check(const LossArgs& a) {
     const int groups = a.groups > 1 ? a.groups : 1;
     if (a.B < 1 || a.B > 256 * groups || a.groups < 0 || a.B % groups != 0) return DBOA_ERR_SHAPE;
     if (a.kp_count < 0 || a.kp_first < 0 || a.kp_first + a.kp_count > 49) return DBOA_ERR_ARG;
-    return launch_ex(loss_multi_kernel, dim3(groups), dim3(256), 0, st, dim3(1, 1, 1), true, a);
+    return DBOA_OK;
+}
+int loss_multi_launch(const LossArgs& a, cudaStream_t st) {
+    DBOA_TRY(loss_multi_check(a));
+    return launch_ex(loss_multi_kernel, dim3(a.groups > 1 ? a.groups : 1), dim3(256), 0, st, dim3(1, 1, 1), true, a);
+}
+int loss_multi_weights_launch(const LossArgs& a, const float* w, cudaStream_t st) {
+    const int groups = a.groups > 1 ? a.groups : 1;
+    if (groups > MAX_VIDEOS) return DBOA_ERR_SHAPE;
+    DBOA_TRY(loss_multi_check(a));
+    VideoWeights t;
+    for (int g = 0; g < groups; ++g)
+        for (int k = 0; k < 8; ++k) t.w[g][k] = w[g * 8 + k];
+    return launch_ex(loss_multi_weights_kernel, dim3(groups), dim3(256), 0, st, dim3(1, 1, 1), true, a, t);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -278,10 +324,9 @@ int loss_multi_launch(const LossArgs& a, cudaStream_t st) {
 //   L = mean_{B*count*2} [conf_a + conf_h == 2] * ((pa - ph) - (ka - kh))^2   on joints [first, first + count)  (benchmark: 25..48)
 // A video whose `active` bit is clear gets term 0 and leaves its rows of dpa and dph untouched.
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) loss_motion_kernel(const float* __restrict__ pa, const float* __restrict__ ph,
-                                                          const float* __restrict__ ka, const float* __restrict__ kh, float w,
-                                                          float* __restrict__ term, float* __restrict__ dpa, float* __restrict__ dph,
-                                                          int B, int acc_a, int first, int count, unsigned long long active) {
+__device__ __forceinline__ void loss_motion_body(const float* __restrict__ pa, const float* __restrict__ ph, const float* __restrict__ ka,
+                                                 const float* __restrict__ kh, float w, float* __restrict__ term, float* __restrict__ dpa,
+                                                 float* __restrict__ dph, int B, int acc_a, int first, int count, unsigned long long active) {
     pdl_wait();
     pdl_trigger();
     __shared__ float red[32];
@@ -311,6 +356,29 @@ __global__ void __launch_bounds__(256) loss_motion_kernel(const float* __restric
     }
     acc = block_sum(acc, red);
     if (threadIdx.x == 0) term[0] = acc / n;
+}
+__global__ void __launch_bounds__(256) loss_motion_kernel(const float* __restrict__ pa, const float* __restrict__ ph,
+                                                          const float* __restrict__ ka, const float* __restrict__ kh, float w,
+                                                          float* __restrict__ term, float* __restrict__ dpa, float* __restrict__ dph,
+                                                          int B, int acc_a, int first, int count, unsigned long long active) {
+    loss_motion_body(pa, ph, ka, kh, w, term, dpa, dph, B, acc_a, first, count, active);
+}
+// per-video weight: block g weighs its gradient with t.scale[g]
+__global__ void __launch_bounds__(256) loss_motion_weights_kernel(const float* __restrict__ pa, const float* __restrict__ ph,
+                                                                  const float* __restrict__ ka, const float* __restrict__ kh,
+                                                                  float* __restrict__ term, float* __restrict__ dpa, float* __restrict__ dph,
+                                                                  int B, int acc_a, int first, int count, unsigned long long active,
+                                                                  const VideoScales t) {
+    loss_motion_body(pa, ph, ka, kh, t.scale[blockIdx.x], term, dpa, dph, B, acc_a, first, count, active);
+}
+int loss_motion_weights_launch(const float* pa, const float* ph, const float* ka, const float* kh, const float* w, float* term, float* dpa,
+                               float* dph, int B, int acc_a, int first, int count, cudaStream_t st, int groups, unsigned long long active) {
+    if (first < 0 || count < 1 || first + count > 49) return DBOA_ERR_ARG;
+    if (groups < 1 || groups > MAX_VIDEOS || B % groups != 0) return DBOA_ERR_SHAPE;
+    VideoScales t;
+    for (int g = 0; g < groups; ++g) t.scale[g] = w[g];
+    return launch_ex(loss_motion_weights_kernel, dim3(groups), dim3(256), 0, st, dim3(1, 1, 1), true, pa, ph, ka, kh, term, dpa, dph, B, acc_a,
+                     first, count, active, t);
 }
 int loss_motion_launch(const float* pa, const float* ph, const float* ka, const float* kh, float w, float* term, float* dpa, float* dph,
                        int B, int acc_a, int first, int count, cudaStream_t st, int groups, unsigned long long active) {

@@ -18,14 +18,16 @@ static inline int sweep_grid(size_t n4) {
     return (int)(blocks < cap ? (blocks ? blocks : 1) : cap);
 }
 
+// float4 i of one SGD step, shared by the one-arena and the per-video kernels
+__device__ __forceinline__ void sgd_at(const float* __restrict__ p, const float* __restrict__ g, float* __restrict__ out, float neg_lr, size_t i) {
+    float4 a = reinterpret_cast<const float4*>(p)[i], b = reinterpret_cast<const float4*>(g)[i], o;
+    o.x = __fadd_rn(a.x, __fmul_rn(neg_lr, b.x)); o.y = __fadd_rn(a.y, __fmul_rn(neg_lr, b.y));
+    o.z = __fadd_rn(a.z, __fmul_rn(neg_lr, b.z)); o.w = __fadd_rn(a.w, __fmul_rn(neg_lr, b.w));
+    reinterpret_cast<float4*>(out)[i] = o;
+}
 __global__ void __launch_bounds__(256) sgd_update_kernel(const float* __restrict__ p, const float* __restrict__ g, float* __restrict__ out,
                                                          float neg_lr, size_t n4) {
-    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n4; i += (size_t)gridDim.x * 256) {
-        float4 a = reinterpret_cast<const float4*>(p)[i], b = reinterpret_cast<const float4*>(g)[i], o;
-        o.x = __fadd_rn(a.x, __fmul_rn(neg_lr, b.x)); o.y = __fadd_rn(a.y, __fmul_rn(neg_lr, b.y));
-        o.z = __fadd_rn(a.z, __fmul_rn(neg_lr, b.z)); o.w = __fadd_rn(a.w, __fmul_rn(neg_lr, b.w));
-        reinterpret_cast<float4*>(out)[i] = o;
-    }
+    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n4; i += (size_t)gridDim.x * 256) sgd_at(p, g, out, neg_lr, i);
 }
 int sgd_update(const float* p, const float* g, float* out, float lr, size_t n, cudaStream_t st) {
     if (n % 4) return DBOA_ERR_SHAPE;
@@ -44,29 +46,34 @@ __device__ __forceinline__ void adam_one(float& p, float g, float& m, float& v, 
     p = __fadd_rn(p, __fmul_rn(neg_step, __fdiv_rn(m, denom)));
 }
 
-// one grid-stride Adam (+ EMA) sweep; the two kernels below differ only in where they read their scalars from
+// float4 i of one Adam (+ EMA) step, shared by the sweeps below, which differ only in where they read their scalars from
+__device__ __forceinline__ void adam_ema_at(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+                                            float* __restrict__ teacher, size_t i, float w1, float b2, float one_m_b2, float bc2_sqrt,
+                                            float eps, float neg_step, float alpha, float one_m_alpha, float gscale) {
+    float4 pp = reinterpret_cast<float4*>(p)[i], gg = reinterpret_cast<const float4*>(g)[i];
+    float4 mm = reinterpret_cast<float4*>(m)[i], vv = reinterpret_cast<float4*>(v)[i];
+    // data-parallel mean of the all-reduced (summed) gradient: g / R folded into this sweep (1.0f is exact: single-GPU results unchanged)
+    gg.x = __fmul_rn(gg.x, gscale); gg.y = __fmul_rn(gg.y, gscale); gg.z = __fmul_rn(gg.z, gscale); gg.w = __fmul_rn(gg.w, gscale);
+    adam_one(pp.x, gg.x, mm.x, vv.x, w1, b2, one_m_b2, bc2_sqrt, eps, neg_step);
+    adam_one(pp.y, gg.y, mm.y, vv.y, w1, b2, one_m_b2, bc2_sqrt, eps, neg_step);
+    adam_one(pp.z, gg.z, mm.z, vv.z, w1, b2, one_m_b2, bc2_sqrt, eps, neg_step);
+    adam_one(pp.w, gg.w, mm.w, vv.w, w1, b2, one_m_b2, bc2_sqrt, eps, neg_step);
+    reinterpret_cast<float4*>(p)[i] = pp; reinterpret_cast<float4*>(m)[i] = mm; reinterpret_cast<float4*>(v)[i] = vv;
+    if (teacher != nullptr) {
+        float4 tt = reinterpret_cast<float4*>(teacher)[i];
+        tt.x = __fadd_rn(__fmul_rn(tt.x, alpha), __fmul_rn(one_m_alpha, pp.x));
+        tt.y = __fadd_rn(__fmul_rn(tt.y, alpha), __fmul_rn(one_m_alpha, pp.y));
+        tt.z = __fadd_rn(__fmul_rn(tt.z, alpha), __fmul_rn(one_m_alpha, pp.z));
+        tt.w = __fadd_rn(__fmul_rn(tt.w, alpha), __fmul_rn(one_m_alpha, pp.w));
+        reinterpret_cast<float4*>(teacher)[i] = tt;
+    }
+}
+// one grid-stride Adam (+ EMA) sweep over one arena
 __device__ __forceinline__ void adam_ema_sweep(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
                                                float* __restrict__ teacher, size_t n4, float w1, float b2, float one_m_b2, float bc2_sqrt,
                                                float eps, float neg_step, float alpha, float one_m_alpha, float gscale) {
-    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n4; i += (size_t)gridDim.x * 256) {
-        float4 pp = reinterpret_cast<float4*>(p)[i], gg = reinterpret_cast<const float4*>(g)[i];
-        float4 mm = reinterpret_cast<float4*>(m)[i], vv = reinterpret_cast<float4*>(v)[i];
-        // data-parallel mean of the all-reduced (summed) gradient: g / R folded into this sweep (1.0f is exact: single-GPU results unchanged)
-        gg.x = __fmul_rn(gg.x, gscale); gg.y = __fmul_rn(gg.y, gscale); gg.z = __fmul_rn(gg.z, gscale); gg.w = __fmul_rn(gg.w, gscale);
-        adam_one(pp.x, gg.x, mm.x, vv.x, w1, b2, one_m_b2, bc2_sqrt, eps, neg_step);
-        adam_one(pp.y, gg.y, mm.y, vv.y, w1, b2, one_m_b2, bc2_sqrt, eps, neg_step);
-        adam_one(pp.z, gg.z, mm.z, vv.z, w1, b2, one_m_b2, bc2_sqrt, eps, neg_step);
-        adam_one(pp.w, gg.w, mm.w, vv.w, w1, b2, one_m_b2, bc2_sqrt, eps, neg_step);
-        reinterpret_cast<float4*>(p)[i] = pp; reinterpret_cast<float4*>(m)[i] = mm; reinterpret_cast<float4*>(v)[i] = vv;
-        if (teacher != nullptr) {
-            float4 tt = reinterpret_cast<float4*>(teacher)[i];
-            tt.x = __fadd_rn(__fmul_rn(tt.x, alpha), __fmul_rn(one_m_alpha, pp.x));
-            tt.y = __fadd_rn(__fmul_rn(tt.y, alpha), __fmul_rn(one_m_alpha, pp.y));
-            tt.z = __fadd_rn(__fmul_rn(tt.z, alpha), __fmul_rn(one_m_alpha, pp.z));
-            tt.w = __fadd_rn(__fmul_rn(tt.w, alpha), __fmul_rn(one_m_alpha, pp.w));
-            reinterpret_cast<float4*>(teacher)[i] = tt;
-        }
-    }
+    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n4; i += (size_t)gridDim.x * 256)
+        adam_ema_at(p, g, m, v, teacher, i, w1, b2, one_m_b2, bc2_sqrt, eps, neg_step, alpha, one_m_alpha, gscale);
 }
 __global__ void __launch_bounds__(256) adam_ema_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                                        float* __restrict__ v, float* __restrict__ teacher, size_t n4, float w1, float b2,
@@ -79,6 +86,63 @@ __global__ void __launch_bounds__(256) adam_ema_dev_kernel(float* __restrict__ p
                                                            float* __restrict__ v, float* __restrict__ teacher, size_t n4,
                                                            const float* __restrict__ s) {
     adam_ema_sweep(p, g, m, v, teacher, n4, s[0], s[1], s[2], s[3], s[4], s[5], s[6], s[7], s[8]);
+}
+
+// ---------------------------------------------------------------------------------------------
+// per-video sweeps: video g owns the float4s [g n4, (g + 1) n4) of every arena and has its own scalars, which travel in the
+// launch parameters (no device table).  The grid strides over the active videos' float4s as over one arena of nact * n4
+// float4s, with the one-arena sweep's grid: step j of the walk is float4 j % n4 of the (j / n4)-th active video (t.video), the
+// pair advanced by subtraction rather than division.
+// ---------------------------------------------------------------------------------------------
+struct VideoSweep {
+    float s[MAX_VIDEOS][ADAM_SCALARS];      // SGD: s[g][0] = -lr of video g; Adam: dboa_adam_scalars' row of video g
+    unsigned char video[MAX_VIDEOS];
+};
+
+// the active videos into t.video; returns their number
+static int active_videos(VideoSweep& t, int groups, unsigned long long active) {
+    int nact = 0;
+    for (int g = 0; g < groups; ++g)
+        if ((active >> g) & 1ULL) t.video[nact++] = (unsigned char)g;
+    return nact;
+}
+
+// calls at(video, float4 index in the stack) for every float4 of the walk this thread takes
+template <class At>
+__device__ __forceinline__ void video_walk(size_t n4, int nact, const VideoSweep& t, const At& at) {
+    const size_t total = n4 * nact, stride = (size_t)gridDim.x * 256;
+    size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
+    if (i >= total) return;
+    int k = (int)(i / n4);
+    size_t off = i - (size_t)k * n4;
+    for (; i < total; i += stride) {
+        const int v = t.video[k];
+        at(v, (size_t)v * n4 + off);
+        off += stride;
+        while (off >= n4) { off -= n4; ++k; }
+    }
+}
+
+__global__ void __launch_bounds__(256) sgd_update_groups_kernel(const float* __restrict__ p, const float* __restrict__ g, float* __restrict__ out,
+                                                                size_t n4, int nact, const VideoSweep t) {
+    video_walk(n4, nact, t, [&](int v, size_t i) { sgd_at(p, g, out, t.s[v][0], i); });
+}
+int sgd_update_groups(const float* p, const float* g, float* out, const float* lr, size_t n, int groups, unsigned long long active,
+                      cudaStream_t st) {
+    VideoSweep t;
+    for (int v = 0; v < groups; ++v)
+        if ((active >> v) & 1ULL) t.s[v][0] = -lr[v];
+    const int nact = active_videos(t, groups, active);
+    sgd_update_groups_kernel<<<sweep_grid(n / 4 * nact), 256, 0, st>>>(p, g, out, n / 4, nact, t);
+    return check_launch();
+}
+
+__global__ void __launch_bounds__(256) adam_ema_groups_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                                                              float* __restrict__ v, float* __restrict__ teacher, size_t n4, int nact,
+                                                              const VideoSweep t) {
+    video_walk(n4, nact, t, [&](int k, size_t i) {
+        adam_ema_at(p, g, m, v, teacher, i, t.s[k][0], t.s[k][1], t.s[k][2], t.s[k][3], t.s[k][4], t.s[k][5], t.s[k][6], t.s[k][7], t.s[k][8]);
+    });
 }
 void adam_scalars(double lr, double beta1, double beta2, double eps, int step, double alpha, float gscale, float out[ADAM_SCALARS]) {
     // torch.optim.Adam (single-tensor path) derives these from the hyperparameters in Python doubles, then casts each
@@ -98,6 +162,16 @@ int adam_ema(float* p, const float* g, float* m, float* v, float* teacher, size_
 int adam_ema_dev(float* p, const float* g, float* m, float* v, float* teacher, size_t n, const float* scalars, cudaStream_t st) {
     if (n % 4) return DBOA_ERR_ARG;
     adam_ema_dev_kernel<<<sweep_grid(n / 4), 256, 0, st>>>(p, g, m, v, teacher, n / 4, scalars);
+    return check_launch();
+}
+int adam_ema_groups(float* p, const float* g, float* m, float* v, float* teacher, size_t n, const float* scalars, int groups,
+                    unsigned long long active, cudaStream_t st) {
+    VideoSweep t;
+    for (int k = 0; k < groups; ++k)
+        if ((active >> k) & 1ULL)
+            for (int i = 0; i < ADAM_SCALARS; ++i) t.s[k][i] = scalars[k * ADAM_SCALARS + i];
+    const int nact = active_videos(t, groups, active);
+    adam_ema_groups_kernel<<<sweep_grid(n / 4 * nact), 256, 0, st>>>(p, g, m, v, teacher, n / 4, nact, t);
     return check_launch();
 }
 

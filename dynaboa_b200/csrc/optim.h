@@ -25,6 +25,14 @@ constexpr int ADAM_SCALARS = 9;
 void adam_scalars(double lr, double beta1, double beta2, double eps, int step, double alpha, float gscale, float out[ADAM_SCALARS]);
 // adam_ema with the scalars read from the device block `scalars` (ADAM_SCALARS floats) when the kernel runs
 int adam_ema_dev(float* p, const float* g, float* m, float* v, float* teacher, size_t n, const float* scalars, cudaStream_t st);
+// Per-video sweeps over `groups` (1..64) arenas of n floats each, only the videos whose bit is set in `active` (others: not read,
+// not written).  lr: host (groups,) array, video g's learning rate; scalars: host (groups, ADAM_SCALARS) array, video g's row of
+// adam_scalars.  Video g's floats are bit-identical to sgd_update / adam_ema_dev over its arenas with its scalars.  The
+// caller checks the arguments (n % 4 == 0, groups, active).
+int sgd_update_groups(const float* p, const float* g, float* out, const float* lr, size_t n, int groups, unsigned long long active,
+                      cudaStream_t st);
+int adam_ema_groups(float* p, const float* g, float* m, float* v, float* teacher, size_t n, const float* scalars, int groups,
+                    unsigned long long active, cudaStream_t st);
 int ema_update(float* teacher, const float* p, size_t n, double alpha, cudaStream_t st);
 // out[i] = cos(a_i, b_i) (NULL to skip); terms[i] = (a.b, |a|^2, |b|^2) in double (NULL to skip): the data-parallel feature test all-reduces them.
 // Per video g whose bit is set in `active`: out[g][i], terms[g][i], each from video g's parts alone; the rows of other videos

@@ -19,6 +19,7 @@ call) and callbacks for what stays with the adaptor.  A set of videos is an int 
 """
 import collections
 import ctypes as C
+from types import SimpleNamespace
 
 import torch
 
@@ -43,17 +44,21 @@ class Step:
     per-video generators; ``save_hist(image, kp, mask)`` / ``get_hist(live)``: the history frames; ``adam(mask, teacher=None,
     alpha=0.0)``: Adam (+ EMA into ``teacher``) of the videos in ``mask``; ``evaluate(batch, arena, mask, inner)``: one
     evaluation of ``arena`` (``inner``: the inner step of fast weights, None for theta); ``reduce_terms(terms)``: the
-    data-parallel sum of the feature test's sums (None: one rank).  Set per frame: ``eval_mode`` ('none', 'final', 'all'),
-    ``grad_sync`` (the data-parallel ``BucketedGradSync`` or None) and ``phase_events`` (a list: CUDA events per phase)."""
+    data-parallel sum of the feature test's sums (None: one rank); ``hparams``: per video, a dict of the options it sets for
+    itself (``multivideo.PER_VIDEO``; None: every video runs with ``options``).  Set per frame: ``eval_mode`` ('none', 'final',
+    'all'), ``grad_sync`` (the data-parallel ``BucketedGradSync`` or None) and ``phase_events`` (a list: CUDA events per phase);
+    ``fused_adapt`` sets ``hp`` (``frame_options``)."""
 
     def __init__(self, options, G, theta, grad, buffers, smpl_neutral, gmm_f, teacher=None, teacher_buffers=None, teacher_masks=None,
                  kp_range=(25, 24), motion_lead=0, bank=None, rngs=None, save_hist=None, get_hist=None, adam=None, evaluate=None,
-                 reduce_terms=None):
+                 reduce_terms=None, hparams=None):
         self.options, self.G, self.theta, self.grad, self.buffers, self.smpl_neutral, self.gmm_f = options, G, theta, grad, buffers, smpl_neutral, gmm_f
         self.teacher, self.teacher_buffers, self.teacher_masks = teacher, teacher_buffers, teacher_masks
         self.kp_range, self.motion_lead, self.bank, self.rngs = kp_range, motion_lead, bank, rngs
         self.save_hist, self.get_hist, self.adam, self.evaluate, self.reduce_terms = save_hist, get_hist, adam, evaluate, reduce_terms
         self.eval_mode, self.grad_sync, self.phase_events = 'none', None, None
+        self.hparams, self.hp = hparams, None
+        self._motion_w = None                   # (values, device tensor) of _motion_weights
         # the step's scratch: motion pair images and gradients, cosine partial sums, fast weights, inner gradient, cluster index
         self._pair = self._bgrad_flat = self._cos_partial = self._fast = self._inner_grad = None
         self._best = None if bank is None else torch.zeros(G, dtype=torch.int32, device=bank.centers.device)
@@ -85,6 +90,26 @@ def merge(old, new, mask, G):
     for k, v in new.items():
         out[k] = pick(mask, G, v, old[k]) if k in old else v
     return out
+
+
+def frame_options(s, mask):
+    """The one choice of a frame between the uniform and the per-video calls: None when no video in ``mask`` carries a value
+    of its own that differs from ``options`` (the step issues exactly the uniform calls), else the G effective option
+    namespaces (``options`` for the videos outside ``mask``)."""
+    o, hps = s.options, s.hparams
+    on = [g for g in range(s.G) if (mask >> g) & 1]
+    if hps is None or not any(v != getattr(o, k, None) for g in on for k, v in hps[g].items()):
+        return None
+    return [SimpleNamespace(**{**vars(o), **hps[g]}) if g in on else o for g in range(s.G)]
+
+
+def _motion_weights(s, device):
+    """(G,) fp32 device tensor of every video's own ``motionloss_weight``: the fp32 value the scalar product of the uniform path
+    rounds its Python float to.  Uploaded again only when a video's value changes (``start``), so a frame makes no copy."""
+    key = tuple(float(h.get('motionloss_weight', s.options.motionloss_weight)) for h in s.hparams)
+    if s._motion_w is None or s._motion_w[0] != key or s._motion_w[1].device != device:
+        s._motion_w = (key, torch.tensor(key, dtype=torch.float32, device=device))
+    return s._motion_w[1]
 
 
 def _side_stream(device):
@@ -144,8 +169,9 @@ def forward_graph(s, arena, buffers, image, mask, masks=None):
 
 def _loss_head(s, p, w, kp=None, t_p2d=None, t_j3d=None, t_beta=None, t_R=None, gt_s3d=None, grads=None, nb=None):
     """Runs the (optional) pose prior and the multi-term head on the first ``nb`` samples of ``p``, each video's rows on their
-    own (per-video means and gradient scaling); returns (terms (G, 9), dp2d, dj3d, dR, dbeta).  ``grads``: preallocated
-    (possibly larger-batch) gradient buffers whose leading ``nb`` rows are written."""
+    own (per-video means and gradient scaling); returns (terms (G, 9), dp2d, dj3d, dR, dbeta).  ``w``: the 8 weights, or one
+    row of 8 per video (the per-video calls).  ``grads``: preallocated (possibly larger-batch) gradient buffers whose leading
+    ``nb`` rows are written."""
     B, dev, G = (p.B if nb is None else nb), p.rot.device, p.groups
     if grads is None:
         dp2d, dj3d = torch.empty_like(p.p2d), torch.empty_like(p.joints)
@@ -153,12 +179,16 @@ def _loss_head(s, p, w, kp=None, t_p2d=None, t_j3d=None, t_beta=None, t_R=None, 
     else:
         dp2d, dj3d, dR, dbeta = grads
     terms = torch.empty(G, 9, dtype=torch.float32, device=dev)
-    prior_b = None
-    if w[2] != 0.0:
+    prior_b, rows = None, isinstance(w[0], (list, tuple))
+    if (any(r[2] != 0.0 for r in w) if rows else w[2] != 0.0):
         prior_b = torch.empty(B, dtype=torch.float32, device=dev)
         g = s.gmm_f
-        _lib.call('dboa_pose_prior', ptr(p.rot), ptr(g.means), ptr(g.precisions), ptr(g.neg_log_weights), ptr(prior_b), ptr(dR),
-                  float(w[2]) / (B // G), B, stream())                   # per-video mean: scale w / b
+        if rows:
+            _lib.call('dboa_pose_prior_groups', ptr(p.rot), ptr(g.means), ptr(g.precisions), ptr(g.neg_log_weights), ptr(prior_b), ptr(dR),
+                      (C.c_float * G)(*[float(r[2]) / (B // G) for r in w]), B, G, stream())
+        else:
+            _lib.call('dboa_pose_prior', ptr(p.rot), ptr(g.means), ptr(g.precisions), ptr(g.neg_log_weights), ptr(prior_b), ptr(dR),
+                      float(w[2]) / (B // G), B, stream())                   # per-video mean: scale w / b
     a = _lib.LossArgsStruct()
     a.B, a.groups = B, G
     keep = []
@@ -169,11 +199,14 @@ def _loss_head(s, p, w, kp=None, t_p2d=None, t_j3d=None, t_beta=None, t_R=None, 
             t = t if (t.is_contiguous() and t.dtype == torch.float32) else t.contiguous().float()
             keep.append(t)
         setattr(a, name, None if t is None else t.data_ptr())
-    for i in range(8):
-        a.w[i] = float(w[i])
     a.dR_accumulate = 1 if prior_b is not None else 0
     a.kp_first, a.kp_count = s.kp_range                             # joints of the re-projection term (webcam client: (0, 25))
-    _lib.call('dboa_loss_multi', C.byref(a), stream())
+    if rows:
+        _lib.call('dboa_loss_multi_weights', C.byref(a), (C.c_float * (8 * G))(*[float(x) for r in w for x in r]), stream())
+    else:
+        for i in range(8):
+            a.w[i] = float(w[i])
+        _lib.call('dboa_loss_multi', C.byref(a), stream())
     return terms, dp2d, dj3d, dR, dbeta
 
 
@@ -225,7 +258,7 @@ def level_backward(s, out, arena, image, kp, lower, grad_arena, mask, live, main
     With one video, when the motion loss is live and no forward is supplied, the current and the history frame go through
     ONE batched forward / backward (same weights, independent samples), and the teacher forward runs on a side stream.
     With several, the history frame gets its own grouped pass and the teacher runs on the caller's stream."""
-    o, G = s.options, s.G
+    o, G, hp = s.options, s.G, s.hp
     tag = 'll' if lower else 'ul'
     nb = image.shape[0]
     use_frame = o.use_frame_losses_lower if lower else o.use_frame_losses_upper
@@ -255,10 +288,16 @@ def level_backward(s, out, arena, image, kp, lower, grad_arena, mask, live, main
         main = forward_graph(s, arena, s.buffers, image, mask)
     batched = main.B > nb
     hist = forward_graph(s, arena, s.buffers, hist_image, live) if motion and not batched else None
-    w = [0.0] * 8
+
+    def head_weights(q):                                        # the head's 8 weights under the options q
+        w = [0.0] * 8
+        if use_frame:
+            w[0], w[1], w[2] = q.s2dloss_weight, q.shape_prior_weight, q.pose_prior_weight
+        if tpred is not None:
+            tw = q.teacherloss_weight
+            w[3], w[4], w[5], w[6] = 5 * tw, 5 * tw, 0.001 * tw, 1 * tw
+        return w
     targets = {}
-    if use_frame:
-        w[0], w[1], w[2] = o.s2dloss_weight, o.shape_prior_weight, o.pose_prior_weight
     if tpred is not None:
         t = tpred
         if side is not None:
@@ -266,8 +305,6 @@ def level_backward(s, out, arena, image, kp, lower, grad_arena, mask, live, main
             cur.wait_stream(side)
             for ten in (t.p2d, t.joints, t.shape, t.rot, t.tape, t.verts, t.smpl_tape, t.cam):
                 ten.record_stream(cur)
-        tw = o.teacherloss_weight
-        w[3], w[4], w[5], w[6] = 5 * tw, 5 * tw, 0.001 * tw, 1 * tw
         targets = dict(t_p2d=t.p2d, t_j3d=t.joints, t_beta=t.shape, t_R=t.rot)
     _mark(s, f'{tag}: forward(s) issued')
     grads = None
@@ -279,6 +316,7 @@ def level_backward(s, out, arena, image, kp, lower, grad_arena, mask, live, main
         flat = s._bgrad_flat
         _zero(flat)
         grads = tuple(t.view(Bm, *sh) for t, sh in zip(flat.split(sizes), ((49, 2), (49, 3), (24, 3, 3), (10,))))
+    w = head_weights(o) if hp is None else [head_weights(q) for q in hp]
     terms, dp2d, dj3d, dR, dbeta = _loss_head(s, main, w, kp=kp if use_frame else None, grads=grads, nb=nb, **targets)
     total = terms[:, 8]
     if use_frame:
@@ -290,13 +328,19 @@ def level_backward(s, out, arena, image, kp, lower, grad_arena, mask, live, main
         p_hist = main.p2d[nb:] if batched else hist.p2d
         dph = dp2d[nb:] if batched else torch.empty_like(hist.p2d)
         kf, kn = s.kp_range
-        margs = (ptr(main.p2d), ptr(p_hist), ptr(kp), ptr(hist_kp.contiguous()), float(o.motionloss_weight), ptr(mterm), ptr(dp2d), ptr(dph),
-                 nb, 1, kf, kn, G)
-        _lib.call('dboa_loss_motion_active', *margs, live, stream())
+        if hp is None:
+            mw, entry = float(o.motionloss_weight), 'dboa_loss_motion_active'
+        else:
+            mw, entry = (C.c_float * G)(*[q.motionloss_weight for q in hp]), 'dboa_loss_motion_weights'
+        margs = (ptr(main.p2d), ptr(p_hist), ptr(kp), ptr(hist_kp.contiguous()), mw, ptr(mterm), ptr(dp2d), ptr(dph), nb, 1, kf, kn, G)
+        _lib.call(entry, *margs, live, stream())
         if not batched:
             backward_graph(s, arena, hist, dph, torch.zeros_like(hist.joints), torch.zeros_like(hist.rot), torch.zeros_like(hist.shape),
                            grad_arena)
-        total = total + mterm * o.motionloss_weight
+        if hp is None:
+            total = total + mterm * o.motionloss_weight
+        else:
+            total = total + mterm * _motion_weights(s, image.device)
         fit['ul/motion_loss'] = mterm
     _mark(s, f'{tag}: loss head')
     mix = bool(o.retrieval and (o.lower_level_mixtrain if lower else o.upper_level_mixtrain))
@@ -311,9 +355,9 @@ def level_backward(s, out, arena, image, kp, lower, grad_arena, mask, live, main
             n = e.B
             gt_R = torch.empty(n, 24, 3, 3, dtype=torch.float32, device=image.device)
             _lib.call('dboa_rodrigues', ptr(ex['pose'].reshape(-1, 3).contiguous()), ptr(gt_R), n * 24, 0, stream())
-            lw = o.labelloss_weight
-            eterms, a, b, c, d = _loss_head(s, e, [5 * lw, 0, 0, 0, 0, 0.001 * lw, 1 * lw, 5 * lw], kp=ex['keypoints'], t_beta=ex['betas'],
-                                            t_R=gt_R, gt_s3d=ex['pose_3d'])
+            label = lambda lw: [5 * lw, 0, 0, 0, 0, 0.001 * lw, 1 * lw, 5 * lw]
+            ew = label(o.labelloss_weight) if hp is None else [label(q.labelloss_weight) for q in hp]
+            eterms, a, b, c, d = _loss_head(s, e, ew, kp=ex['keypoints'], t_beta=ex['betas'], t_R=gt_R, gt_s3d=ex['pose_3d'])
             backward_graph(s, arena, e, a, b, c, d, grad_arena, sync=sync)
             total = total + eterms[:, 8]
             fit[f'{tag}/labled_loss'] = eterms[:, 8]
@@ -364,14 +408,16 @@ def feature_test(s, fit, a, b, mask):
     return out
 
 
-def _continuing(o, sims, steps):
+def _continuing(o, sims, steps, hp=None):
     """Bit mask of the videos of ``sims`` whose own test says 'continue' and whose trip count ``steps[g]`` (advanced here, as
-    the reference's loop does before its cap test) is still within ``optim_steps``."""
+    the reference's loop does before its cap test) is still within ``optim_steps``.  ``hp``: the frame's per-video options
+    (``frame_options``; None: ``o`` for every video), whose ``cos_sim_threshold`` and ``optim_steps`` video g uses."""
     mask = 0
     for g, s in sims.items():
-        if 1 - s[12]['cos'] > o.cos_sim_threshold:
+        q = o if hp is None else hp[g]
+        if 1 - s[12]['cos'] > q.cos_sim_threshold:
             steps[g] += 1
-            if steps[g] <= o.optim_steps:
+            if steps[g] <= q.optim_steps:
                 mask |= 1 << g
     return mask
 
@@ -381,6 +427,7 @@ def fused_adapt(s, batch, mask, frames):
     SGD steps of the lower level, the upper level, one Adam + EMA teacher sweep, then the optional ``dynamic_boa`` loop.
     ``frames[g]``: the frames video g adapted before this one (its motion term's clock).  Returns the ``Frame``."""
     o, G, theta, buffers, grad = s.options, s.G, s.theta, s.buffers, s.grad
+    s.hp = hp = frame_options(s, mask)                                   # uniform or per-video calls, for the whole frame
     out = Frame(mask)
     image, kp = batch['image'].contiguous().float(), batch['smpl_j2d'].contiguous().float()
     s.save_hist(image, kp, mask)
@@ -406,8 +453,12 @@ def fused_adapt(s, batch, mask, frames):
             level_backward(s, out, fast, image, kp, True, s._inner_grad, mask, live, main=cur if i == 0 else None)
             _mark(s, 'lower level (loss + backward)')
             nxt = s._fast[i % 2]
-            for f, g, n in zip(_active_rows(fast, mask, G), _active_rows(s._inner_grad, mask, G), _active_rows(nxt, mask, G)):
-                _lib.call('dboa_sgd_update', ptr(f), ptr(g), ptr(n), float(o.fastlr), f.numel(), stream())
+            if hp is None:
+                for f, g, n in zip(_active_rows(fast, mask, G), _active_rows(s._inner_grad, mask, G), _active_rows(nxt, mask, G)):
+                    _lib.call('dboa_sgd_update', ptr(f), ptr(g), ptr(n), float(o.fastlr), f.numel(), stream())
+            else:
+                _lib.call('dboa_sgd_update_groups', ptr(fast), ptr(s._inner_grad), ptr(nxt), (C.c_float * G)(*[q.fastlr for q in hp]),
+                          fast.numel() // G, G, mask, stream())
             fast = nxt
             _mark(s, 'inner SGD step')
             if evaluate == 'all':
@@ -426,7 +477,7 @@ def fused_adapt(s, batch, mask, frames):
             after = forward_graph(s, theta, buffers, image, mask)
             sims = feature_test(s, out.fit, probe, after, mask)
             out.sims, out.steps = {g: [x] for g, x in sims.items()}, dict.fromkeys(sims, 0)
-            loop = _continuing(o, sims, out.steps)
+            loop = _continuing(o, sims, out.steps, hp)
             while loop:
                 for t in _active_rows(grad, loop, G):
                     _zero(t)
@@ -439,7 +490,7 @@ def fused_adapt(s, batch, mask, frames):
                     out.sims[g].append(x)
                 if evaluate == 'all':
                     out.result = s.evaluate(batch, theta, loop, None)
-                loop = _continuing(o, sims, out.steps)
+                loop = _continuing(o, sims, out.steps, hp)
             if evaluate == 'final':
                 out.result = s.evaluate(batch, theta, mask, None)
         return out

@@ -11,8 +11,11 @@ G slots are a pool: a slot whose batch is None sits the frame out (its CTAs retu
 """
 import ctypes as C
 import itertools
+import math
+import numbers
 import os
 import random
+from types import SimpleNamespace
 
 import numpy as np
 import torch
@@ -27,6 +30,10 @@ PENDING_FRAMES = 256        # device records kept before adapt forms them on the
 # a slot's host records, one entry per slot, as a slot state holds them
 SLOT_RECORDS = ('mpjpe_all', 'pampjpe_all', 'pve_all', 'mpjpe_all_lower', 'pampjpe_all_lower', 'mpjpe_statistics', 'pampjpe_statistics',
                 'kp2dloss_lower_all', 'kp2dloss_upper_all', 'optim_step_record', 'feat_sims', 'optimized_step', 'last_retrieval')
+# the options a slot may set for itself (start(g, hparams=...)): the learning rates, Adam's betas, the teacher rate, the loss
+# weights and the dynamic loop's test.  Every other option changes which passes a step runs, or their rows, and is the pool's.
+PER_VIDEO = frozenset({'lr', 'beta1', 'beta2', 'fastlr', 'alpha', 's2dloss_weight', 'shape_prior_weight', 'pose_prior_weight',
+                       'teacherloss_weight', 'motionloss_weight', 'labelloss_weight', 'cos_sim_threshold', 'optim_steps'})
 
 
 def check_options(options, n_videos, dynamic_loop=False):
@@ -48,6 +55,51 @@ def check_options(options, n_videos, dynamic_loop=False):
         rows = max(rows, int(options.sample_num))
     if G * rows > 64:
         raise ValueError(f'{G} videos x {rows} rows per grouped call exceed the 64 samples of the network tape')
+
+
+def check_hparams(options, hparams, n_videos=None):
+    """Raise ValueError for per-video hyperparameters the pool of ``options`` cannot run (no device needed); return them checked.
+    ``hparams``: a dict from keys of ``PER_VIDEO`` to values (one slot), or, given ``n_videos``, a list of such dicts or None, one
+    per video (None for the list: none).  Returns the dict with float values (``optim_steps``: int), or the list of them ({} for
+    None).  A slot's ``pose_prior_weight`` must be zero exactly when the pool's is: the prior pass runs for a non-zero weight
+    only, so a mix would change the step's passes."""
+    if n_videos is not None:
+        if hparams is None:
+            return [{} for _ in range(n_videos)]
+        hparams = list(hparams)
+        if len(hparams) != n_videos:
+            raise ValueError(f'{len(hparams)} hparams for {n_videos} videos')
+        return [{} if h is None else check_hparams(options, h) for h in hparams]
+    if not isinstance(hparams, dict):
+        raise ValueError(f'hparams must be a dict of options, got {type(hparams).__name__}')
+    out = {}
+    for k, v in hparams.items():
+        if k not in PER_VIDEO:
+            raise ValueError(f'{k!r} is not an option a slot may set: one of {", ".join(sorted(PER_VIDEO))}')
+        if k == 'optim_steps':
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, numbers.Integral) or v < 0:
+                raise ValueError(f'optim_steps must be a non-negative int, got {v!r}')
+            out[k] = int(v)
+            continue
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, numbers.Real) or not math.isfinite(v):
+            raise ValueError(f'{k} must be a finite number, got {v!r}')
+        v = float(v)
+        if k in ('lr', 'fastlr') and v < 0:
+            raise ValueError(f'{k} must not be negative, got {v!r}')
+        if k in ('beta1', 'beta2') and not 0.0 <= v < 1.0:
+            raise ValueError(f'{k} must lie in [0, 1), got {v!r}')
+        if k == 'alpha' and not 0.0 <= v <= 1.0:
+            raise ValueError(f'alpha must lie in [0, 1], got {v!r}')
+        if k == 'pose_prior_weight' and (v == 0.0) != (getattr(options, 'pose_prior_weight', 0.0) == 0.0):
+            raise ValueError(f'pose_prior_weight {v!r}: zero in some slots and non-zero in others would change the step '
+                             f'(the pool\'s is {getattr(options, "pose_prior_weight", None)!r})')
+        out[k] = v
+    return out
+
+
+def own_values(options, hparams):
+    """The entries of ``hparams`` that differ from ``options``: what a slot runs with beyond the pool's options."""
+    return {k: v for k, v in hparams.items() if v != getattr(options, k, None)}
 
 
 def video_names(videos, names, default):
@@ -132,10 +184,12 @@ class MultiVideoAdaptor:
         self.mpjpe_statistics, self.pampjpe_statistics = [{} for _ in range(G)], [{} for _ in range(G)]
         self.kp2dloss_lower_all, self.kp2dloss_upper_all = [[] for _ in range(G)], [{} for _ in range(G)]
         self._writer, self._pinned = state_mod.Writer(), state_mod.Pinned()     # checkpoints written in the background (save)
+        self.hparams = [{} for _ in range(G)]   # per slot: the PER_VIDEO values it runs with where they differ from options
         self._step = Step(o, G, self.thetas, self.grad, self.buffers, base.smpl_neutral, base.gmm_f, teacher=self.teachers,
                           teacher_buffers=self.buffers, teacher_masks=self._teacher_masks, kp_range=self.kp_range,
                           motion_lead=self.motion_lead, bank=base.bank if o.retrieval else None, rngs=self.rngs,
-                          save_hist=self._save_hist, get_hist=self._get_hist, adam=self._adam_ema, evaluate=self._evaluate)
+                          save_hist=self._save_hist, get_hist=self._get_hist, adam=self._adam_ema, evaluate=self._evaluate,
+                          hparams=self.hparams)
         for g in range(G):
             self.start(g)
 
@@ -144,17 +198,27 @@ class MultiVideoAdaptor:
         from .adaptor import Adaptor
         return Adaptor(options)
 
-    def start(self, g, seed=None, state=None):
+    def start(self, g, seed=None, state=None, hparams=None):
         """Put a new video into slot g: theta and teacher from the checkpoint, zero Adam moments, step and frame counts, an empty
         history, empty records, and ``rngs[g] = random.Random(seed)`` (default ``options.seed * 1000 + g``).  The records of
         the frames adapted so far are formed on the host first (one synchronisation, if any are pending).
 
+        ``hparams``: a dict from keys of ``PER_VIDEO`` to values (``check_hparams``): slot g runs with ``options`` plus these
+        values until its next ``start`` (``slot_options(g)``).
+
         ``state``: a video state written by ``save_slot`` (its path, or the dict ``state.read_video`` returned) of a pool with
         the same G and compatible options, from any slot: slot g continues that video instead -- theta, teacher, moments, step
-        count, ``video_steps[g]``, history ring, ``rngs[g]`` and records.  It is checked before any device work (ValueError)."""
+        count, ``video_steps[g]``, history ring, ``rngs[g]``, records and its hparams (``hparams`` that contradict them raise).
+        Everything is checked before any device work (ValueError)."""
+        self._check_slot(g)
         if state is not None and not isinstance(state, dict):
-            self._check_slot(g)
-            state = state_mod.read_video(state, self.options, 'slot', self.G)
+            state = state_mod.read_video(state, self.options, 'slot', self.G, own=PER_VIDEO)
+        hp = None if hparams is None else own_values(self.options, check_hparams(self.options, hparams))
+        if state is not None:
+            saved = own_values(self.options, check_hparams(self.options, state_mod.saved_options(state, PER_VIDEO)))
+            if hp is not None and hp != saved:
+                raise ValueError(f'slot {g}: hparams {hparams!r} contradict the state\'s {saved!r}')
+            hp = saved
         self._reset_weights(g)
         self._form_records()
         self.video_steps[g] = 0
@@ -166,8 +230,14 @@ class MultiVideoAdaptor:
         self.mpjpe_all_lower[g], self.pampjpe_all_lower[g] = [[] for _ in range(n)], [[] for _ in range(n)]
         self.mpjpe_statistics[g], self.pampjpe_statistics[g] = {}, {}
         self.kp2dloss_lower_all[g], self.kp2dloss_upper_all[g] = [], {}
+        self.hparams[g] = hp or {}
         if state is not None:
             self._restore_slot(g, state)
+
+    def slot_options(self, g):
+        """Slot g's effective options: the pool's ``options`` with the slot's hparams."""
+        self._check_slot(g)
+        return SimpleNamespace(**{**vars(self.options), **self.hparams[g]})
 
     def _check_slot(self, g):
         if not isinstance(g, int) or not 0 <= g < self.G:
@@ -234,10 +304,21 @@ class MultiVideoAdaptor:
 
     def _adam_ema(self, on, teacher=None, alpha=0.0):
         """Adam + EMA into the teacher stack ``teacher`` of the slots in ``on``, each at its own step count: one sweep per run of
-        consecutive slots that share a step count (one sweep over the whole stack while every slot runs in step)."""
-        o = self.options
+        consecutive slots that share a step count (one sweep over the whole stack while every slot runs in step).  In a frame
+        of per-video calls (the step's ``hp``), one ``dboa_adam_ema_groups`` sweep with each slot's lr, betas, step count and
+        alpha."""
+        o, hp = self.options, self._step.hp
         for g in self._slots(on):
             self.step_counts[g] += 1
+        if hp is not None:
+            rows, one = (C.c_float * (self.G * _lib.ADAM_SCALARS))(), (C.c_float * _lib.ADAM_SCALARS)()
+            for g in self._slots(on):
+                q = hp[g]
+                _lib.call('dboa_adam_scalars', one, float(q.lr), float(q.beta1), float(q.beta2), 1e-8, self.step_counts[g], float(q.alpha), 1.0)
+                rows[g * _lib.ADAM_SCALARS:(g + 1) * _lib.ADAM_SCALARS] = one[:]
+            _lib.call('dboa_adam_ema_groups', ptr(self.thetas), ptr(self.grad), ptr(self.m), ptr(self.v), ptr(teacher),
+                      self.thetas.shape[1], rows, self.G, on, stream())
+            return
         for a, b in runs(on, self.G, key=lambda g: self.step_counts[g]):
             _lib.call('dboa_adam_ema_scaled', ptr(self.thetas[a:b]), ptr(self.grad[a:b]), ptr(self.m[a:b]), ptr(self.v[a:b]),
                       ptr(None if teacher is None else teacher[a:b]), self.thetas[a:b].numel(), float(o.lr), float(o.beta1), float(o.beta2), 1e-8,
@@ -376,7 +457,7 @@ class MultiVideoAdaptor:
                     feat_sims=dict(self.feat_sims[g]), optim_step_record=list(self.optim_step_record[g]),
                     kp2dlosses_lower=list(self.kp2dloss_lower_all[g]), kp2dlosses_upper=dict(self.kp2dloss_upper_all[g]))
 
-    def run(self, videos, exppath=None, names=None, checkpoint=None, every=0):
+    def run(self, videos, exppath=None, names=None, checkpoint=None, every=0, hparams=None):
         """Adapt every video of ``videos`` (a list of iterables of batch dicts with batch size 1: a ``DataLoader`` over a
         sequence, a ``SyntheticStream``) through the G slots.  Slots are filled in order and refilled from the queue as soon as
         their video ends; video i starts with ``start(g, seed=options.seed * 1000 + i)``, so its seed follows the video, and
@@ -388,9 +469,13 @@ class MultiVideoAdaptor:
         ``checkpoint``: a directory of pool checkpoints (``save``), written every ``every`` ticks and once more at the end.  When it
         holds a complete checkpoint the run resumes from it: the finished videos' summaries are returned as recorded (their
         result files are left alone), every video in flight continues in its slot from its own frame, and the queue goes on
-        from there.  The summaries and result files are those of a run that was never interrupted."""
+        from there.  The summaries and result files are those of a run that was never interrupted.
+
+        ``hparams``: one dict of ``start``'s hparams, or None, per video; the dict follows the video into its slot, as its seed
+        does.  A resumed run must be given the hparams of the run it continues."""
         from .adaptor import write_records
         videos = list(videos)
+        hparams = check_hparams(self.options, hparams, len(videos))
         names = video_names(videos, names, default=[str(i) for i in range(len(videos))])
         mean = lambda v: float(np.mean(v)) if len(v) else float('nan')
 
@@ -403,23 +488,32 @@ class MultiVideoAdaptor:
                 os.makedirs(d, exist_ok=True)
                 write_records(d, rec['frames'] - 1, rec)
             return dict(name=names[i], frames=rec['frames'], mpjpe=mean(rec['mpjpe']), pampjpe=mean(rec['pampjpe']), pve=mean(rec['pve']))
-        return self._queue(videos, self.adapt, finish, checkpoint=checkpoint, every=every)
+        return self._queue(videos, self.adapt, finish, checkpoint=checkpoint, every=every, hparams=hparams)
 
-    def _queue(self, videos, tick, finish, checkpoint=None, every=0, items_from=None, barrier=None):
+    def _queue(self, videos, tick, finish, checkpoint=None, every=0, items_from=None, barrier=None, hparams=None):
         """``run``'s queue: the slots are filled in order and refilled as soon as their video ends; video i starts with
         ``start(g, seed=options.seed * 1000 + i)`` and ``slot_video[g] = i``.  ``tick(items)`` advances the pool by one frame,
         ``items[g]`` being slot g's next item of its video (None: an idle slot); ``finish(i, g)`` returns video i's summary once
         it ended in slot g (g None: video i was empty), before the slot is refilled.  Returns the summaries in order.
 
         ``checkpoint`` / ``every``: ``run``'s.  ``items_from(i, k)``: an iterator over video i's items from item k on (default
-        ``items_from``); ``barrier()``: futures of files a checkpoint taken now covers (``save``)."""
+        ``items_from``); ``barrier()``: futures of files a checkpoint taken now covers (``save``); ``hparams``: video i's
+        ``start`` hparams (checked; None: none)."""
         n = len(videos)
+        hparams = check_hparams(self.options, hparams, n)
+        own = [own_values(self.options, h) for h in hparams]
         queue, its, nxt, out = list(range(n)), [None] * self.G, [None] * self.G, [None] * n
         items_from = items_from or (lambda i, k: _items_from(videos[i], k))
-        run = self.load(checkpoint) if checkpoint is not None else None
-        if run is not None:
+
+        def check_run(run):                                  # before the checkpoint's slots are restored
+            if run is None:
+                return
             if run['videos'] != n:
                 raise ValueError(f'{checkpoint}: the checkpoint is of a queue of {run["videos"]} videos, not {n}')
+            if run.get('hparams', [{}] * n) != own:
+                raise ValueError(f'{checkpoint}: the checkpoint is of a run with hparams {run.get("hparams")!r}, not {own!r}')
+        run = self.load(checkpoint, check_run) if checkpoint is not None else None
+        if run is not None:
             queue, out = list(run['queue']), list(run['out'])
             for g in range(self.G):
                 if self.slot_video[g] is not None:
@@ -427,7 +521,7 @@ class MultiVideoAdaptor:
                     nxt[g] = next(its[g], None)
 
         def save():
-            self.save(checkpoint, run=dict(videos=n, queue=queue, out=out), barrier=barrier, wait=False)
+            self.save(checkpoint, run=dict(videos=n, queue=queue, out=out, hparams=own), barrier=barrier, wait=False)
 
         def fill(g):
             self.slot_video[g] = None
@@ -438,7 +532,7 @@ class MultiVideoAdaptor:
                 if nxt[g] is None:
                     out[i] = finish(i, None)
                     continue
-                self.start(g, seed=self.options.seed * 1000 + i)
+                self.start(g, seed=self.options.seed * 1000 + i, hparams=hparams[i])
                 self.slot_video[g] = i
                 return
 
@@ -474,7 +568,7 @@ class MultiVideoAdaptor:
             hist.append((k, small(image[g * b:(g + 1) * b]), small(kp[g * b:(g + 1) * b])))
         records = {name: getattr(self, name)[g] for name in SLOT_RECORDS}
         records['last_upper_loss'] = small(self.last_upper_loss[g:g + 1])
-        return state_mod.video_state(self.options, 'slot', G, copy(('theta', g), self.thetas[g]),
+        return state_mod.video_state(self.slot_options(g), 'slot', G, copy(('theta', g), self.thetas[g]),
                                      None if self.teachers is None else copy(('teacher', g), self.teachers[g]),
                                      copy(('m', g), self.m[g]), copy(('v', g), self.v[g]), self.step_counts[g], self.video_steps[g], hist,
                                      dict(random=self.rngs[g].getstate()), records)
@@ -544,10 +638,12 @@ class MultiVideoAdaptor:
         if wait:
             self._writer.wait()
 
-    def load(self, root):
+    def load(self, root, check_run=None):
         """Continue from the newest complete checkpoint ``save`` wrote under ``root``: every file is checked first (ValueError),
         then the saved slots are restored with ``start(g, state=...)``, the others marked empty in ``slot_video``, and
-        ``global_step`` and torch's CUDA generator set.  Returns the checkpoint's ``run`` (None without a checkpoint)."""
+        ``global_step`` and torch's CUDA generator set.  Returns the checkpoint's ``run`` (None without a checkpoint).
+        ``check_run(run)``: raises for a ``run`` the caller cannot continue, after the files are checked and before anything is
+        restored."""
         found = state_mod.latest(root)
         if found is None:
             return None
@@ -556,7 +652,10 @@ class MultiVideoAdaptor:
         pool = state_mod.read(os.path.join(path, man['pool']), state_mod.POOL, self.options)
         if pool.get('G') != self.G:
             raise ValueError(f'{path}: a checkpoint of a {pool.get("G")}-slot pool cannot be loaded into {self.G} slots')
-        states = {g: state_mod.read_video(os.path.join(path, f), self.options, 'slot', self.G) for g, f in man['slots'].items()}
+        states = {g: state_mod.read_video(os.path.join(path, f), self.options, 'slot', self.G, own=PER_VIDEO) for g, f in man['slots'].items()}
+        run = state_mod.unplain(pool['run'])
+        if check_run is not None:
+            check_run(run)
         for g in range(self.G):
             self.slot_video[g] = pool['slot_video'][g] if g in states else None
             if g in states:
@@ -564,7 +663,7 @@ class MultiVideoAdaptor:
         self.global_step = pool['global_step']
         torch.cuda.set_rng_state(pool['cuda_rng'], self.thetas.device)
         torch.cuda.synchronize(self.thetas.device)
-        return state_mod.unplain(pool['run'])
+        return run
 
     def export_model(self, g, path):
         """Write video g's adapted weights as a checkpoint in the reference's format (``Adaptor.export_model``)."""

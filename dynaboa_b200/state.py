@@ -86,11 +86,11 @@ def options_dict(options):
     return out
 
 
-def check_options(saved, options):
+def check_options(saved, options, own=frozenset()):
     """Raise ValueError naming every option that differs between ``saved`` (a state's options) and ``options`` outside
-    ``MAY_DIFFER``."""
+    ``MAY_DIFFER`` and ``own``."""
     now, missing = options_dict(options), object()
-    bad = sorted(k for k in set(saved) | set(now) if k not in MAY_DIFFER and not _same(saved.get(k, missing), now.get(k, missing)))
+    bad = sorted(k for k in set(saved) | set(now) if k not in MAY_DIFFER and k not in own and not _same(saved.get(k, missing), now.get(k, missing)))
     if bad:
         detail = ', '.join(f'{k} (saved {saved.get(k, "unset")!r}, now {now.get(k, "unset")!r})' for k in bad)
         raise ValueError(f'the state was saved with different options: {detail}')
@@ -136,9 +136,9 @@ def _fsync_dir(d):
         os.close(fd)
 
 
-def read(path, fmt, options=None):
+def read(path, fmt, options=None, own=frozenset()):
     """Load ``path`` with ``weights_only=True`` and check it: format ``fmt``, this version, this library's arena size and
-    parameter table and, given ``options``, options that differ only in ``MAY_DIFFER``.  ValueError otherwise."""
+    parameter table and, given ``options``, options that differ only in ``MAY_DIFFER`` and ``own``.  ValueError otherwise."""
     try:
         obj = torch.load(path, map_location='cpu', weights_only=True)
     except FileNotFoundError:
@@ -158,7 +158,7 @@ def read(path, fmt, options=None):
     if not isinstance(obj.get('options'), dict):
         raise ValueError(f'{path}: malformed state: no options')
     if options is not None:
-        check_options(obj['options'], options)
+        check_options(obj['options'], options, own)
     return obj
 
 
@@ -174,9 +174,11 @@ def video_state(options, kind, G, theta, teacher, m, v, step_count, frames, hist
     return out
 
 
-def read_video(path, options, kind, G=1):
-    """A video state checked against ``options``, its ``kind`` and pool width ``G``, with its records unpacked."""
-    st = read(path, VIDEO, options)
+def read_video(path, options, kind, G=1, own=frozenset()):
+    """A video state checked against ``options``, its ``kind`` and pool width ``G``, with its records unpacked.  ``own``: options
+    the video may carry values of its own in (a pool slot's per-video hyperparameters; its state holds the slot's effective
+    options), which ``saved_options`` returns."""
+    st = read(path, VIDEO, options, own)
     missing = [k for k in VIDEO_FIELDS if k not in st]
     if missing:
         raise ValueError(f'{path}: malformed video state: no {", ".join(missing)}')
@@ -196,6 +198,11 @@ def read_video(path, options, kind, G=1):
     st['records'] = unplain(st['records'])
     st['rng'] = unplain(st['rng'])
     return st
+
+
+def saved_options(st, keys):
+    """The values of the options ``keys`` a video state ``st`` was saved with (those it holds)."""
+    return {k: unplain(st['options'][k]) for k in keys if k in st['options']}
 
 
 # ------------------------------------------------------------------ background writes

@@ -157,8 +157,8 @@ class MultiWebcamAdaptor(MultiVideoAdaptor):
 
     def reload(self, g):
         """Key ``r`` of the demo for stream g (reference dynaboa_webcam.py:184-194): theta and teacher back to the checkpoint and
-        a fresh Adam (zero moments, step count 0).  The stream's history and frame count are kept, so its motion term stays as
-        it was; the other streams are left alone."""
+        a fresh Adam (zero moments, step count 0).  The stream's history, frame count and hparams (``start(g, hparams=...)``) are
+        kept, so its motion term stays as it was; the other streams are left alone."""
         self._reset_weights(g)
 
     def online_adaptation(self, frames, detections):

@@ -298,6 +298,26 @@ int dboa_loss_motion_active(const float* p_cur, const float* p_hist, const float
                             float* dp_cur, float* dp_hist, int B, int accumulate_cur, int first, int count, int groups,
                             unsigned long long active, dboa_stream_t stream);
 
+/* ---- per-video hyperparameters ---------------------------------------------------------------
+ * The calls below give each of `groups` (1..64) videos its own scalars, in the layout of the grouped calls above: video g owns
+ * the rows [g B / groups, (g + 1) B / groups) of every per-row buffer (and, in the sweeps further down, the floats
+ * [g n, (g + 1) n) of every arena).  The per-video scalars are HOST arrays with one row per video; they travel in the launch
+ * parameters, so no device table is allocated and a captured call holds its values.  Video g's outputs are bit-identical to
+ * the uniform call on its rows with its row of scalars (each entry the fp32 value the uniform call receives).  Checked before any
+ * device access: DBOA_ERR_ARG for a NULL pointer or table, DBOA_ERR_SHAPE for groups outside 1..64 or B % groups != 0, then
+ * (calls with `active`) DBOA_ERR_ARG for active == 0 or a bit at position >= groups.
+ * dboa_pose_prior_groups: dboa_pose_prior with scale (groups,): body b's gradient is scaled by scale[b / (B / groups)]. */
+int dboa_pose_prior_groups(const float* rotmat, const float* means, const float* precisions, const float* neg_log_w, float* prior_b,
+                           float* d_rotmat, const float* scale, int B, int groups, dboa_stream_t stream);
+/* dboa_loss_multi with w (a->groups, 8): video g's block uses row g in place of a->w (a->w is not read); the other arguments
+ * and their checks are dboa_loss_multi's */
+int dboa_loss_multi_weights(const dboa_loss_args* a, const float* w, dboa_stream_t stream);
+/* dboa_loss_motion_active with weight (groups,): video g's gradient is weighed with weight[g]; a video whose bit is clear gets
+ * term[g] = 0 and leaves its rows of dp_cur and dp_hist untouched, as there */
+int dboa_loss_motion_weights(const float* p_cur, const float* p_hist, const float* kp_cur, const float* kp_hist, const float* weight,
+                             float* term, float* dp_cur, float* dp_hist, int B, int accumulate_cur, int first, int count, int groups,
+                             unsigned long long active, dboa_stream_t stream);
+
 /* ---- whole-model sweeps, feature test, retrieval -------------------------------------------- */
 int dboa_sgd_update(const float* p, const float* g, float* out, float lr, long long n, dboa_stream_t stream);   /* l2l maml_update */
 /* Adam + EMA teacher (base_adaptor.py:126,193-201) with the arithmetic of torch's single-tensor Adam: the fp32 scalars of
@@ -318,6 +338,16 @@ int dboa_adam_scalars(float* out, double lr, double beta1, double beta2, double 
  * arithmetic, bit for bit */
 int dboa_adam_ema_dev(float* p, const float* g, float* m, float* v, float* teacher /* or NULL */, long long n, const float* scalars,
                       dboa_stream_t stream);
+/* Per-video sweeps (see "per-video hyperparameters" above): `groups` arenas of n floats each (n % 4 == 0, else
+ * DBOA_ERR_SHAPE), of which only the videos whose bit is set in `active` take part -- the floats of the others are neither read
+ * nor written, and the grid covers the active videos only.  dboa_sgd_update_groups: lr (groups,), video g's step is
+ * dboa_sgd_update with lr[g].  dboa_adam_ema_groups: scalars (groups, DBOA_ADAM_SCALARS), row g written by dboa_adam_scalars
+ * from video g's lr, betas, eps, step count and alpha; video g's sweep is dboa_adam_ema_dev with that row, so active videos at
+ * different step counts share one launch. */
+int dboa_sgd_update_groups(const float* p, const float* g, float* out, const float* lr, long long n, int groups, unsigned long long active,
+                           dboa_stream_t stream);
+int dboa_adam_ema_groups(float* p, const float* g, float* m, float* v, float* teacher /* or NULL */, long long n, const float* scalars,
+                         int groups, unsigned long long active, dboa_stream_t stream);
 /* stream-ordered fill / device-to-device copy on the copy engine (gradient arenas, frame staging: no ATen kernels in a step) */
 int dboa_fill_zero(void* dst, long long bytes, dboa_stream_t stream);
 int dboa_copy_async(void* dst, const void* src, long long bytes, dboa_stream_t stream);
