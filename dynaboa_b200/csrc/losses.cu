@@ -57,10 +57,12 @@ int project_bwd_launch(const float* cam, const float* j3d, const float* dp2d, fl
 // ---------------------------------------------------------------------------------------------
 // FROM_ROT: input is the (24,3,3) rotation stack, gradient goes to d_rot (B,24,3,3)
 // otherwise : input is the 69-d axis-angle body pose, gradient goes to d_in (B,69)
+// body b belongs to video b / rows and scales its gradient by vs.scale[b / rows] (rows = B: one scale for every body)
+struct VideoScales { float scale[MAX_VIDEOS]; };
 template <bool FROM_ROT>
-__device__ __forceinline__ void pose_prior_body(const float* __restrict__ in, const float* __restrict__ means, const float* __restrict__ prec,
-                                                const float* __restrict__ neg_log_w, float* __restrict__ prior_b, float* __restrict__ d_in,
-                                                float scale) {
+__global__ void __launch_bounds__(256) pose_prior_kernel(const float* __restrict__ in, const float* __restrict__ means,
+                                                         const float* __restrict__ prec, const float* __restrict__ neg_log_w,
+                                                         float* __restrict__ prior_b, float* __restrict__ d_in, int rows, const VideoScales vs) {
     pdl_wait();
     pdl_trigger();
     __shared__ float sx[69], sd[8][69], sPd[8][69], sg[8][69], sll[8];
@@ -125,6 +127,7 @@ __device__ __forceinline__ void pose_prior_body(const float* __restrict__ in, co
     }
     __syncthreads();
     if (d_in != nullptr) {
+        const float scale = vs.scale[b / rows];
         if (FROM_ROT) {
             if (t < 9) d_in[(size_t)b * 216 + t] = 0.f;            // root joint carries no prior
             if (t < 23) {
@@ -140,33 +143,24 @@ __device__ __forceinline__ void pose_prior_body(const float* __restrict__ in, co
     }
 }
 template <bool FROM_ROT>
-__global__ void __launch_bounds__(256) pose_prior_kernel(const float* __restrict__ in, const float* __restrict__ means,
-                                                         const float* __restrict__ prec, const float* __restrict__ neg_log_w,
-                                                         float* __restrict__ prior_b, float* __restrict__ d_in, float scale) {
-    pose_prior_body<FROM_ROT>(in, means, prec, neg_log_w, prior_b, d_in, scale);
-}
-// per-video scale: body b belongs to video b / rows and scales its gradient by t.scale[video]
-struct VideoScales { float scale[MAX_VIDEOS]; };
-__global__ void __launch_bounds__(256) pose_prior_groups_kernel(const float* __restrict__ in, const float* __restrict__ means,
-                                                                const float* __restrict__ prec, const float* __restrict__ neg_log_w,
-                                                                float* __restrict__ prior_b, float* __restrict__ d_in, int rows,
-                                                                const VideoScales t) {
-    pose_prior_body<true>(in, means, prec, neg_log_w, prior_b, d_in, t.scale[blockIdx.x / rows]);
+static int prior_launch(const float* in, const float* means, const float* prec, const float* neg_log_w, float* prior_b, float* d_in,
+                        const float* scale, int B, int groups, cudaStream_t st) {
+    VideoScales t;
+    for (int g = 0; g < groups; ++g) t.scale[g] = scale[g];
+    return launch_ex(pose_prior_kernel<FROM_ROT>, dim3(B), dim3(256), 0, st, dim3(1, 1, 1), true, in, means, prec, neg_log_w, prior_b, d_in,
+                     B / groups, t);
 }
 int pose_prior_launch(const float* rot, const float* means, const float* prec, const float* neg_log_w, float* prior_b, float* drot,
                       float scale, int B, cudaStream_t st) {
-    return launch_ex(pose_prior_kernel<true>, dim3(B), dim3(256), 0, st, dim3(1, 1, 1), true, rot, means, prec, neg_log_w, prior_b, drot, scale);
+    return prior_launch<true>(rot, means, prec, neg_log_w, prior_b, drot, &scale, B, 1, st);
 }
 int pose_prior_groups_launch(const float* rot, const float* means, const float* prec, const float* neg_log_w, float* prior_b, float* drot,
                              const float* scale, int B, int groups, cudaStream_t st) {
-    VideoScales t;
-    for (int g = 0; g < groups; ++g) t.scale[g] = scale[g];
-    return launch_ex(pose_prior_groups_kernel, dim3(B), dim3(256), 0, st, dim3(1, 1, 1), true, rot, means, prec, neg_log_w, prior_b, drot,
-                     B / groups, t);
+    return prior_launch<true>(rot, means, prec, neg_log_w, prior_b, drot, scale, B, groups, st);
 }
 int gmm_prior_launch(const float* pose69, const float* means, const float* prec, const float* neg_log_w, float* prior_b, float* dpose,
                      float scale, int B, cudaStream_t st) {
-    return launch_ex(pose_prior_kernel<false>, dim3(B), dim3(256), 0, st, dim3(1, 1, 1), true, pose69, means, prec, neg_log_w, prior_b, dpose, scale);
+    return prior_launch<false>(pose69, means, prec, neg_log_w, prior_b, dpose, &scale, B, 1, st);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -174,10 +168,14 @@ int gmm_prior_launch(const float* pose69, const float* means, const float* prec,
 // terms: 0 s2d(masked, joints 25..48)  1 shape prior  2 pose prior (value only, from prior_b)
 //        3 target p2d MSE  4 target j3d MSE  5 target beta MSE  6 target R MSE  7 hip-centred 3D
 // ---------------------------------------------------------------------------------------------
-// grouped (a.groups > 1): block g computes video g's terms on its own rows
-// w(k): weight k of the block's video
-template <class W>
-__device__ __forceinline__ void loss_multi_body(LossArgs& a, const W& w) {
+// grouped (a.groups > 1): block g computes video g's terms on its own rows, with the weights of row g * stride of vw.w (stride 0:
+// row 0 for every video).  With __launch_bounds__(256) alone ptxas spills here (sm_90a, CUDA 12.9: 79 registers, 8 bytes stack
+// frame, 8 bytes spill stores); with a minimum of one block per SM it keeps every value in registers (82 registers, no stack
+// frame).  One block per video never needs more residency than that.
+struct VideoWeights { float w[MAX_VIDEOS][8]; };
+__global__ void __launch_bounds__(256, 1) loss_multi_weights_kernel(LossArgs a, int stride, const VideoWeights vw) {
+    const int row = blockIdx.x * stride;
+    auto w = [&](int k) { return vw.w[row][k]; };               // weight k of the block's video
     pdl_wait();
     pdl_trigger();
     __shared__ float red[32];
@@ -289,34 +287,25 @@ __device__ __forceinline__ void loss_multi_body(LossArgs& a, const W& w) {
         a.terms[8] = total;
     }
 }
-__global__ void __launch_bounds__(256) loss_multi_kernel(LossArgs a) {
-    loss_multi_body(a, [&](int k) { return a.w[k]; });
-}
-// per-video weights: block g reads t.w[g] in place of a.w.  With __launch_bounds__(256) alone ptxas spills here (sm_90a, CUDA
-// 12.9: 79 registers, 8 bytes stack frame, 8 bytes spill stores); with a minimum of one block per SM it keeps every value in
-// registers (84 registers, no stack frame).  One block per video never needs more residency than that.
-struct VideoWeights { float w[MAX_VIDEOS][8]; };
-__global__ void __launch_bounds__(256, 1) loss_multi_weights_kernel(LossArgs a, const VideoWeights t) {
-    loss_multi_body(a, [&](int k) { return t.w[blockIdx.x][k]; });
-}
 static int loss_multi_check(const LossArgs& a) {
     const int groups = a.groups > 1 ? a.groups : 1;
     if (a.B < 1 || a.B > 256 * groups || a.groups < 0 || a.B % groups != 0) return DBOA_ERR_SHAPE;
     if (a.kp_count < 0 || a.kp_first < 0 || a.kp_first + a.kp_count > 49) return DBOA_ERR_ARG;
     return DBOA_OK;
 }
-int loss_multi_launch(const LossArgs& a, cudaStream_t st) {
+// w: one row of 8 weights per video (stride 1) or one row for every video (stride 0)
+static int loss_multi_rows(const LossArgs& a, const float* w, int stride, cudaStream_t st) {
     DBOA_TRY(loss_multi_check(a));
-    return launch_ex(loss_multi_kernel, dim3(a.groups > 1 ? a.groups : 1), dim3(256), 0, st, dim3(1, 1, 1), true, a);
-}
-int loss_multi_weights_launch(const LossArgs& a, const float* w, cudaStream_t st) {
     const int groups = a.groups > 1 ? a.groups : 1;
-    if (groups > MAX_VIDEOS) return DBOA_ERR_SHAPE;
-    DBOA_TRY(loss_multi_check(a));
     VideoWeights t;
-    for (int g = 0; g < groups; ++g)
+    for (int g = 0; g < (stride ? groups : 1); ++g)
         for (int k = 0; k < 8; ++k) t.w[g][k] = w[g * 8 + k];
-    return launch_ex(loss_multi_weights_kernel, dim3(groups), dim3(256), 0, st, dim3(1, 1, 1), true, a, t);
+    return launch_ex(loss_multi_weights_kernel, dim3(groups), dim3(256), 0, st, dim3(1, 1, 1), true, a, stride, t);
+}
+int loss_multi_launch(const LossArgs& a, cudaStream_t st) { return loss_multi_rows(a, a.w, 0, st); }
+int loss_multi_weights_launch(const LossArgs& a, const float* w, cudaStream_t st) {
+    if ((a.groups > 1 ? a.groups : 1) > MAX_VIDEOS) return DBOA_ERR_SHAPE;
+    return loss_multi_rows(a, w, 1, st);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -324,9 +313,13 @@ int loss_multi_weights_launch(const LossArgs& a, const float* w, cudaStream_t st
 //   L = mean_{B*count*2} [conf_a + conf_h == 2] * ((pa - ph) - (ka - kh))^2   on joints [first, first + count)  (benchmark: 25..48)
 // A video whose `active` bit is clear gets term 0 and leaves its rows of dpa and dph untouched.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void loss_motion_body(const float* __restrict__ pa, const float* __restrict__ ph, const float* __restrict__ ka,
-                                                 const float* __restrict__ kh, float w, float* __restrict__ term, float* __restrict__ dpa,
-                                                 float* __restrict__ dph, int B, int acc_a, int first, int count, unsigned long long active) {
+// Block g weighs its gradient with vs.scale[g * stride] (stride 0: one weight for every video).
+__global__ void __launch_bounds__(256) loss_motion_weights_kernel(const float* __restrict__ pa, const float* __restrict__ ph,
+                                                                  const float* __restrict__ ka, const float* __restrict__ kh,
+                                                                  float* __restrict__ term, float* __restrict__ dpa, float* __restrict__ dph,
+                                                                  int B, int acc_a, int first, int count, unsigned long long active,
+                                                                  int stride, const VideoScales vs) {
+    const float w = vs.scale[blockIdx.x * stride];
     pdl_wait();
     pdl_trigger();
     __shared__ float red[32];
@@ -357,35 +350,25 @@ __device__ __forceinline__ void loss_motion_body(const float* __restrict__ pa, c
     acc = block_sum(acc, red);
     if (threadIdx.x == 0) term[0] = acc / n;
 }
-__global__ void __launch_bounds__(256) loss_motion_kernel(const float* __restrict__ pa, const float* __restrict__ ph,
-                                                          const float* __restrict__ ka, const float* __restrict__ kh, float w,
-                                                          float* __restrict__ term, float* __restrict__ dpa, float* __restrict__ dph,
-                                                          int B, int acc_a, int first, int count, unsigned long long active) {
-    loss_motion_body(pa, ph, ka, kh, w, term, dpa, dph, B, acc_a, first, count, active);
-}
-// per-video weight: block g weighs its gradient with t.scale[g]
-__global__ void __launch_bounds__(256) loss_motion_weights_kernel(const float* __restrict__ pa, const float* __restrict__ ph,
-                                                                  const float* __restrict__ ka, const float* __restrict__ kh,
-                                                                  float* __restrict__ term, float* __restrict__ dpa, float* __restrict__ dph,
-                                                                  int B, int acc_a, int first, int count, unsigned long long active,
-                                                                  const VideoScales t) {
-    loss_motion_body(pa, ph, ka, kh, t.scale[blockIdx.x], term, dpa, dph, B, acc_a, first, count, active);
+// w: `groups` weights (stride 1) or one for every video (stride 0)
+static int loss_motion_rows(const float* pa, const float* ph, const float* ka, const float* kh, const float* w, int stride, float* term,
+                            float* dpa, float* dph, int B, int acc_a, int first, int count, cudaStream_t st, int groups,
+                            unsigned long long active) {
+    if (first < 0 || count < 1 || first + count > 49) return DBOA_ERR_ARG;
+    if (groups < 1 || B % groups != 0) return DBOA_ERR_SHAPE;
+    VideoScales t;
+    for (int g = 0; g < (stride ? groups : 1); ++g) t.scale[g] = w[g];
+    return launch_ex(loss_motion_weights_kernel, dim3(groups), dim3(256), 0, st, dim3(1, 1, 1), true, pa, ph, ka, kh, term, dpa, dph, B, acc_a,
+                     first, count, active, stride, t);
 }
 int loss_motion_weights_launch(const float* pa, const float* ph, const float* ka, const float* kh, const float* w, float* term, float* dpa,
                                float* dph, int B, int acc_a, int first, int count, cudaStream_t st, int groups, unsigned long long active) {
-    if (first < 0 || count < 1 || first + count > 49) return DBOA_ERR_ARG;
-    if (groups < 1 || groups > MAX_VIDEOS || B % groups != 0) return DBOA_ERR_SHAPE;
-    VideoScales t;
-    for (int g = 0; g < groups; ++g) t.scale[g] = w[g];
-    return launch_ex(loss_motion_weights_kernel, dim3(groups), dim3(256), 0, st, dim3(1, 1, 1), true, pa, ph, ka, kh, term, dpa, dph, B, acc_a,
-                     first, count, active, t);
+    if (groups > MAX_VIDEOS) return DBOA_ERR_SHAPE;
+    return loss_motion_rows(pa, ph, ka, kh, w, 1, term, dpa, dph, B, acc_a, first, count, st, groups, active);
 }
 int loss_motion_launch(const float* pa, const float* ph, const float* ka, const float* kh, float w, float* term, float* dpa, float* dph,
                        int B, int acc_a, int first, int count, cudaStream_t st, int groups, unsigned long long active) {
-    if (first < 0 || count < 1 || first + count > 49) return DBOA_ERR_ARG;
-    if (groups < 1 || B % groups != 0) return DBOA_ERR_SHAPE;
-    return launch_ex(loss_motion_kernel, dim3(groups), dim3(256), 0, st, dim3(1, 1, 1), true, pa, ph, ka, kh, w, term, dpa, dph, B, acc_a, first,
-                     count, active);
+    return loss_motion_rows(pa, ph, ka, kh, &w, 0, term, dpa, dph, B, acc_a, first, count, st, groups, active);
 }
 
 }  // namespace dboa

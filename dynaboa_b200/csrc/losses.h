@@ -19,7 +19,8 @@ int loss_motion_launch(const float* pa, const float* ph, const float* ka, const 
                        int B, int acc_a, int first, int count, cudaStream_t st, int groups = 1, unsigned long long active = ~0ULL);
 // Per-video scalars for `groups` (1..64) videos of B / groups rows each, passed as HOST arrays and sent with the launch:
 // scale (groups,) of the pose prior, w (groups, 8) of the loss head (block g uses row g for a.w), w (groups,) of the motion term.
-// Video g's outputs are bit-identical to the uniform launch on its rows with its scalars.
+// The uniform launches above are the same kernels with one row for every video; video g's outputs are bit-identical to a uniform
+// launch on its rows with its scalars.
 int pose_prior_groups_launch(const float* rot, const float* means, const float* prec, const float* neg_log_w, float* prior_b, float* drot,
                              const float* scale, int B, int groups, cudaStream_t st);
 int loss_multi_weights_launch(const LossArgs& a, const float* w, cudaStream_t st);

@@ -18,23 +18,6 @@ static inline int sweep_grid(size_t n4) {
     return (int)(blocks < cap ? (blocks ? blocks : 1) : cap);
 }
 
-// float4 i of one SGD step, shared by the one-arena and the per-video kernels
-__device__ __forceinline__ void sgd_at(const float* __restrict__ p, const float* __restrict__ g, float* __restrict__ out, float neg_lr, size_t i) {
-    float4 a = reinterpret_cast<const float4*>(p)[i], b = reinterpret_cast<const float4*>(g)[i], o;
-    o.x = __fadd_rn(a.x, __fmul_rn(neg_lr, b.x)); o.y = __fadd_rn(a.y, __fmul_rn(neg_lr, b.y));
-    o.z = __fadd_rn(a.z, __fmul_rn(neg_lr, b.z)); o.w = __fadd_rn(a.w, __fmul_rn(neg_lr, b.w));
-    reinterpret_cast<float4*>(out)[i] = o;
-}
-__global__ void __launch_bounds__(256) sgd_update_kernel(const float* __restrict__ p, const float* __restrict__ g, float* __restrict__ out,
-                                                         float neg_lr, size_t n4) {
-    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n4; i += (size_t)gridDim.x * 256) sgd_at(p, g, out, neg_lr, i);
-}
-int sgd_update(const float* p, const float* g, float* out, float lr, size_t n, cudaStream_t st) {
-    if (n % 4) return DBOA_ERR_SHAPE;
-    sgd_update_kernel<<<sweep_grid(n / 4), 256, 0, st>>>(p, g, out, -lr, n / 4);
-    return check_launch();
-}
-
 __device__ __forceinline__ void adam_one(float& p, float g, float& m, float& v, float w1, float b2, float one_m_b2, float bc2_sqrt,
                                          float eps, float neg_step) {
     // exp_avg.lerp_(grad, 1 - beta1): ATen evaluates  w < 0.5 ? a + w (b - a) : b - (b - a)(1 - w)
@@ -68,31 +51,21 @@ __device__ __forceinline__ void adam_ema_at(float* __restrict__ p, const float* 
         reinterpret_cast<float4*>(teacher)[i] = tt;
     }
 }
-// one grid-stride Adam (+ EMA) sweep over one arena
-__device__ __forceinline__ void adam_ema_sweep(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                                               float* __restrict__ teacher, size_t n4, float w1, float b2, float one_m_b2, float bc2_sqrt,
-                                               float eps, float neg_step, float alpha, float one_m_alpha, float gscale) {
-    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n4; i += (size_t)gridDim.x * 256)
-        adam_ema_at(p, g, m, v, teacher, i, w1, b2, one_m_b2, bc2_sqrt, eps, neg_step, alpha, one_m_alpha, gscale);
-}
-__global__ void __launch_bounds__(256) adam_ema_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                                                       float* __restrict__ v, float* __restrict__ teacher, size_t n4, float w1, float b2,
-                                                       float one_m_b2, float bc2_sqrt, float eps, float neg_step, float alpha,
-                                                       float one_m_alpha, float gscale) {
-    adam_ema_sweep(p, g, m, v, teacher, n4, w1, b2, one_m_b2, bc2_sqrt, eps, neg_step, alpha, one_m_alpha, gscale);
-}
 // the scalars from a device block (adam_scalars' order): a replayed CUDA graph reads the bias correction of the current step
 __global__ void __launch_bounds__(256) adam_ema_dev_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                                            float* __restrict__ v, float* __restrict__ teacher, size_t n4,
                                                            const float* __restrict__ s) {
-    adam_ema_sweep(p, g, m, v, teacher, n4, s[0], s[1], s[2], s[3], s[4], s[5], s[6], s[7], s[8]);
+    const float w1 = s[0], b2 = s[1], one_m_b2 = s[2], bc2_sqrt = s[3], eps = s[4], neg_step = s[5], alpha = s[6], one_m_alpha = s[7],
+                gscale = s[8];
+    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n4; i += (size_t)gridDim.x * 256)
+        adam_ema_at(p, g, m, v, teacher, i, w1, b2, one_m_b2, bc2_sqrt, eps, neg_step, alpha, one_m_alpha, gscale);
 }
 
 // ---------------------------------------------------------------------------------------------
 // per-video sweeps: video g owns the float4s [g n4, (g + 1) n4) of every arena and has its own scalars, which travel in the
-// launch parameters (no device table).  The grid strides over the active videos' float4s as over one arena of nact * n4
-// float4s, with the one-arena sweep's grid: step j of the walk is float4 j % n4 of the (j / n4)-th active video (t.video), the
-// pair advanced by subtraction rather than division.
+// launch parameters (no device table); a one-arena call is one video.  The grid strides over the active videos' float4s as
+// over one arena of nact * n4 float4s, with the one-arena sweep's grid: step j of the walk is float4 j % n4 of the (j / n4)-th
+// active video (t.video), the pair advanced by subtraction rather than division.
 // ---------------------------------------------------------------------------------------------
 struct VideoSweep {
     float s[MAX_VIDEOS][ADAM_SCALARS];      // SGD: s[g][0] = -lr of video g; Adam: dboa_adam_scalars' row of video g
@@ -125,7 +98,17 @@ __device__ __forceinline__ void video_walk(size_t n4, int nact, const VideoSweep
 
 __global__ void __launch_bounds__(256) sgd_update_groups_kernel(const float* __restrict__ p, const float* __restrict__ g, float* __restrict__ out,
                                                                 size_t n4, int nact, const VideoSweep t) {
-    video_walk(n4, nact, t, [&](int v, size_t i) { sgd_at(p, g, out, t.s[v][0], i); });
+    video_walk(n4, nact, t, [&](int v, size_t i) {
+        const float neg_lr = t.s[v][0];
+        float4 a = reinterpret_cast<const float4*>(p)[i], b = reinterpret_cast<const float4*>(g)[i], o;
+        o.x = __fadd_rn(a.x, __fmul_rn(neg_lr, b.x)); o.y = __fadd_rn(a.y, __fmul_rn(neg_lr, b.y));
+        o.z = __fadd_rn(a.z, __fmul_rn(neg_lr, b.z)); o.w = __fadd_rn(a.w, __fmul_rn(neg_lr, b.w));
+        reinterpret_cast<float4*>(out)[i] = o;
+    });
+}
+int sgd_update(const float* p, const float* g, float* out, float lr, size_t n, cudaStream_t st) {
+    if (n % 4) return DBOA_ERR_SHAPE;
+    return sgd_update_groups(p, g, out, &lr, n, 1, 1ULL, st);
 }
 int sgd_update_groups(const float* p, const float* g, float* out, const float* lr, size_t n, int groups, unsigned long long active,
                       cudaStream_t st) {
@@ -156,8 +139,7 @@ int adam_ema(float* p, const float* g, float* m, float* v, float* teacher, size_
     if (n % 4 || step < 1) return DBOA_ERR_ARG;
     float s[ADAM_SCALARS];
     adam_scalars(lr, beta1, beta2, eps, step, alpha, gscale, s);
-    adam_ema_kernel<<<sweep_grid(n / 4), 256, 0, st>>>(p, g, m, v, teacher, n / 4, s[0], s[1], s[2], s[3], s[4], s[5], s[6], s[7], s[8]);
-    return check_launch();
+    return adam_ema_groups(p, g, m, v, teacher, n, s, 1, 1ULL, st);
 }
 int adam_ema_dev(float* p, const float* g, float* m, float* v, float* teacher, size_t n, const float* scalars, cudaStream_t st) {
     if (n % 4) return DBOA_ERR_ARG;

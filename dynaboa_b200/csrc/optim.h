@@ -27,8 +27,8 @@ void adam_scalars(double lr, double beta1, double beta2, double eps, int step, d
 int adam_ema_dev(float* p, const float* g, float* m, float* v, float* teacher, size_t n, const float* scalars, cudaStream_t st);
 // Per-video sweeps over `groups` (1..64) arenas of n floats each, only the videos whose bit is set in `active` (others: not read,
 // not written).  lr: host (groups,) array, video g's learning rate; scalars: host (groups, ADAM_SCALARS) array, video g's row of
-// adam_scalars.  Video g's floats are bit-identical to sgd_update / adam_ema_dev over its arenas with its scalars.  The
-// caller checks the arguments (n % 4 == 0, groups, active).
+// adam_scalars.  sgd_update and adam_ema are these sweeps over one video; video g's floats are bit-identical to adam_ema_dev over
+// its arenas with its scalars.  The caller checks the arguments (n % 4 == 0, groups, active).
 int sgd_update_groups(const float* p, const float* g, float* out, const float* lr, size_t n, int groups, unsigned long long active,
                       cudaStream_t st);
 int adam_ema_groups(float* p, const float* g, float* m, float* v, float* teacher, size_t n, const float* scalars, int groups,

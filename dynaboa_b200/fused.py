@@ -19,7 +19,6 @@ call) and callbacks for what stays with the adaptor.  A set of videos is an int 
 """
 import collections
 import ctypes as C
-from types import SimpleNamespace
 
 import torch
 
@@ -44,20 +43,20 @@ class Step:
     per-video generators; ``save_hist(image, kp, mask)`` / ``get_hist(live)``: the history frames; ``adam(mask, teacher=None,
     alpha=0.0)``: Adam (+ EMA into ``teacher``) of the videos in ``mask``; ``evaluate(batch, arena, mask, inner)``: one
     evaluation of ``arena`` (``inner``: the inner step of fast weights, None for theta); ``reduce_terms(terms)``: the
-    data-parallel sum of the feature test's sums (None: one rank); ``hparams``: per video, a dict of the options it sets for
-    itself (``multivideo.PER_VIDEO``; None: every video runs with ``options``).  Set per frame: ``eval_mode`` ('none', 'final',
-    'all'), ``grad_sync`` (the data-parallel ``BucketedGradSync`` or None) and ``phase_events`` (a list: CUDA events per phase);
-    ``fused_adapt`` sets ``hp`` (``frame_options``)."""
+    data-parallel sum of the feature test's sums (None: one rank); ``video_options``: G option namespaces, video g's learning
+    rates, loss weights and dynamic-loop test (``multivideo.PER_VIDEO``) read from the g-th (default: ``options`` for every
+    video; a pool sets them per frame).  Set per frame: ``eval_mode`` ('none', 'final', 'all'), ``grad_sync`` (the
+    data-parallel ``BucketedGradSync`` or None) and ``phase_events`` (a list: CUDA events per phase)."""
 
     def __init__(self, options, G, theta, grad, buffers, smpl_neutral, gmm_f, teacher=None, teacher_buffers=None, teacher_masks=None,
                  kp_range=(25, 24), motion_lead=0, bank=None, rngs=None, save_hist=None, get_hist=None, adam=None, evaluate=None,
-                 reduce_terms=None, hparams=None):
+                 reduce_terms=None, video_options=None):
         self.options, self.G, self.theta, self.grad, self.buffers, self.smpl_neutral, self.gmm_f = options, G, theta, grad, buffers, smpl_neutral, gmm_f
         self.teacher, self.teacher_buffers, self.teacher_masks = teacher, teacher_buffers, teacher_masks
         self.kp_range, self.motion_lead, self.bank, self.rngs = kp_range, motion_lead, bank, rngs
         self.save_hist, self.get_hist, self.adam, self.evaluate, self.reduce_terms = save_hist, get_hist, adam, evaluate, reduce_terms
         self.eval_mode, self.grad_sync, self.phase_events = 'none', None, None
-        self.hparams, self.hp = hparams, None
+        self.video_options = [options] * G if video_options is None else video_options
         self._motion_w = None                   # (values, device tensor) of _motion_weights
         # the step's scratch: motion pair images and gradients, cosine partial sums, fast weights, inner gradient, cluster index
         self._pair = self._bgrad_flat = self._cos_partial = self._fast = self._inner_grad = None
@@ -92,21 +91,14 @@ def merge(old, new, mask, G):
     return out
 
 
-def frame_options(s, mask):
-    """The one choice of a frame between the uniform and the per-video calls: None when no video in ``mask`` carries a value
-    of its own that differs from ``options`` (the step issues exactly the uniform calls), else the G effective option
-    namespaces (``options`` for the videos outside ``mask``)."""
-    o, hps = s.options, s.hparams
-    on = [g for g in range(s.G) if (mask >> g) & 1]
-    if hps is None or not any(v != getattr(o, k, None) for g in on for k, v in hps[g].items()):
-        return None
-    return [SimpleNamespace(**{**vars(o), **hps[g]}) if g in on else o for g in range(s.G)]
-
-
 def _motion_weights(s, device):
-    """(G,) fp32 device tensor of every video's own ``motionloss_weight``: the fp32 value the scalar product of the uniform path
-    rounds its Python float to.  Uploaded again only when a video's value changes (``start``), so a frame makes no copy."""
-    key = tuple(float(h.get('motionloss_weight', s.options.motionloss_weight)) for h in s.hparams)
+    """Every video's ``motionloss_weight`` as a factor of the (G,) motion term: the one float all videos share, or else a (G,)
+    fp32 device tensor of the fp32 values a float factor rounds to (the same products).  The tensor is uploaded again only when
+    a video's value changes (``start``), so a frame makes no copy, and a captured single-video frame holds no host-written
+    tensor."""
+    key = tuple(float(q.motionloss_weight) for q in s.video_options)
+    if len(set(key)) == 1:
+        return key[0]
     if s._motion_w is None or s._motion_w[0] != key or s._motion_w[1].device != device:
         s._motion_w = (key, torch.tensor(key, dtype=torch.float32, device=device))
     return s._motion_w[1]
@@ -169,9 +161,8 @@ def forward_graph(s, arena, buffers, image, mask, masks=None):
 
 def _loss_head(s, p, w, kp=None, t_p2d=None, t_j3d=None, t_beta=None, t_R=None, gt_s3d=None, grads=None, nb=None):
     """Runs the (optional) pose prior and the multi-term head on the first ``nb`` samples of ``p``, each video's rows on their
-    own (per-video means and gradient scaling); returns (terms (G, 9), dp2d, dj3d, dR, dbeta).  ``w``: the 8 weights, or one
-    row of 8 per video (the per-video calls).  ``grads``: preallocated (possibly larger-batch) gradient buffers whose leading
-    ``nb`` rows are written."""
+    own (per-video means and gradient scaling); returns (terms (G, 9), dp2d, dj3d, dR, dbeta).  ``w``: one row of 8 weights
+    per video, or one row of 8 for every video.  ``grads``: preallocated (possibly larger-batch) gradient buffers whose leading ``nb`` rows are written."""
     B, dev, G = (p.B if nb is None else nb), p.rot.device, p.groups
     if grads is None:
         dp2d, dj3d = torch.empty_like(p.p2d), torch.empty_like(p.joints)
@@ -179,16 +170,14 @@ def _loss_head(s, p, w, kp=None, t_p2d=None, t_j3d=None, t_beta=None, t_R=None, 
     else:
         dp2d, dj3d, dR, dbeta = grads
     terms = torch.empty(G, 9, dtype=torch.float32, device=dev)
-    prior_b, rows = None, isinstance(w[0], (list, tuple))
-    if (any(r[2] != 0.0 for r in w) if rows else w[2] != 0.0):
+    if not isinstance(w[0], (list, tuple)):
+        w = [w] * G
+    prior_b = None
+    if any(r[2] != 0.0 for r in w):
         prior_b = torch.empty(B, dtype=torch.float32, device=dev)
         g = s.gmm_f
-        if rows:
-            _lib.call('dboa_pose_prior_groups', ptr(p.rot), ptr(g.means), ptr(g.precisions), ptr(g.neg_log_weights), ptr(prior_b), ptr(dR),
-                      (C.c_float * G)(*[float(r[2]) / (B // G) for r in w]), B, G, stream())
-        else:
-            _lib.call('dboa_pose_prior', ptr(p.rot), ptr(g.means), ptr(g.precisions), ptr(g.neg_log_weights), ptr(prior_b), ptr(dR),
-                      float(w[2]) / (B // G), B, stream())                   # per-video mean: scale w / b
+        _lib.call('dboa_pose_prior_groups', ptr(p.rot), ptr(g.means), ptr(g.precisions), ptr(g.neg_log_weights), ptr(prior_b), ptr(dR),
+                  (C.c_float * G)(*[float(r[2]) / (B // G) for r in w]), B, G, stream())     # per-video mean: scale w / b
     a = _lib.LossArgsStruct()
     a.B, a.groups = B, G
     keep = []
@@ -201,12 +190,7 @@ def _loss_head(s, p, w, kp=None, t_p2d=None, t_j3d=None, t_beta=None, t_R=None, 
         setattr(a, name, None if t is None else t.data_ptr())
     a.dR_accumulate = 1 if prior_b is not None else 0
     a.kp_first, a.kp_count = s.kp_range                             # joints of the re-projection term (webcam client: (0, 25))
-    if rows:
-        _lib.call('dboa_loss_multi_weights', C.byref(a), (C.c_float * (8 * G))(*[float(x) for r in w for x in r]), stream())
-    else:
-        for i in range(8):
-            a.w[i] = float(w[i])
-        _lib.call('dboa_loss_multi', C.byref(a), stream())
+    _lib.call('dboa_loss_multi_weights', C.byref(a), (C.c_float * (8 * G))(*[float(x) for r in w for x in r]), stream())
     return terms, dp2d, dj3d, dR, dbeta
 
 
@@ -258,7 +242,7 @@ def level_backward(s, out, arena, image, kp, lower, grad_arena, mask, live, main
     With one video, when the motion loss is live and no forward is supplied, the current and the history frame go through
     ONE batched forward / backward (same weights, independent samples), and the teacher forward runs on a side stream.
     With several, the history frame gets its own grouped pass and the teacher runs on the caller's stream."""
-    o, G, hp = s.options, s.G, s.hp
+    o, G, vo = s.options, s.G, s.video_options
     tag = 'll' if lower else 'ul'
     nb = image.shape[0]
     use_frame = o.use_frame_losses_lower if lower else o.use_frame_losses_upper
@@ -316,7 +300,7 @@ def level_backward(s, out, arena, image, kp, lower, grad_arena, mask, live, main
         flat = s._bgrad_flat
         _zero(flat)
         grads = tuple(t.view(Bm, *sh) for t, sh in zip(flat.split(sizes), ((49, 2), (49, 3), (24, 3, 3), (10,))))
-    w = head_weights(o) if hp is None else [head_weights(q) for q in hp]
+    w = [head_weights(q) for q in vo]
     terms, dp2d, dj3d, dR, dbeta = _loss_head(s, main, w, kp=kp if use_frame else None, grads=grads, nb=nb, **targets)
     total = terms[:, 8]
     if use_frame:
@@ -328,19 +312,12 @@ def level_backward(s, out, arena, image, kp, lower, grad_arena, mask, live, main
         p_hist = main.p2d[nb:] if batched else hist.p2d
         dph = dp2d[nb:] if batched else torch.empty_like(hist.p2d)
         kf, kn = s.kp_range
-        if hp is None:
-            mw, entry = float(o.motionloss_weight), 'dboa_loss_motion_active'
-        else:
-            mw, entry = (C.c_float * G)(*[q.motionloss_weight for q in hp]), 'dboa_loss_motion_weights'
-        margs = (ptr(main.p2d), ptr(p_hist), ptr(kp), ptr(hist_kp.contiguous()), mw, ptr(mterm), ptr(dp2d), ptr(dph), nb, 1, kf, kn, G)
-        _lib.call(entry, *margs, live, stream())
+        _lib.call('dboa_loss_motion_weights', ptr(main.p2d), ptr(p_hist), ptr(kp), ptr(hist_kp.contiguous()),
+                  (C.c_float * G)(*[q.motionloss_weight for q in vo]), ptr(mterm), ptr(dp2d), ptr(dph), nb, 1, kf, kn, G, live, stream())
         if not batched:
             backward_graph(s, arena, hist, dph, torch.zeros_like(hist.joints), torch.zeros_like(hist.rot), torch.zeros_like(hist.shape),
                            grad_arena)
-        if hp is None:
-            total = total + mterm * o.motionloss_weight
-        else:
-            total = total + mterm * _motion_weights(s, image.device)
+        total = total + mterm * _motion_weights(s, image.device)
         fit['ul/motion_loss'] = mterm
     _mark(s, f'{tag}: loss head')
     mix = bool(o.retrieval and (o.lower_level_mixtrain if lower else o.upper_level_mixtrain))
@@ -356,7 +333,7 @@ def level_backward(s, out, arena, image, kp, lower, grad_arena, mask, live, main
             gt_R = torch.empty(n, 24, 3, 3, dtype=torch.float32, device=image.device)
             _lib.call('dboa_rodrigues', ptr(ex['pose'].reshape(-1, 3).contiguous()), ptr(gt_R), n * 24, 0, stream())
             label = lambda lw: [5 * lw, 0, 0, 0, 0, 0.001 * lw, 1 * lw, 5 * lw]
-            ew = label(o.labelloss_weight) if hp is None else [label(q.labelloss_weight) for q in hp]
+            ew = [label(q.labelloss_weight) for q in vo]
             eterms, a, b, c, d = _loss_head(s, e, ew, kp=ex['keypoints'], t_beta=ex['betas'], t_R=gt_R, gt_s3d=ex['pose_3d'])
             backward_graph(s, arena, e, a, b, c, d, grad_arena, sync=sync)
             total = total + eterms[:, 8]
@@ -408,13 +385,13 @@ def feature_test(s, fit, a, b, mask):
     return out
 
 
-def _continuing(o, sims, steps, hp=None):
+def _continuing(o, sims, steps, vo=None):
     """Bit mask of the videos of ``sims`` whose own test says 'continue' and whose trip count ``steps[g]`` (advanced here, as
-    the reference's loop does before its cap test) is still within ``optim_steps``.  ``hp``: the frame's per-video options
-    (``frame_options``; None: ``o`` for every video), whose ``cos_sim_threshold`` and ``optim_steps`` video g uses."""
+    the reference's loop does before its cap test) is still within ``optim_steps``.  Video g's test uses the
+    ``cos_sim_threshold`` and ``optim_steps`` of ``vo[g]`` (the step's ``video_options``; None: ``o`` for every video)."""
     mask = 0
     for g, s in sims.items():
-        q = o if hp is None else hp[g]
+        q = o if vo is None else vo[g]
         if 1 - s[12]['cos'] > q.cos_sim_threshold:
             steps[g] += 1
             if steps[g] <= q.optim_steps:
@@ -427,7 +404,6 @@ def fused_adapt(s, batch, mask, frames):
     SGD steps of the lower level, the upper level, one Adam + EMA teacher sweep, then the optional ``dynamic_boa`` loop.
     ``frames[g]``: the frames video g adapted before this one (its motion term's clock).  Returns the ``Frame``."""
     o, G, theta, buffers, grad = s.options, s.G, s.theta, s.buffers, s.grad
-    s.hp = hp = frame_options(s, mask)                                   # uniform or per-video calls, for the whole frame
     out = Frame(mask)
     image, kp = batch['image'].contiguous().float(), batch['smpl_j2d'].contiguous().float()
     s.save_hist(image, kp, mask)
@@ -453,12 +429,8 @@ def fused_adapt(s, batch, mask, frames):
             level_backward(s, out, fast, image, kp, True, s._inner_grad, mask, live, main=cur if i == 0 else None)
             _mark(s, 'lower level (loss + backward)')
             nxt = s._fast[i % 2]
-            if hp is None:
-                for f, g, n in zip(_active_rows(fast, mask, G), _active_rows(s._inner_grad, mask, G), _active_rows(nxt, mask, G)):
-                    _lib.call('dboa_sgd_update', ptr(f), ptr(g), ptr(n), float(o.fastlr), f.numel(), stream())
-            else:
-                _lib.call('dboa_sgd_update_groups', ptr(fast), ptr(s._inner_grad), ptr(nxt), (C.c_float * G)(*[q.fastlr for q in hp]),
-                          fast.numel() // G, G, mask, stream())
+            lr = (C.c_float * G)(*[q.fastlr for q in s.video_options])
+            _lib.call('dboa_sgd_update_groups', ptr(fast), ptr(s._inner_grad), ptr(nxt), lr, fast.numel() // G, G, mask, stream())
             fast = nxt
             _mark(s, 'inner SGD step')
             if evaluate == 'all':
@@ -477,7 +449,7 @@ def fused_adapt(s, batch, mask, frames):
             after = forward_graph(s, theta, buffers, image, mask)
             sims = feature_test(s, out.fit, probe, after, mask)
             out.sims, out.steps = {g: [x] for g, x in sims.items()}, dict.fromkeys(sims, 0)
-            loop = _continuing(o, sims, out.steps, hp)
+            loop = _continuing(o, sims, out.steps, s.video_options)
             while loop:
                 for t in _active_rows(grad, loop, G):
                     _zero(t)
@@ -490,7 +462,7 @@ def fused_adapt(s, batch, mask, frames):
                     out.sims[g].append(x)
                 if evaluate == 'all':
                     out.result = s.evaluate(batch, theta, loop, None)
-                loop = _continuing(o, sims, out.steps, hp)
+                loop = _continuing(o, sims, out.steps, s.video_options)
             if evaluate == 'final':
                 out.result = s.evaluate(batch, theta, mask, None)
         return out

@@ -22,7 +22,7 @@ import torch
 
 from . import _lib, hmr as hmr_mod, layout, state as state_mod
 from ._lib import ptr, stream
-from .fused import Step, fused_adapt, pick, runs
+from .fused import Step, fused_adapt, pick
 
 EVAL_MODES = ('none', 'final', 'all')
 GT_KEYS = ('pose', 'betas', 'gender')
@@ -188,8 +188,7 @@ class MultiVideoAdaptor:
         self._step = Step(o, G, self.thetas, self.grad, self.buffers, base.smpl_neutral, base.gmm_f, teacher=self.teachers,
                           teacher_buffers=self.buffers, teacher_masks=self._teacher_masks, kp_range=self.kp_range,
                           motion_lead=self.motion_lead, bank=base.bank if o.retrieval else None, rngs=self.rngs,
-                          save_hist=self._save_hist, get_hist=self._get_hist, adam=self._adam_ema, evaluate=self._evaluate,
-                          hparams=self.hparams)
+                          save_hist=self._save_hist, get_hist=self._get_hist, adam=self._adam_ema, evaluate=self._evaluate)
         for g in range(G):
             self.start(g)
 
@@ -303,26 +302,17 @@ class MultiVideoAdaptor:
         return torch.cat(per, 2)
 
     def _adam_ema(self, on, teacher=None, alpha=0.0):
-        """Adam + EMA into the teacher stack ``teacher`` of the slots in ``on``, each at its own step count: one sweep per run of
-        consecutive slots that share a step count (one sweep over the whole stack while every slot runs in step).  In a frame
-        of per-video calls (the step's ``hp``), one ``dboa_adam_ema_groups`` sweep with each slot's lr, betas, step count and
-        alpha."""
-        o, hp = self.options, self._step.hp
+        """Adam + EMA into the teacher stack ``teacher`` of the slots in ``on``: one ``dboa_adam_ema_groups`` sweep in which each
+        slot takes its own step count and the lr, betas and alpha of its options in the step (``alpha`` is not read)."""
+        vo = self._step.video_options
+        rows, one = (C.c_float * (self.G * _lib.ADAM_SCALARS))(), (C.c_float * _lib.ADAM_SCALARS)()
         for g in self._slots(on):
             self.step_counts[g] += 1
-        if hp is not None:
-            rows, one = (C.c_float * (self.G * _lib.ADAM_SCALARS))(), (C.c_float * _lib.ADAM_SCALARS)()
-            for g in self._slots(on):
-                q = hp[g]
-                _lib.call('dboa_adam_scalars', one, float(q.lr), float(q.beta1), float(q.beta2), 1e-8, self.step_counts[g], float(q.alpha), 1.0)
-                rows[g * _lib.ADAM_SCALARS:(g + 1) * _lib.ADAM_SCALARS] = one[:]
-            _lib.call('dboa_adam_ema_groups', ptr(self.thetas), ptr(self.grad), ptr(self.m), ptr(self.v), ptr(teacher),
-                      self.thetas.shape[1], rows, self.G, on, stream())
-            return
-        for a, b in runs(on, self.G, key=lambda g: self.step_counts[g]):
-            _lib.call('dboa_adam_ema_scaled', ptr(self.thetas[a:b]), ptr(self.grad[a:b]), ptr(self.m[a:b]), ptr(self.v[a:b]),
-                      ptr(None if teacher is None else teacher[a:b]), self.thetas[a:b].numel(), float(o.lr), float(o.beta1), float(o.beta2), 1e-8,
-                      self.step_counts[a], float(alpha), 1.0, stream())
+            q = vo[g]
+            _lib.call('dboa_adam_scalars', one, float(q.lr), float(q.beta1), float(q.beta2), 1e-8, self.step_counts[g], float(q.alpha), 1.0)
+            rows[g * _lib.ADAM_SCALARS:(g + 1) * _lib.ADAM_SCALARS] = one[:]
+        _lib.call('dboa_adam_ema_groups', ptr(self.thetas), ptr(self.grad), ptr(self.m), ptr(self.v), ptr(teacher),
+                  self.thetas.shape[1], rows, self.G, on, stream())
 
     def _stage(self, batches):
         """Copy the active slots' frames into the persistent (G b, ...) batch; the rows of idle slots keep what they held."""
@@ -377,6 +367,7 @@ class MultiVideoAdaptor:
         o, G = self.options, self.G
         self._evals, self._gt = [], None
         self._step.eval_mode = self.fused_eval
+        self._step.video_options = [self.slot_options(g) if self.hparams[g] else o for g in range(G)]
         f = fused_adapt(self._step, batch, on, self.video_steps)
         self._gt = None
         self.fit_losses, self.kp2dlosses_lower, self.last_upper_loss = slot_records(f, G, self.last_upper_loss)

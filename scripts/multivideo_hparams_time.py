@@ -3,9 +3,8 @@
 (a) frame: for G = 4 and 8, ms per pool frame of a uniform pool (no hparams) and of a pool whose slots all carry different values
     of every PER_VIDEO key, alternated `rounds` times in one run, each window `frames` pool frames between CUDA events after
     `warmup` untimed ones;
-(b) sweep: for G = 4 and 8, the per-video Adam + EMA sweep (dboa_adam_ema_groups, every video at its own step count) against
-    dboa_adam_ema_scaled over the same G * P floats, in GB/s of the 9 x 4 bytes each float moves, from CUDA events over `reps`
-    launches, 2 x `rounds` alternated windows per arm.
+(b) sweep: for G = 4 and 8, the per-video Adam + EMA sweep (dboa_adam_ema_groups, every video at its own step count) over
+    G * P floats, in GB/s of the 9 x 4 bytes each float moves, from CUDA events over `reps` launches, 2 x `rounds` windows.
 
     python scripts/multivideo_hparams_time.py [--frames 12] [--warmup 3] [--rounds 3] [--reps 50] [--out FILE]"""
 import argparse
@@ -83,18 +82,14 @@ def main():
             _lib.call('dboa_adam_scalars', one, 3e-6 * FACTORS[g], 0.5, 0.9, 1e-8, 1 + g, 0.1, 1.0)
             table[g * _lib.ADAM_SCALARS:(g + 1) * _lib.ADAM_SCALARS] = one[:]
         ptrs = [x.data_ptr() for x in t]
-        uniform = lambda i: _lib.call('dboa_adam_ema_scaled', *ptrs, G * P, 3e-6, 0.5, 0.9, 1e-8, 1 + i % 7, 0.1, 1.0, stream())
-        per_video = lambda i: _lib.call('dboa_adam_ema_groups', *ptrs, P, table, G, (1 << G) - 1, stream())
-        for fn in (uniform, per_video):
-            for i in range(5):
-                fn(i)
-        gbs = {'uniform': [], 'per_video': []}
-        for r in range(2 * args.rounds):                                          # alternated windows
-            for name, fn in (('uniform', uniform), ('per_video', per_video)):
-                ms = timed_window(fn, range(args.reps)) / args.reps
-                gbs[name].append(round(9 * 4 * G * P / (ms * 1e-3) / 1e9, 1))
-        row = {'measurement': 'sweep', 'G': G, 'floats': G * P, 'bytes_per_float': 36, 'GB_per_s': gbs,
-               'ratio_of_means': round(sum(gbs['per_video']) / sum(gbs['uniform']), 4)}
+        sweep = lambda i: _lib.call('dboa_adam_ema_groups', *ptrs, P, table, G, (1 << G) - 1, stream())
+        for i in range(5):
+            sweep(i)
+        gbs = []
+        for r in range(2 * args.rounds):
+            ms = timed_window(sweep, range(args.reps)) / args.reps
+            gbs.append(round(9 * 4 * G * P / (ms * 1e-3) / 1e9, 1))
+        row = {'measurement': 'sweep', 'G': G, 'floats': G * P, 'bytes_per_float': 36, 'GB_per_s': gbs}
         print(json.dumps(row), flush=True)
         rows.append(row)
         del t

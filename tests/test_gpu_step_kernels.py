@@ -242,12 +242,11 @@ def test_ema_sweep_bits(L):
 
 @pytest.mark.gpu
 def test_pool_adam_runs(L):
-    """A (G, P) pool stack swept as MultiVideoAdaptor._adam_ema does it: one call per run of consecutive active videos
-    that share a step count.  Each video's rows equal a one-video call at its own step; idle videos keep every bit."""
-    from dynaboa_b200.fused import runs
+    """A (G, P) pool stack swept as MultiVideoAdaptor._adam_ema does it: one dboa_adam_ema_groups call, every active video at
+    its own step count.  Each video's rows equal a one-video call at its own step; idle videos keep every bit."""
     G, P = 6, L.load().dboa_hmr_arena_floats()
     steps = [3, 1, 1, 5, 2, 2]
-    on = 0b110111                                     # video 3 idle; runs [0,1) [1,3) [4,6)
+    on = 0b110111                                     # video 3 idle
     lr, betas, alpha = 3e-6, (0.5, 0.9), 0.1
     stack = [torch.empty(G, P, device='cuda') for _ in range(5)]     # theta, grad, m, v, teacher
     for k in range(G):
@@ -255,11 +254,12 @@ def test_pool_adam_runs(L):
             x[k] = y.cuda()
     stack[4].copy_(stack[0] * 0.999)
     bufs = [Buf(x) for x in stack]
-    th, gr, m, v, t = (b.t.view(G, P) for b in bufs)
-    for a, b in runs(on, G, key=lambda k: steps[k]):
-        L.call('dboa_adam_ema_scaled', C.c_void_p(th[a:b].data_ptr()), C.c_void_p(gr[a:b].data_ptr()), C.c_void_p(m[a:b].data_ptr()),
-               C.c_void_p(v[a:b].data_ptr()), C.c_void_p(t[a:b].data_ptr()), (b - a) * P, lr, betas[0], betas[1], 1e-8, steps[a], alpha,
-               1.0, L.stream())
+    rows, row = (C.c_float * (G * L.ADAM_SCALARS))(), (C.c_float * L.ADAM_SCALARS)()
+    for k in range(G):
+        if (on >> k) & 1:
+            L.call('dboa_adam_scalars', row, lr, betas[0], betas[1], 1e-8, steps[k], alpha, 1.0)
+            rows[k * L.ADAM_SCALARS:(k + 1) * L.ADAM_SCALARS] = row[:]
+    L.call('dboa_adam_ema_groups', *(b.ptr for b in bufs), P, rows, G, on, L.stream())
     got = [b.t.view(G, P) for b in bufs]
     assert all(b.intact() for b in bufs)
     for k in range(G):
