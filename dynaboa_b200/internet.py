@@ -17,7 +17,7 @@ import torch
 
 from . import constants, dataprocess, render as render_mod
 from .adaptor import InternetAdaptor
-from .multivideo import MultiVideoAdaptor, check_hparams, check_options as pool_check_options, video_names
+from .multivideo import MultiVideoAdaptor, check_hparams, check_models, check_options as pool_check_options, video_names
 
 COLOR = (205, 129, 98)       # the mesh colour of BaseAdaptor.save_results, in the order it is given there
 PRED_KEYS = ('verts', 'cam', 'rotmat', 'beta')
@@ -189,7 +189,7 @@ class MultiInternetAdaptor(MultiVideoAdaptor):
                 self.writer.image(png_path, image)
 
     # ------------------------------------------------------------------ videos
-    def run(self, videos, exppath, names=None, checkpoint=None, every=0, hparams=None):
+    def run(self, videos, exppath, names=None, checkpoint=None, every=0, hparams=None, models=None):
         """Adapt every video of ``videos`` (``datasets.InternetVideo``s) through the G slots with ``MultiVideoAdaptor.run``'s
         queue (slots filled in order and refilled as soon as their video ends; video i starts with seed ``options.seed * 1000 +
         i``) and write each video's files under ``exppath/<name>/`` (``names``: default the videos' names).  The frames of
@@ -200,13 +200,16 @@ class MultiInternetAdaptor(MultiVideoAdaptor):
 
         ``checkpoint`` / ``every``: ``MultiVideoAdaptor.run``'s pool checkpoints.  A checkpoint is complete only once every
         ``Pred_<t>`` file of the frames it covers is written; a resumed video is advanced to its frame by index, without
-        decoding the frames before it.  ``hparams``: ``MultiVideoAdaptor.run``'s, one dict (or None) per video."""
+        decoding the frames before it.  ``hparams``: ``MultiVideoAdaptor.run``'s, one dict (or None) per video.  ``models``:
+        ``MultiVideoAdaptor.run``'s, one checkpoint path (or None) per video, read and checked before the first tick; each summary
+        then names its video's (``model``)."""
         videos = list(videos)
         for i, v in enumerate(videos):
             if not callable(getattr(v, 'frame', None)) or not hasattr(v, '__len__') or not hasattr(v, 'name'):
                 raise ValueError(f'video {i} is a {type(v).__name__}, expected an InternetVideo (datasets.internet_videos)')
         names = video_names(videos, names, default=[v.name for v in videos])
         hparams = check_hparams(self.options, hparams, len(videos))
+        models = None if models is None else check_models(models, len(videos))
         if len(set(names)) != len(names):
             raise ValueError(f'two videos would write to one directory: names {names}')
         dirs = ('result',) if getattr(self.options, 'cache_results', 1) else ()
@@ -240,10 +243,12 @@ class MultiInternetAdaptor(MultiVideoAdaptor):
                 out = dict(name=names[i], frames=0 if g is None else self.video_steps[g])
                 if getattr(self.options, 'dynamic_boa', 0):
                     out['optim_step_record'] = [] if g is None else list(self.optim_step_record[g])
+                if models is not None:
+                    out['model'] = models[i]
                 return out
 
             out = self._queue([_Frames(frames_of, i) for i in range(len(videos))], tick, finish, checkpoint=checkpoint, every=every,
-                              items_from=frames_of, barrier=lambda: pending, hparams=hparams)
+                              items_from=frames_of, barrier=lambda: pending, hparams=hparams, models=models)
             for f in pending:
                 f.result()
         return out

@@ -8,11 +8,14 @@ the three ``init_*`` buffers.  The CUDA library holds the same table
 
 ``ArenaLayout`` is that table as the library stores it (offset, logical shape and strides of every
 parameter inside the one flat fp32 arena); ``state_dict`` maps an arena to named tensors with it, the
-mapping ``HMR``'s parameters use, and ``digest`` fingerprints it for saved states (state.py).
+mapping ``HMR``'s parameters use, ``arena_from_state_dict`` maps them back, ``read_checkpoint`` reads and checks a
+checkpoint file into an arena for a pool slot, and ``digest`` fingerprints the table for saved states (state.py).
 """
 import ctypes as C
 import hashlib
 from collections import OrderedDict
+
+import torch
 
 BLOCKS = (3, 4, 6, 3)            # reference model/hmr.py:322  hmr() -> HMR(Bottleneck, [3, 4, 6, 3])
 PLANES = (64, 128, 256, 512)
@@ -147,3 +150,63 @@ def state_dict(arena, buffers, prefix=''):
     for k in buffer_shapes():
         out[prefix + k] = own(buffers[k])
     return out
+
+
+def arena_from_state_dict(sd, out, prefix=''):
+    """The inverse of ``state_dict``: each of the 169 parameters ``sd[prefix + name]`` copied into its view of the flat arena
+    ``out`` (cast to fp32 as ``load_state_dict`` does; the arena's padding is not written).  Returns ``out``."""
+    lay = arena_layout()
+    if out.dim() != 1 or out.numel() != lay.floats or out.dtype != torch.float32:
+        raise ValueError(f'expected a flat fp32 arena of {lay.floats} floats, got {out.dtype} of shape {tuple(out.shape)}')
+    for n, v in zip(lay.names, lay.views(out)):
+        v.copy_(sd[prefix + n])
+    return out
+
+
+def read_checkpoint(path, buffers):
+    """A checkpoint in the reference's format (``{'model': {'module.<name>': tensor}}``: what ``export_model`` writes and
+    ``model_file`` names) read into a host arena and checked against the pool whose ``init_*`` buffers are ``buffers``.
+    Returns (the (P,) fp32 host arena, its digest).  The arena is zero outside the parameters, as the arena of a model loaded
+    with ``load_state_dict``.
+
+    Every check runs on the host and raises ValueError naming the file and the key: a file that is no readable checkpoint, a
+    missing or extra key (strict, as ``load_state_dict(strict=True)``), a shape other than ``param_shapes()`` /
+    ``buffer_shapes()``, a value that is not finite float data, ``init_*`` buffers that differ in any bit from ``buffers`` (the
+    grouped forward reads one buffer set for every video).  The digest is the sha256 of the arena's and the buffers' bytes:
+    two files with the same weights are one model, whatever their path, pickling or key order."""
+    try:
+        obj = torch.load(path, map_location='cpu', weights_only=True)
+    except Exception as e:                                     # missing, truncated, not a torch file, or a pickled object
+        raise ValueError(f'{path}: not a readable checkpoint: {type(e).__name__}: {e}') from None
+    sd = obj.get('model') if isinstance(obj, dict) else None
+    if not isinstance(sd, dict):
+        raise ValueError(f'{path}: not a checkpoint: expected a dict with a \'model\' state dict, got {type(obj).__name__}'
+                         + (f' with keys {sorted(map(str, obj))[:8]}' if isinstance(obj, dict) else ''))
+    want = OrderedDict(('module.' + k, s) for k, s in list(param_shapes().items()) + list(buffer_shapes().items()))
+    missing, extra = [k for k in want if k not in sd], sorted(str(k) for k in sd if k not in want)
+    if missing:
+        raise ValueError(f'{path}: missing key {missing[0]!r}' + (f' and {len(missing) - 1} more' if len(missing) > 1 else ''))
+    if extra:
+        raise ValueError(f'{path}: unexpected key {extra[0]!r}' + (f' and {len(extra) - 1} more' if len(extra) > 1 else ''))
+    for k, shp in want.items():
+        t = sd[k]
+        if not isinstance(t, torch.Tensor) or not t.is_floating_point():
+            raise ValueError(f'{path}: {k} is not float data ({type(t).__name__}{"" if not isinstance(t, torch.Tensor) else " " + str(t.dtype)})')
+        if tuple(t.shape) != tuple(shp):
+            raise ValueError(f'{path}: {k} has shape {tuple(t.shape)}, expected {tuple(shp)}')
+        if not bool(torch.isfinite(t).all()):
+            raise ValueError(f'{path}: {k} holds values that are not finite')
+    for k in buffer_shapes():
+        mine, pool = sd['module.' + k].float().contiguous(), buffers[k].detach().float().cpu().contiguous()
+        if not torch.equal(mine.view(torch.int32), pool.view(torch.int32)):
+            raise ValueError(f'{path}: module.{k} differs from the pool\'s {k}: every slot reads the pool\'s init_* buffers')
+    arena = arena_from_state_dict(sd, torch.zeros(arena_layout().floats, dtype=torch.float32), prefix='module.')
+    return arena, arena_digest(arena, buffers)
+
+
+def arena_digest(arena, buffers):
+    """sha256 of a flat arena's bytes and of the ``init_*`` buffers': the identity of a model (``read_checkpoint``)."""
+    h = hashlib.sha256(arena.detach().float().cpu().contiguous().numpy().tobytes())
+    for k in buffer_shapes():
+        h.update(buffers[k].detach().float().cpu().contiguous().numpy().tobytes())
+    return h.hexdigest()

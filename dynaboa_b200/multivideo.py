@@ -15,6 +15,7 @@ import math
 import numbers
 import os
 import random
+import sys
 from types import SimpleNamespace
 
 import numpy as np
@@ -102,6 +103,30 @@ def own_values(options, hparams):
     return {k: v for k, v in hparams.items() if v != getattr(options, k, None)}
 
 
+def check_models(models, n_videos):
+    """``run``'s ``models``: one checkpoint path (str or ``os.PathLike``) or None per video, None for the list: none.  Returns
+    them as a list of str / None (no device or file needed)."""
+    if models is None:
+        return [None] * n_videos
+    if isinstance(models, (str, bytes, os.PathLike)):
+        raise ValueError(f'models must hold one checkpoint path or None per video, not one path for all: {models!r}')
+    models = list(models)
+    if len(models) != n_videos:
+        raise ValueError(f'{len(models)} models for {n_videos} videos')
+    return [check_model(m, f'video {i}') for i, m in enumerate(models)]
+
+
+def check_model(model, who):
+    """A checkpoint path (str or ``os.PathLike``) as str, or None.  The str is interned, as ``state.unplain`` interns the
+    strings of a checkpoint's records: the summaries of a resumed run then pickle byte-identically to an uninterrupted run's."""
+    if model is None:
+        return None
+    path = os.fspath(model) if isinstance(model, os.PathLike) else model
+    if not isinstance(path, str) or not path:
+        raise ValueError(f'{who}: model must be a checkpoint path or None, got {model!r}')
+    return sys.intern(path)
+
+
 def video_names(videos, names, default):
     """The directory names of ``videos`` for ``run``: ``names`` as strings (None: ``default``), one per video."""
     names = list(default) if names is None else [str(x) for x in names]
@@ -141,6 +166,9 @@ class MultiVideoAdaptor:
     level until its own feature test passes or its own trip count exceeds ``optim_steps``.  Per slot, as ``Adaptor`` records
     them: ``optim_step_record[g]`` (one trip count per frame the slot advanced), ``feat_sims[g][frame]`` (the cosines of each
     test, ``frame`` counted from the slot's ``start``), and ``optimized_step`` ((G,), None for slots that sat the frame out).
+
+    ``start(g, model=path)`` starts slot g from a checkpoint of its own instead (``slot_model(g)``; DESIGN.md section 10,
+    "Per-slot checkpoints"): the pool keeps one device arena per distinct model its slots hold.
 
     ``fused_eval`` ('none', 'final' or 'all', as ``Adaptor``'s): evaluate every advancing video against its ground truth
     (batches then need pose, betas and gender).  Each evaluation stays on the device; ``records(g)`` forms slot g's host
@@ -185,6 +213,9 @@ class MultiVideoAdaptor:
         self.kp2dloss_lower_all, self.kp2dloss_upper_all = [[] for _ in range(G)], [{} for _ in range(G)]
         self._writer, self._pinned = state_mod.Writer(), state_mod.Pinned()     # checkpoints written in the background (save)
         self.hparams = [{} for _ in range(G)]   # per slot: the PER_VIDEO values it runs with where they differ from options
+        self.slot_models = [None] * G           # per slot: (path, digest) of its own checkpoint, None: options.model_file
+        self._store = {}                        # digest -> (P,) device arena of a model some slot holds
+        self._pool_digest = None                # digest of the pool's checkpoint (computed when a slot is given a model)
         self._step = Step(o, G, self.thetas, self.grad, self.buffers, base.smpl_neutral, base.gmm_f, teacher=self.teachers,
                           teacher_buffers=self.buffers, teacher_masks=self._teacher_masks, kp_range=self.kp_range,
                           motion_lead=self.motion_lead, bank=base.bank if o.retrieval else None, rngs=self.rngs,
@@ -197,7 +228,7 @@ class MultiVideoAdaptor:
         from .adaptor import Adaptor
         return Adaptor(options)
 
-    def start(self, g, seed=None, state=None, hparams=None):
+    def start(self, g, seed=None, state=None, hparams=None, model=None):
         """Put a new video into slot g: theta and teacher from the checkpoint, zero Adam moments, step and frame counts, an empty
         history, empty records, and ``rngs[g] = random.Random(seed)`` (default ``options.seed * 1000 + g``).  The records of
         the frames adapted so far are formed on the host first (one synchronisation, if any are pending).
@@ -205,11 +236,21 @@ class MultiVideoAdaptor:
         ``hparams``: a dict from keys of ``PER_VIDEO`` to values (``check_hparams``): slot g runs with ``options`` plus these
         values until its next ``start`` (``slot_options(g)``).
 
+        ``model``: a checkpoint path (``layout.read_checkpoint``; what ``export_model`` writes): slot g starts from it instead of
+        ``options.model_file`` and keeps it until its next ``start`` (``slot_model(g)``; the webcam pool's ``reload`` and base
+        outputs go back to it).  A checkpoint with the pool's weights is the pool's checkpoint.
+
         ``state``: a video state written by ``save_slot`` (its path, or the dict ``state.read_video`` returned) of a pool with
         the same G and compatible options, from any slot: slot g continues that video instead -- theta, teacher, moments, step
         count, ``video_steps[g]``, history ring, ``rngs[g]``, records and its hparams (``hparams`` that contradict them raise).
-        Everything is checked before any device work (ValueError)."""
+        A state of a slot on a checkpoint of its own needs that model again: ``model`` (default the path the state records)
+        must hold the same weights.  Everything is checked before any device work (ValueError)."""
+        self._start(g, seed, state, hparams, model)
+
+    def _start(self, g, seed=None, state=None, hparams=None, model=None, expect=None):
+        """``start``; ``expect``: the digest the checkpoint ``model`` had when ``run`` read it."""
         self._check_slot(g)
+        model = check_model(model, f'slot {g}')
         if state is not None and not isinstance(state, dict):
             state = state_mod.read_video(state, self.options, 'slot', self.G, own=PER_VIDEO)
         hp = None if hparams is None else own_values(self.options, check_hparams(self.options, hparams))
@@ -218,6 +259,14 @@ class MultiVideoAdaptor:
             if hp is not None and hp != saved:
                 raise ValueError(f'slot {g}: hparams {hparams!r} contradict the state\'s {saved!r}')
             hp = saved
+        want = None if state is None else state_mod.saved_model(state)
+        if model is None and want is not None:
+            model = want[0]                                  # the checkpoint the state was adapted from, where it was
+        own = self._read_model(model, expect) if model is not None else None
+        if state is not None and own is not None and own[1] != (want[1] if want is not None else self._pool_model_digest()):
+            raise ValueError(f'slot {g}: model {model!r} (digest {own[1][:12]}...) is not the checkpoint the state was adapted from: '
+                             + (f'{want[0]!r} (digest {want[1][:12]}...)' if want is not None else 'the pool\'s'))
+        self._set_model(g, own)
         self._reset_weights(g)
         self._form_records()
         self.video_steps[g] = 0
@@ -233,6 +282,43 @@ class MultiVideoAdaptor:
         if state is not None:
             self._restore_slot(g, state)
 
+    def slot_model(self, g):
+        """(path, digest) of slot g's own checkpoint (``start(g, model=...)``), or None when it is on the pool's."""
+        self._check_slot(g)
+        return self.slot_models[g]
+
+    def _pool_model_digest(self):
+        if self._pool_digest is None:
+            self._pool_digest = layout.arena_digest(self.base.model.module.arena, self.buffers)
+        return self._pool_digest
+
+    def _read_model(self, path, expect=None):
+        """(path, digest, host arena) of the checkpoint at ``path``, read and checked on the host; the arena is None when the
+        checkpoint holds the pool's weights.  ``expect``: the digest the file must still have (ValueError otherwise)."""
+        arena, digest = layout.read_checkpoint(path, self.buffers)
+        if expect is not None and digest != expect:
+            raise ValueError(f'{path}: the checkpoint changed since it was read (digest {digest[:12]}..., was {expect[:12]}...)')
+        return path, digest, None if digest == self._pool_model_digest() else arena
+
+    def _set_model(self, g, own):
+        """Slot g on the model ``own`` (``_read_model``'s triple; None or a None arena: the pool's checkpoint): its arena
+        uploaded unless a slot already holds it, and the arenas no slot refers to any more freed."""
+        self.slot_models[g] = None if own is None or own[2] is None else (own[0], own[1])
+        held = {m[1] for m in self.slot_models if m is not None}
+        for d in [d for d in self._store if d not in held]:
+            del self._store[d]
+        if self.slot_models[g] is not None and own[1] not in self._store:
+            self._store[own[1]] = own[2].to(self.thetas.device)
+        self._slot_model_set(g)
+
+    def _slot_model_set(self, g):
+        """Called once slot g's model is set (the webcam pool keeps its base-output arenas here)."""
+
+    def _model_arena(self, g):
+        """The device arena slot g starts from: its own model's, or the pool's checkpoint."""
+        m = self.slot_models[g]
+        return self.base.model.module.arena if m is None else self._store[m[1]]
+
     def slot_options(self, g):
         """Slot g's effective options: the pool's ``options`` with the slot's hparams."""
         self._check_slot(g)
@@ -243,11 +329,13 @@ class MultiVideoAdaptor:
             raise ValueError(f'slot {g!r} is not one of the {self.G} slots')
 
     def _reset_weights(self, g):
-        """Slot g's theta and teacher back to the checkpoint and a fresh Adam (zero moments, step count 0)."""
+        """Slot g's theta and teacher back to its checkpoint (``slot_model(g)``, else the pool's) and a fresh Adam (zero
+        moments, step count 0)."""
         self._check_slot(g)
-        self.thetas[g].copy_(self.base.model.module.arena.detach())
+        own = self.slot_models[g] is not None
+        self.thetas[g].copy_(self._model_arena(g).detach())
         if self.teachers is not None:
-            self.teachers[g].copy_(self.base.teacher.arena.detach())
+            self.teachers[g].copy_(self._model_arena(g) if own else self.base.teacher.arena.detach())
         self.m[g].zero_()
         self.v[g].zero_()
         self.step_counts[g] = 0
@@ -448,7 +536,7 @@ class MultiVideoAdaptor:
                     feat_sims=dict(self.feat_sims[g]), optim_step_record=list(self.optim_step_record[g]),
                     kp2dlosses_lower=list(self.kp2dloss_lower_all[g]), kp2dlosses_upper=dict(self.kp2dloss_upper_all[g]))
 
-    def run(self, videos, exppath=None, names=None, checkpoint=None, every=0, hparams=None):
+    def run(self, videos, exppath=None, names=None, checkpoint=None, every=0, hparams=None, models=None):
         """Adapt every video of ``videos`` (a list of iterables of batch dicts with batch size 1: a ``DataLoader`` over a
         sequence, a ``SyntheticStream``) through the G slots.  Slots are filled in order and refilled from the queue as soon as
         their video ends; video i starts with ``start(g, seed=options.seed * 1000 + i)``, so its seed follows the video, and
@@ -463,25 +551,34 @@ class MultiVideoAdaptor:
         from there.  The summaries and result files are those of a run that was never interrupted.
 
         ``hparams``: one dict of ``start``'s hparams, or None, per video; the dict follows the video into its slot, as its seed
-        does.  A resumed run must be given the hparams of the run it continues."""
+        does.  A resumed run must be given the hparams of the run it continues.
+
+        ``models``: one checkpoint path, or None for ``options.model_file``, per video; the model follows the video into its slot
+        (``start(g, model=...)``) and each summary names it (``model``).  Every distinct path is read and checked once before the
+        first tick; a resumed run must be given checkpoints with the weights of the run it continues."""
         from .adaptor import write_records
         videos = list(videos)
         hparams = check_hparams(self.options, hparams, len(videos))
+        models = None if models is None else check_models(models, len(videos))
         names = video_names(videos, names, default=[str(i) for i in range(len(videos))])
         mean = lambda v: float(np.mean(v)) if len(v) else float('nan')
 
         def finish(i, g):
             if g is None:                                    # an empty video
-                return dict(name=names[i], frames=0, mpjpe=float('nan'), pampjpe=float('nan'), pve=float('nan'))
-            rec = self.records(g)
-            if exppath is not None:
-                d = os.path.join(exppath, names[i])
-                os.makedirs(d, exist_ok=True)
-                write_records(d, rec['frames'] - 1, rec)
-            return dict(name=names[i], frames=rec['frames'], mpjpe=mean(rec['mpjpe']), pampjpe=mean(rec['pampjpe']), pve=mean(rec['pve']))
-        return self._queue(videos, self.adapt, finish, checkpoint=checkpoint, every=every, hparams=hparams)
+                out = dict(name=names[i], frames=0, mpjpe=float('nan'), pampjpe=float('nan'), pve=float('nan'))
+            else:
+                rec = self.records(g)
+                if exppath is not None:
+                    d = os.path.join(exppath, names[i])
+                    os.makedirs(d, exist_ok=True)
+                    write_records(d, rec['frames'] - 1, rec)
+                out = dict(name=names[i], frames=rec['frames'], mpjpe=mean(rec['mpjpe']), pampjpe=mean(rec['pampjpe']), pve=mean(rec['pve']))
+            if models is not None:
+                out['model'] = models[i]
+            return out
+        return self._queue(videos, self.adapt, finish, checkpoint=checkpoint, every=every, hparams=hparams, models=models)
 
-    def _queue(self, videos, tick, finish, checkpoint=None, every=0, items_from=None, barrier=None, hparams=None):
+    def _queue(self, videos, tick, finish, checkpoint=None, every=0, items_from=None, barrier=None, hparams=None, models=None):
         """``run``'s queue: the slots are filled in order and refilled as soon as their video ends; video i starts with
         ``start(g, seed=options.seed * 1000 + i)`` and ``slot_video[g] = i``.  ``tick(items)`` advances the pool by one frame,
         ``items[g]`` being slot g's next item of its video (None: an idle slot); ``finish(i, g)`` returns video i's summary once
@@ -489,10 +586,15 @@ class MultiVideoAdaptor:
 
         ``checkpoint`` / ``every``: ``run``'s.  ``items_from(i, k)``: an iterator over video i's items from item k on (default
         ``items_from``); ``barrier()``: futures of files a checkpoint taken now covers (``save``); ``hparams``: video i's
-        ``start`` hparams (checked; None: none)."""
+        ``start`` hparams (checked; None: none); ``models``: video i's checkpoint path (None: the pool's), each distinct one read and
+        checked here, before the first tick, with only its digest kept."""
         n = len(videos)
         hparams = check_hparams(self.options, hparams, n)
         own = [own_values(self.options, h) for h in hparams]
+        paths = check_models(models, n)
+        digests = {p: self._read_model(p)[1] for p in dict.fromkeys(p for p in paths if p is not None)}
+        # per video: (path, digest) of its own checkpoint, None on the pool's (a checkpoint with the pool's weights is the pool's)
+        own_models = [None if p is None or digests[p] == self._pool_model_digest() else (p, digests[p]) for p in paths]
         queue, its, nxt, out = list(range(n)), [None] * self.G, [None] * self.G, [None] * n
         items_from = items_from or (lambda i, k: _items_from(videos[i], k))
 
@@ -503,7 +605,11 @@ class MultiVideoAdaptor:
                 raise ValueError(f'{checkpoint}: the checkpoint is of a queue of {run["videos"]} videos, not {n}')
             if run.get('hparams', [{}] * n) != own:
                 raise ValueError(f'{checkpoint}: the checkpoint is of a run with hparams {run.get("hparams")!r}, not {own!r}')
-        run = self.load(checkpoint, check_run) if checkpoint is not None else None
+            saved = [None if m is None else m[1] for m in run.get('models', [None] * n)]
+            if saved != [None if m is None else m[1] for m in own_models]:
+                raise ValueError(f'{checkpoint}: the checkpoint is of a run with models {run.get("models")!r}, whose weights differ from '
+                                 f'{[None if m is None else m[0] for m in own_models]!r}')
+        run = self.load(checkpoint, check_run, models=paths) if checkpoint is not None else None
         if run is not None:
             queue, out = list(run['queue']), list(run['out'])
             for g in range(self.G):
@@ -512,7 +618,10 @@ class MultiVideoAdaptor:
                     nxt[g] = next(its[g], None)
 
         def save():
-            self.save(checkpoint, run=dict(videos=n, queue=queue, out=out, hparams=own), barrier=barrier, wait=False)
+            rec = dict(videos=n, queue=queue, out=out, hparams=own)
+            if any(m is not None for m in own_models):
+                rec['models'] = own_models
+            self.save(checkpoint, run=rec, barrier=barrier, wait=False)
 
         def fill(g):
             self.slot_video[g] = None
@@ -523,7 +632,7 @@ class MultiVideoAdaptor:
                 if nxt[g] is None:
                     out[i] = finish(i, None)
                     continue
-                self.start(g, seed=self.options.seed * 1000 + i, hparams=hparams[i])
+                self._start(g, seed=self.options.seed * 1000 + i, hparams=hparams[i], model=paths[i], expect=digests.get(paths[i]))
                 self.slot_video[g] = i
                 return
 
@@ -562,7 +671,7 @@ class MultiVideoAdaptor:
         return state_mod.video_state(self.slot_options(g), 'slot', G, copy(('theta', g), self.thetas[g]),
                                      None if self.teachers is None else copy(('teacher', g), self.teachers[g]),
                                      copy(('m', g), self.m[g]), copy(('v', g), self.v[g]), self.step_counts[g], self.video_steps[g], hist,
-                                     dict(random=self.rngs[g].getstate()), records)
+                                     dict(random=self.rngs[g].getstate()), records, model=self.slot_models[g])
 
     def _restore_slot(self, g, st):
         G, dev = self.G, self.thetas.device
@@ -629,12 +738,13 @@ class MultiVideoAdaptor:
         if wait:
             self._writer.wait()
 
-    def load(self, root, check_run=None):
+    def load(self, root, check_run=None, models=None):
         """Continue from the newest complete checkpoint ``save`` wrote under ``root``: every file is checked first (ValueError),
         then the saved slots are restored with ``start(g, state=...)``, the others marked empty in ``slot_video``, and
         ``global_step`` and torch's CUDA generator set.  Returns the checkpoint's ``run`` (None without a checkpoint).
         ``check_run(run)``: raises for a ``run`` the caller cannot continue, after the files are checked and before anything is
-        restored."""
+        restored.  ``models``: per video of the run, the checkpoint path its slot is restored with (None: the path its state
+        records, if any)."""
         found = state_mod.latest(root)
         if found is None:
             return None
@@ -650,7 +760,7 @@ class MultiVideoAdaptor:
         for g in range(self.G):
             self.slot_video[g] = pool['slot_video'][g] if g in states else None
             if g in states:
-                self.start(g, state=states[g])
+                self.start(g, state=states[g], model=None if models is None else models[self.slot_video[g]])
         self.global_step = pool['global_step']
         torch.cuda.set_rng_state(pool['cuda_rng'], self.thetas.device)
         torch.cuda.synchronize(self.thetas.device)

@@ -1,7 +1,8 @@
 """Saved adaptation state: the one module that knows the file layout (DESIGN.md section 11).
 
 A *video state* is one ``torch.save`` file holding everything one video's adaptation continues from: its theta, teacher, Adam
-moments and step count, its frame count, its history ring, its retrieval generator and its records.  ``Adaptor.save_state`` /
+moments and step count, its frame count, its history ring, its retrieval generator and its records, and, for a pool slot
+started from a checkpoint of its own, that checkpoint's path and digest (``model``).  ``Adaptor.save_state`` /
 ``load_state`` and the pools' ``save_slot`` / ``start(g, state=...)`` write and read them through ``video_state`` /
 ``read_video``.  A *pool checkpoint* is a directory of numbered checkpoints, each one video state per occupied slot, one pool
 file and a manifest written last: ``latest`` returns the newest checkpoint whose manifest is complete.
@@ -163,14 +164,17 @@ def read(path, fmt, options=None, own=frozenset()):
 
 
 # ------------------------------------------------------------------ video states
-def video_state(options, kind, G, theta, teacher, m, v, step_count, frames, history, rng, records):
+def video_state(options, kind, G, theta, teacher, m, v, step_count, frames, history, rng, records, model=None):
     """A video state as a dict of host tensors and plain containers.  ``kind``: 'adaptor' (``Adaptor``) or 'slot' (a pool slot
     of a G-slot pool); ``theta``, ``teacher`` (None without one), ``m``, ``v``: (P,) arenas; ``frames``: the video's frame count;
-    ``history``: {frame: (image, keypoints)}; ``rng``: generator states; ``records``: the adaptor's records of the video."""
+    ``history``: {frame: (image, keypoints)}; ``rng``: generator states; ``records``: the adaptor's records of the video.
+    ``model``: (path, digest) of the slot's own checkpoint, kept as the ``model`` entry; None (no entry): the pool's."""
     out = header(VIDEO, options)
     out.update(kind=kind, G=int(G), theta=plain(theta), teacher=None if teacher is None else plain(teacher), m=plain(m), v=plain(v),
                step_count=int(step_count), frames=int(frames), history={int(k): (plain(a), plain(b)) for k, a, b in history},
                rng=plain(rng), records=plain(records))
+    if model is not None:
+        out['model'] = {'path': str(model[0]), 'digest': str(model[1])}
     return out
 
 
@@ -195,9 +199,23 @@ def read_video(path, options, kind, G=1, own=frozenset()):
             raise ValueError(f'{path}: malformed video state: {k} is not a ({P},) float32 tensor')
     if (st['teacher'] is None) != (not getattr(options, 'use_meanteacher', 0)):
         raise ValueError(f'{path}: malformed video state: teacher does not match use_meanteacher')
+    saved_model(st, path)
     st['records'] = unplain(st['records'])
     st['rng'] = unplain(st['rng'])
     return st
+
+
+def saved_model(st, where='state'):
+    """(path, digest) of the slot's own checkpoint a video state ``st`` records, or None for the pool's (no ``model`` entry, or
+    None).  ValueError for a malformed entry (``where`` names the file)."""
+    m = st.get('model')
+    if m is None:
+        return None
+    if (not isinstance(m, dict) or set(m) != {'path', 'digest'} or not isinstance(m['path'], str) or not isinstance(m['digest'], str)
+            or not re.fullmatch(r'[0-9a-f]{64}', m['digest'])):
+        raise ValueError(f'{where}: malformed video state: the model entry must be None or {{path, digest}} with a sha256 digest, '
+                         f'got {m!r}')
+    return m['path'], m['digest']
 
 
 def saved_options(st, keys):

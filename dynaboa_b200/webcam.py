@@ -136,12 +136,13 @@ class MultiWebcamAdaptor(MultiVideoAdaptor):
     the host, one grouped crop and one grouped keypoint call into the pool's staging rows, the bilevel step, one masked output
     forward.  ``adapt_processed`` does the same on already cropped rows.  ``render(frames, results)`` draws the tick's meshes
     in one grouped overlay call.  ``reload(g)`` is the demo's key ``r`` for stream g; ``start(g)`` puts a new camera into slot
-    g.  Per slot, ``video_steps[g]`` counts the stream's frames."""
+    g (``start(g, model=path)``: from a checkpoint of its own, which ``reload`` and the base outputs then use).  Per slot, ``video_steps[g]`` counts the stream's frames."""
     colors = ((205, 129, 98), (100, 100, 200))             # adapted and base mesh (reference dynaboa_webcam.py:410,416)
     kp_range = (0, 25)
     motion_lead = 1
 
     def __init__(self, options, n_streams, dynamic_loop=False):
+        self._base_stack = None              # (G, P) base arenas of the streams, while one holds a model of its own (test_basemodel)
         super().__init__(webcam_options(options), n_streams, dynamic_loop)
         self.fused_eval = 'none'
 
@@ -155,9 +156,21 @@ class MultiWebcamAdaptor(MultiVideoAdaptor):
             self._frames = {'image': torch.zeros(self.G, 3, 224, 224, device=dev), 'smpl_j2d': torch.zeros(self.G, 49, 3, device=dev)}
         return self._frames
 
+    def _slot_model_set(self, g):
+        """With ``test_basemodel``: the (G, P) stack of base arenas the tick's base outputs read while any stream holds a model
+        of its own, allocated when the first one does (every row filled) and freed when none does; otherwise row g is filled."""
+        if not self.options.test_basemodel:
+            return
+        if all(m is None for m in self.slot_models):
+            self._base_stack = None
+        elif self._base_stack is None:
+            self._base_stack = torch.stack([self._model_arena(h) for h in range(self.G)])
+        else:
+            self._base_stack[g].copy_(self._model_arena(g))
+
     def reload(self, g):
-        """Key ``r`` of the demo for stream g (reference dynaboa_webcam.py:184-194): theta and teacher back to the checkpoint and
-        a fresh Adam (zero moments, step count 0).  The stream's history, frame count and hparams (``start(g, hparams=...)``) are
+        """Key ``r`` of the demo for stream g (reference dynaboa_webcam.py:184-194): theta and teacher back to the stream's
+        checkpoint (``slot_model(g)``, else the pool's) and a fresh Adam (zero moments, step count 0).  The stream's history, frame count and hparams (``start(g, hparams=...)``) are
         kept, so its motion term stays as it was; the other streams are left alone."""
         self._reset_weights(g)
 
@@ -229,15 +242,19 @@ class MultiWebcamAdaptor(MultiVideoAdaptor):
         return self._tick(on, [None] * G if bboxes is None else bboxes)
 
     def _tick(self, on, bboxes):
-        """The pool step on the staged rows, then one masked forward of the adapted weights (and, with ``test_basemodel``, one
-        forward of the checkpoint arena the base adaptor holds) and the result dictionaries."""
+        """The pool step on the staged rows, then one masked forward of the adapted weights and the result dictionaries.  With
+        ``test_basemodel``, the base outputs: one forward of the checkpoint arena the base adaptor holds while no active stream
+        holds a model of its own, else one grouped forward of the active streams over the stack of base arenas."""
         rows = self._frames
         self._adapt_staged(on, rows)
         preds = self.predict(rows['image'], on)
         base = None
         if self.options.test_basemodel:
             with torch.no_grad():
-                rot, shape, cam, _, _ = hmr_mod.raw_forward(self.base.model.module.arena, self.buffers, rows['image'])
+                if any(self.slot_models[g] is not None for g in self._slots(on)):
+                    rot, shape, cam, _, _ = hmr_mod.raw_forward(self._base_stack, self.buffers, rows['image'], groups=self.G, active=on)
+                else:
+                    rot, shape, cam, _, _ = hmr_mod.raw_forward(self.base.model.module.arena, self.buffers, rows['image'])
                 base = (self.base.decode_smpl_params(rot, shape)['vts'], cam)
         out = []
         for g, p in enumerate(preds):
